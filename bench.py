@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""bench.py - learner sequence-steps/sec (batch x seq_len per learner iteration) of the B200-native learner hot
-path.  Headline workload = BASELINE.json configs[2], the largest single-GPU configuration: synthetic Humanoid
+"""bench.py - learner sequence-steps/sec (batch x seq_len per learner iteration) of the GPU-native (H100, sm_90a)
+learner hot path.  Headline workload = BASELINE.json configs[2], the largest single-GPU configuration: synthetic Humanoid
 shape obs=376 act=17 hidden=512 seq_len=80 burn_in=40 batch=512 PER GPU (weak scaling: every rank owns a replay
 shard in HBM and a batch of 512; the two flat gradient blocks are all-reduced over NCCL at the optimiser steps).
 
@@ -8,6 +8,7 @@ shard in HBM and a batch of 512; the two flat gradient blocks are all-reduced ov
   python bench.py --impl reference ...                   # the reference's CPU implementation (oracle port)
   python bench.py --config cfg2|cfg1                     # BASELINE.json configs[1] / configs[0] shapes
   python bench.py --config replay                        # configs[3]: 250k stored sequence starts per GPU, sample / update
+  python bench.py --dump-outputs DIR ...                 # also write what the last timed step computed as DIR/<name>.npy
 
 A step = one pass of learner.py:84-139: prioritized sample from the HBM replay shard -> gather -> target/online
 chains -> TD/priority kernels -> critic BPTT + Adam -> actor chain -> DPG backward + Adam -> priority write-back into
@@ -53,16 +54,13 @@ def lstm_flops_per_iteration(c):
 
 
 def measured_peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.isfile(path):
-        d = json.load(open(path))
-        return {"bf16_burst": d["bf16_tflops"], "bf16_sustained": d["bf16_tflops_sustained"], "hbm": d["hbm_gbs"],
-                "source": "measured"}
-    return {"bf16_burst": 1590.0, "bf16_sustained": 1400.0, "hbm": 6650.0, "source": "fallback"}
+    """Denominators of the roofline fractions: NVIDIA's H100 SXM data sheet (dense BF16, HBM3), a 700 W card.  A card
+    with a lower power limit clocks lower under sustained load, so these are upper bounds, not reached rates."""
+    return {"bf16_burst": 989.0, "bf16_sustained": 989.0, "hbm": 3350.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling DURING the timed region: SM clock, power and throttle reasons next to the number."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -145,12 +143,13 @@ def pick_cpu_threads(name, c):
     """Thread count of the CPU arms.  torch CPU ops of this size stop scaling - and can collapse - long before a
     100+ core box is full, so FULL-BATCH port iterations (all phases: sample, chains, BPTT, Adam; a shortened window
     so that a probe iteration costs ~1/10 of a real one) are timed for a few candidates and the fastest is kept.  The
-    choice is cached per (CPU model, core count, config) in /tmp so that `--impl reference` and the `cpu_baseline` leg
-    of the B200 arm, which run back to back on one box, use the same setting (round 1: a 12-step LSTMCell probe flipped
-    between 16 and 32 threads from run to run and moved the reference arm by 2.8x)."""
+    choice is cached per (CPU model, core count, config) in the temporary directory so that `--impl reference` and the
+    `cpu_baseline` leg of the GPU arm, which run back to back on one host, use the same setting (a 12-step LSTMCell
+    probe flipped between 16 and 32 threads from run to run and moved the reference arm by 2.8x)."""
     ncpu = os.cpu_count() or 1
     key = f"{cpu_model()}|{ncpu}|{name}"
-    cache_path = "/tmp/r2d2_b200_cpu_threads.json"
+    import tempfile
+    cache_path = os.path.join(tempfile.gettempdir(), "r2d2_b200_cpu_threads.json")
     try:
         cache = json.load(open(cache_path))
     except Exception:
@@ -221,8 +220,8 @@ def run_reference(args, name, c):
             "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload_string(name, c),
-                       "note": "reference CPU learner (oracle/ref_port.py port; /root/reference is python and not "
-                               "present on this box), full batch and full window per step; a step is one learner "
+                       "note": "reference CPU learner (oracle/ref_port.py port of the python reference), "
+                               "full batch and full window per step; a step is one learner "
                                "iteration (seconds on the host): at most 200 s of them are timed (steps_timed, median), "
                                "the rate does not depend on the count"},
             "cpu_baseline": {"value": value, "unit": "seq-steps/s", "cores": threads, "kind": "port",
@@ -416,22 +415,13 @@ def scan_roofline(nv, c, dev, peaks, ms_iter):
         out[name] = ev0.elapsed_time(ev1) / reps
     scan_flops = 2.0 * B * H * 4 * H * S
     achieved = scan_flops / (out["fwd"] * 1e-3) / 1e12
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r02_scan_fwd_traffic.json")
-    if os.path.isfile(tpath):
-        try:
-            traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
-    kname = ("lstm_scan_fwd_big_kernel (H=512: cluster of 16, 7 resident clusters x <=80 rows as two ping-pong sub-tiles, "
-             "W_hh in TMEM + smem tail, h_t all-gather through L2 multicast)") if H == 512 else \
-        "lstm_scan_fwd_pp_kernel (persistent cluster LSTM scan, tcgen05 ping-pong over two row sub-tiles, W_hh in TMEM)"
+    kname = ("lstm_scan_fwd_kernel (persistent cluster LSTM scan, cluster of 16, W_hh lo plane in registers and hi plane "
+             "in shared memory, mma.sync, h_t all-gather through DSMEM)") if H == 512 else \
+        "lstm_scan_fwd_kernel (persistent cluster LSTM scan, W_hh in registers, mma.sync, h_t all-gather through DSMEM)"
     flops_it = lstm_flops_per_iteration(c)
     return {"kernel": kname + f", {S} cell steps", "bound": "tensor", "achieved": achieved, "peak": peaks["bf16_burst"],
-            "unit": "TFLOP/s", "frac": achieved / peaks["bf16_burst"], "traffic": traffic,
-            "traffic_source": "profiles/r02_scan_fwd_traffic.json (ncu --set full of this kernel, dram read + write per launch)"
-            if traffic else None,
-            "peak_source": peaks["source"] + " bf16 dense burst (kernel timed alone)",
+            "unit": "TFLOP/s", "frac": achieved / peaks["bf16_burst"], "traffic": None,
+            "peak_source": peaks["source"] + " bf16 dense (kernel timed alone)",
             "us_per_step": out["fwd"] * 1e3 / S,
             "bptt_kernel": {"us_per_step": out["bwd"] * 1e3 / S,
                             "achieved_tflops": scan_flops / (out["bwd"] * 1e-3) / 1e12,
@@ -471,7 +461,7 @@ def run_replay_bench(args, engine, dev, world, rank, dist, barrier):
     gen = torch.Generator(device=dev).manual_seed(rank)
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     B = cfg.batch
-    steps, warm = max(args.steps, 50), max(args.warmup, 5)
+    steps, warm = args.steps, args.warmup
     for _ in range(warm):
         rp.sample_into(eng, generator=gen)
     barrier()
@@ -532,6 +522,23 @@ def run_replay_bench(args, engine, dev, world, rank, dist, barrier):
               "gpu_launches": 3 * steps})
 
 
+def dump_outputs(eng, out_dir):
+    """What a caller of the timed step receives after the last timed step: Q values, TD targets, the priorities written
+    back to the tree, the two losses and the updated actor / critic parameters.  The inputs are seeded (replay content,
+    sampler generator, initial weights) and the library adds partial sums in a fixed order, so two runs with the same
+    arguments write the same arrays and two builds can be compared array by array."""
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"q_value": eng.q_value, "target_q_value": eng.target_q_value, "priority": eng.priority,
+              "losses": eng.losses}
+    for net in ("actor", "critic"):
+        for k, v in eng.views(net).items():
+            arrays[f"{net}.{k}"] = v
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), v.detach().float().cpu().numpy())
+    log(f"wrote {len(arrays)} arrays to {out_dir}")
+
+
 def main():
     _claim_stdout()
     ap = argparse.ArgumentParser()
@@ -544,7 +551,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary configs / strong-scaling legs (profiling runs)")
     ap.add_argument("--cpu-steps", type=int, default=4)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.config == "replay"):
+        ap.error("--dump-outputs writes what the GPU learner step computed: it does not apply to --impl reference "
+                 "or --config replay")
     if args.warmup < 3:
         args.warmup = 3
     name = args.config if args.config != "replay" else "cfg3"
@@ -588,6 +600,8 @@ def main():
     log("HBM-resident arm")
     ms = arm.time_resident(args.steps, args.warmup, barrier, clocks)
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(arm.eng, args.dump_outputs)
 
     def max_over_ranks(x):
         t = torch.tensor([x], device=dev)

@@ -1,4 +1,4 @@
-/* libr2d2_b200 - C ABI of the B200-native learner hot path of pytorch-r2d2-DPG.
+/* libr2d2_b200 - C ABI of the GPU-native (H100, sm_90a) learner hot path of pytorch-r2d2-DPG.
  *
  * The reference (pure Python) has no FFI; its boundary for this path is the module surface
  * learner.py / replay_memory.py / models.py / utils.py.  Each entry point below replaces the
@@ -35,7 +35,7 @@ extern "C" {
 typedef void* r2d2_stream_t; /* cudaStream_t */
 
 int r2d2_version(void);                /* 100 * major + minor */
-const char* r2d2_arch(void);           /* "sm_100a" */
+const char* r2d2_arch(void);           /* "sm_90a" */
 const char* r2d2_last_error(void);
 int r2d2_device_sm_count(int* out);
 
@@ -81,34 +81,26 @@ int r2d2_lstm_net_backward(const r2d2_net_shape* shape, const float* params, con
 
 /* The serial scan alone (the persistent-RNN kernel; bench.py times it for the roofline line):
  * gin [T,B,4H] pre-activation input projection, whh [4H,H], h0/c0 [B,H] or NULL; outputs gates [T*repeat,B,4H]
- * (may alias gin when repeat == 1), hs/cs [T*repeat+1,B,H], head_in [T,B,H] or NULL.  scratch: NULL for
- * H in {32,64,128,256}, else [B,4H] floats. */
+ * (may alias gin when repeat == 1), hs/cs [T*repeat+1,B,H], head_in [T,B,H] or NULL.  scratch: [B,4H] floats
+ * (used by the per-step path; NULL is accepted when the cluster kernels cover H and are selected). */
 int r2d2_lstm_scan_forward(const float* gin, const float* whh, const float* h0, const float* c0, float* gates,
                            float* hs, float* cs, float* head_in, int T, int B, int H, int repeat, float* scratch,
                            r2d2_stream_t stream);
 /* BPTT twin: dgates [S,B,4H] (may alias gates), dgin [T,B,4H] (only when repeat > 1), dh_head [*,B,H] or NULL
- * consumed from step head_first_step on.  scratch: NULL for the cluster sizes, else [2,B,H]. */
+ * consumed from step head_first_step on.  scratch: [2,B,H] (NULL as for the forward scan). */
 int r2d2_lstm_scan_backward(const float* gates, const float* hs, const float* cs, const float* whh,
                             const float* dh_head, int head_first_step, float* dgates, float* dgin, int T, int B,
                             int H, int repeat, float* scratch, r2d2_stream_t stream);
 
-/* debug: forward scan that also records per-step globaltimer stamps [grid][S][8] (thread 0 of every CTA) */
-int r2d2_debug_scan_forward_trace(const float* gin, const float* whh, float* gates, float* hs, float* cs, int T, int B,
-                                  int H, long long* trace, r2d2_stream_t stream);
-/* debug: BPTT scan (H = 512 kernel) that also records per-step globaltimer stamps [grid][S][8] */
-int r2d2_debug_scan_backward_trace(const float* gates, const float* hs, const float* cs, const float* whh,
-                                   const float* dh_head, float* dgates, int T, int B, int H, long long* trace,
-                                   r2d2_stream_t stream);
-/* debug: clusters of the tcgen05 scan kernel the device can keep resident at once (-1 if not instantiated) */
-int r2d2_debug_max_active_clusters(int H, int nb, int backward);
-/* GEMM implementation switch for A/B checks: 1 = tcgen05/TMEM with skinny problems (K<64, N<32 or M<32) on the
- * single-launch mma.sync kernel (default), 2 = tcgen05 for every shape, 0 = mma.sync v1 kernel only */
+/* GEMM implementation switch for A/B checks: 1 = wgmma with skinny problems (K<64, N<32 or M<32) on the fp32
+ * streaming / single-launch mma.sync kernels (default), 2 = wgmma for every shape, 0 = mma.sync kernel only */
 int r2d2_set_gemm_impl(int impl);
 int r2d2_get_gemm_impl(void);
-/* scan implementation switch for A/B checks: 1 = tcgen05/TMEM (default), 0 = mma.sync v1 kernels */
+/* scan implementation switch for A/B checks: 1 = persistent cluster kernels where they cover H (default),
+ * 0 = per-step path (one GEMM + one cell kernel per step) for every H */
 int r2d2_set_scan_impl(int impl);
 int r2d2_get_scan_impl(void);
-/* *status != 0 if a bounded mbarrier wait inside a tcgen05 scan kernel ever timed out; synchronises the stream */
+/* *status != 0 if a scan kernel reported a protocol error; synchronises the stream */
 int r2d2_scan_status(int* status, r2d2_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------

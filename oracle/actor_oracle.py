@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE (checker only; never imported by the product path).
 
 numpy float64 restatement of the actor-side n-step reward pre-sum and initial priorities
-(/root/reference/actor.py:74-76 `calc_nstep_reward`, :78-107 `calc_priorities`), pinned against
+(reference actor.py:74-76 `calc_nstep_reward`, :78-107 `calc_priorities`), pinned against
 tests/golden/ref_actor_prio.npz (produced by the UNMODIFIED reference, oracle/make_golden.py).
 
 What the reference does, per finished episode of E real rows + n pad rows (actor.py:173):

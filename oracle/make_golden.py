@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.npz by executing the UNMODIFIED reference (/root/reference) on CPU.
+"""Generate tests/golden/*.npz by executing the UNMODIFIED reference (R2D2_REFERENCE_DIR) on CPU.
 
-Run in the build container only (the reference is not present on the GPU box):
+Run where a checkout of the reference is available (it is not part of this repository):
     python oracle/make_golden.py
 The fixtures pin the oracles (oracle/ref_port.py, oracle/learner_oracle.py) and, through them,
 the CUDA path.  torch version used is recorded in each file (the reference pins none).
@@ -37,6 +37,31 @@ from oracle import ref_harness, ref_port  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
 NETS = ("actor", "critic")
+PART_BYTES = 800_000   # raw bytes per stored file: every fixture file stays under 1 MB
+
+
+def save_golden(path, d):
+    """np.savez_compressed, split into <stem>.partN.npz files of at most PART_BYTES raw bytes each when the fixture is
+    larger (tests/conftest.py load_golden merges the parts)."""
+    stem = path[:-len(".npz")]
+    for old in [f for f in os.listdir(OUT) if f.startswith(os.path.basename(stem) + ".part")]:
+        os.remove(os.path.join(OUT, old))
+    if sum(np.asarray(v).nbytes for v in d.values()) <= PART_BYTES:
+        np.savez_compressed(path, **d)
+        return
+    if os.path.exists(path):
+        os.remove(path)
+    parts, cur, size = [], {}, 0
+    for k, v in d.items():
+        n = np.asarray(v).nbytes
+        if cur and size + n > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = v
+        size += n
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(f"{stem}.part{i}.npz", **part)
 
 
 def _flatten(records, full_iters=(0,)):
@@ -70,13 +95,12 @@ def gen_learner(name, models_module=None, **kw):
     for k in ("obs_size", "n_actions", "hidden", "batch_size", "burn_in", "learning", "n_step"):
         d[f"cfg/{k}"] = np.int64(kw.get(k, {"hidden": 128, "batch_size": 32, "burn_in": 20,
                                           "learning": 40, "n_step": 5}.get(k, 0)))
-    path = os.path.join(OUT, name)
-    np.savez_compressed(path, **d)
-    print(name, "iters", len(recs), "iter-times", np.round(times, 3), "size %.2f MB" % (os.path.getsize(path) / 1e6))
+    save_golden(os.path.join(OUT, name), d)
+    print(name, "iters", len(recs), "iter-times", np.round(times, 3))
 
 
 def gen_kat():
-    sys.path.insert(0, ref_harness.REFERENCE_DIR)
+    sys.path.insert(0, ref_harness.reference_dir())
     for m in ("utils",):
         sys.modules.pop(m, None)
     import utils as ref_utils
@@ -93,7 +117,7 @@ def gen_kat():
     d["prio_out"] = np.array([ref_utils.calc_priority(r) for r in td], dtype=np.float64)
     np.savez_compressed(os.path.join(OUT, "ref_kat.npz"), **d)
     sys.modules.pop("utils", None)
-    sys.path.remove(ref_harness.REFERENCE_DIR)
+    sys.path.remove(ref_harness.reference_dir())
     print("ref_kat.npz ok")
 
 
@@ -101,7 +125,7 @@ def gen_sampler_hist(n_draw_batches=400, batch=32):
     """Real LearnerReplayMemory.sample() index stream histogram (replay_memory.py:99-119)."""
     ref_harness._install_stubs(3, 1)
     torch.Tensor.cuda = lambda self, *a, **k: self
-    sys.path.insert(0, ref_harness.REFERENCE_DIR)
+    sys.path.insert(0, ref_harness.reference_dir())
     for m in ("replay_memory",):
         sys.modules.pop(m, None)
     import replay_memory as ref_rm
@@ -129,7 +153,7 @@ def gen_sampler_hist(n_draw_batches=400, batch=32):
                         priorities=np.concatenate(prios), episode_offsets=offs,
                         n_draws=np.int64(n_draw_batches * batch))
     sys.modules.pop("replay_memory", None)
-    sys.path.remove(ref_harness.REFERENCE_DIR)
+    sys.path.remove(ref_harness.reference_dir())
     print("ref_sampler_hist.npz ok", counts.sum())
 
 
@@ -170,8 +194,8 @@ def gen_ingest():
             return _orig(*a, **k)
         _load._r2d2_patched = True
         torch.load = _load
-    if ref_harness.REFERENCE_DIR not in sys.path:
-        sys.path.insert(0, ref_harness.REFERENCE_DIR)
+    if ref_harness.reference_dir() not in sys.path:
+        sys.path.insert(0, ref_harness.reference_dir())
     sys.modules.pop("replay_memory", None)
     import replay_memory as ref_rm
     cwd = os.getcwd()
@@ -213,8 +237,8 @@ def gen_actor_priorities():
         torch.nn.Module.cuda = ident
         for m in ("actor", "replay_memory", "models", "utils", "learner"):
             sys.modules.pop(m, None)
-        if ref_harness.REFERENCE_DIR not in sys.path:
-            sys.path.insert(0, ref_harness.REFERENCE_DIR)
+        if ref_harness.reference_dir() not in sys.path:
+            sys.path.insert(0, ref_harness.reference_dir())
         import tempfile
         cwd = os.getcwd()
         os.chdir(tempfile.mkdtemp(prefix="r2d2_actor_"))     # no model_data/model.pt: load_model() is a no-op (actor.py:51)
@@ -255,7 +279,7 @@ def gen_actor_priorities():
             os.chdir(cwd)
             for m in ("actor", "replay_memory", "models", "utils"):
                 sys.modules.pop(m, None)
-    np.savez_compressed(os.path.join(OUT, "ref_actor_prio.npz"), **d)
+    save_golden(os.path.join(OUT, "ref_actor_prio.npz"), d)
     print("ref_actor_prio.npz ok")
 
 

@@ -1,8 +1,8 @@
 """Oracle harness: run the UNMODIFIED reference learner loop on CPU (this container only).
 
 TEST INFRASTRUCTURE - never imported by the product path.  Only `oracle/make_golden.py`
-(fixture generation, run in the build container where /root/reference is mounted) uses it.
-/root/reference does not exist on the GPU box, so nothing under tests/ -m gpu, smoke() or
+(fixture generation, run where a checkout of the reference is available) uses it.
+The reference is not part of this repository, so nothing under tests/ -m gpu, smoke() or
 bench.py may import this module.
 
 What it does (SURVEY.md section 8c / Appendix A):
@@ -31,7 +31,7 @@ from collections import OrderedDict, deque
 import numpy as np
 import torch
 
-REFERENCE_DIR = os.environ.get("R2D2_REFERENCE_DIR", "/root/reference")
+REFERENCE_DIR = os.environ.get("R2D2_REFERENCE_DIR", "")   # a checkout of jinbeizame007/pytorch-r2d2-DPG
 
 
 class _StopLoop(Exception):
@@ -39,7 +39,17 @@ class _StopLoop(Exception):
 
 
 def reference_available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_DIR, "learner.py"))
+    return bool(REFERENCE_DIR) and os.path.isfile(os.path.join(REFERENCE_DIR, "learner.py"))
+
+
+def reference_dir() -> str:
+    """The reference checkout named by R2D2_REFERENCE_DIR; raises with a clear message when it is unset or wrong."""
+    if not REFERENCE_DIR:
+        raise RuntimeError("set R2D2_REFERENCE_DIR to a checkout of jinbeizame007/pytorch-r2d2-DPG (the unmodified "
+                           "reference the fixtures are generated from)")
+    if not reference_available():
+        raise RuntimeError(f"R2D2_REFERENCE_DIR={REFERENCE_DIR!r} has no learner.py: not a pytorch-r2d2-DPG checkout")
+    return REFERENCE_DIR
 
 
 def _install_stubs(obs_size: int, n_actions: int):
@@ -140,7 +150,7 @@ def run_reference_learner(*, obs_size, n_actions, hidden=128, batch_size=32, bur
         sys.modules.pop(m, None)
     if models_module is not None:
         sys.modules["models"] = models_module
-    if REFERENCE_DIR not in sys.path:
+    if reference_dir() not in sys.path:
         sys.path.insert(0, REFERENCE_DIR)
 
     scratch = scratch or tempfile.mkdtemp(prefix="r2d2_ref_")
@@ -153,7 +163,7 @@ def run_reference_learner(*, obs_size, n_actions, hidden=128, batch_size=32, bur
     cwd = os.getcwd()
     os.chdir(scratch)
     try:
-        import learner as ref_learner  # the real /root/reference/learner.py
+        import learner as ref_learner  # the real reference learner.py
 
         torch.manual_seed(seed)
         lr = ref_learner.Learner(1)

@@ -16,6 +16,17 @@ void set_last_error(const std::string& msg) { g_last_error = msg; }
 const char* last_error() { return g_last_error.c_str(); }
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
+int num_sms() {
+  static std::atomic<int> cache[64];   // 0 = not queried yet
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    cache[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 }  // namespace r2d2
 
 using namespace r2d2;
@@ -28,7 +39,7 @@ static inline NetShape shape_of(const r2d2_net_shape* s) {
 extern "C" {
 
 int r2d2_version(void) { return 100; }
-const char* r2d2_arch(void) { return "sm_100a"; }
+const char* r2d2_arch(void) { return "sm_90a"; }
 const char* r2d2_last_error(void) { return last_error(); }
 
 int r2d2_device_sm_count(int* out) {
@@ -112,27 +123,9 @@ int r2d2_lstm_scan_backward(const float* gates, const float* hs, const float* cs
   return lstm_scan_backward(p, S(stream));
 }
 
-int r2d2_debug_scan_forward_trace(const float* gin, const float* whh, float* gates, float* hs, float* cs, int T, int B,
-                                  int H, long long* trace, r2d2_stream_t stream) {
-  ScanFwdParams p;
-  p.gin = gin; p.whh = whh; p.gates = gates; p.hs = hs; p.cs = cs; p.T = T; p.B = B; p.H = H; p.repeat = 1; p.trace = trace;
-  return lstm_scan_forward(p, S(stream));
-}
-
-int r2d2_debug_scan_backward_trace(const float* gates, const float* hs, const float* cs, const float* whh,
-                                   const float* dh_head, float* dgates, int T, int B, int H, long long* trace,
-                                   r2d2_stream_t stream) {
-  ScanBwdParams p;
-  p.gates = gates; p.hs = hs; p.cs = cs; p.whh = whh; p.dh_head = dh_head; p.dgates = dgates; p.dgin = dgates;
-  p.T = T; p.B = B; p.H = H; p.repeat = 1; p.trace = trace;
-  return lstm_scan_backward(p, S(stream));
-}
-
-int r2d2_debug_max_active_clusters(int H, int nb, int backward) { return lstm_scan_max_active_clusters(H, nb, backward); }
-
 int r2d2_set_gemm_impl(int impl) {
   gemm_set_impl(impl != 0);
-  gemm_set_impl_skinny_mma(impl != 2);  // 2 = force the tcgen05 path even for skinny problems (tests)
+  gemm_set_impl_skinny_mma(impl != 2);  // 2 = force the wgmma path even for skinny problems (tests)
   return R2D2_OK;
 }
 int r2d2_get_gemm_impl(void) { return gemm_get_impl(); }

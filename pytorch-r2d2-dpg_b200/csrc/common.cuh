@@ -1,4 +1,4 @@
-// Shared device/host helpers for libr2d2_b200 (sm_100a only).
+// Shared device/host helpers for libr2d2_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -55,13 +55,17 @@ struct PerDeviceOnce {
   }
 };
 
+// streaming multiprocessors of the current device (cached per device): sizes grids of the grid-stride kernels and
+// split-K factors
+int num_sms();
+
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline long long ceil_div_ll(long long a, long long b) { return (a + b - 1) / b; }
 
 // ---- bf16 hi/lo split: x ~= hi + lo with ~16 significant bits; products hi*hi + hi*lo + lo*hi.
 // Done with integer ops on the fp32 bit pattern (round-half-up on the magnitude, then keep the upper 16 bits): the
-// F2F.BF16.F32 conversion instruction runs on a 16/clk/SM pipe and made the operand staging of the tcgen05 GEMM
-// conversion-bound (2 conversions per element); IADD/LOP/PRMT/FADD issue at full rate.
+// F2F.BF16.F32 conversion instruction runs on a 16/clk/SM pipe and makes operand staging conversion-bound
+// (2 conversions per element); IADD/LOP/PRMT/FADD issue at full rate.
 __device__ __forceinline__ uint32_t bf16_hi_bits(float x) { return (__float_as_uint(x) + 0x8000u) & 0xFFFF0000u; }
 
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
@@ -104,15 +108,14 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* 
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per lane and instruction.  The GEMM
-// epilogue has lane = output row, so two 16-byte stores per sector reached L2 as two partial-sector writes.
+// one full 32-byte sector per lane (p 32-byte aligned), as two 16-byte accesses
 __device__ __forceinline__ void st_global_v8(float* p, const float (&v)[8]) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]),
-               "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
+  reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+  reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
 }
 __device__ __forceinline__ void ld_global_v8(const float* p, float (&v)[8]) {
-  asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]),
-               "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p));
+  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }

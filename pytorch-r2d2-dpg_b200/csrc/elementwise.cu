@@ -4,6 +4,9 @@
 #include "elementwise.cuh"
 
 #include <cmath>
+#include <map>
+#include <mutex>
+#include <utility>
 
 namespace r2d2 {
 namespace {
@@ -17,7 +20,7 @@ __device__ __forceinline__ float value_rescale(float x) {
 // fallback (no td_sq buffer to reduce through): grid ceil(B/32) CTAs, 1024 threads = 32 warps; lane -> batch column, warp -> time rows i = w, w+32, ...
 // (the kernel moves ~1 MB: it is bound by the length of the per-thread dependent load chain, hence the wide block)
 constexpr int TD_WARPS = 32;
-__global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPriorityParams p) {
+__global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPriorityParams p, float* loss_part) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int b = blockIdx.x * 32 + lane;
   const int L = p.L, B = p.B, A = p.A;
@@ -60,11 +63,11 @@ __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPri
       const int count = L - ((b == B - 1) ? 1 : 0);
       p.priority[b] = p.eta * mx + (1.0f - p.eta) * (sm / (float)count);  // utils.py:17-18
     }
-    if (lane == 0 && p.loss_sum) {
+    if (lane == 0 && loss_part) {
       float tot = 0.f;
 #pragma unroll
       for (int k = 0; k < TD_WARPS; ++k) tot += s_sq[k];
-      atomicAdd(p.loss_sum, tot / ((float)L * (float)B * (float)A));
+      loss_part[blockIdx.x] = tot / ((float)L * (float)B * (float)A);
     }
   }
 }
@@ -114,7 +117,7 @@ __global__ void __launch_bounds__(TD1_WARPS * 32) td_elem_kernel(TdPriorityParam
 }
 
 constexpr int TD2_WARPS = 8;
-__global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityParams p) {
+__global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityParams p, float* loss_part) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int b = blockIdx.x * 32 + lane;
   const int L = p.L, B = p.B;
@@ -139,13 +142,13 @@ __global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityPar
       p.priority[b] = p.eta * mx + (1.0f - p.eta) * (sm / (float)count);  // utils.py:17-18
     }
     tt = warp_sum(tt);   // critic loss = mean over (i, b, a) of diff^2 = sum of td_sq / (L * B)
-    if (lane == 0 && p.loss_sum) atomicAdd(p.loss_sum, tt / ((float)L * (float)B));
+    if (lane == 0 && loss_part) loss_part[blockIdx.x] = tt / ((float)L * (float)B);
   }
 }
 
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x, long long ld, int M, int N,
-                                                     int rows_per_block, float* __restrict__ out, float* __restrict__ out2) {
-  // block = 32 columns x 8 row lanes; grid.x over column chunks, grid.y over row ranges; atomics into out
+                                                     int rows_per_block, float* __restrict__ part) {
+  // block = 32 columns x 8 row lanes; grid.x over column chunks, grid.y over row ranges; row range y writes slice y
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int col = blockIdx.x * 32 + lane;
   const int r0 = blockIdx.y * rows_per_block;
@@ -160,8 +163,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x
     float t = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) t += sm[k][lane];
-    atomicAdd(out + col, t);
-    if (out2) atomicAdd(out2 + col, t);
+    part[(size_t)blockIdx.y * N + col] = t;
   }
 }
 
@@ -187,7 +189,7 @@ __global__ void __launch_bounds__(256) fill_kernel(float* __restrict__ x, long l
 }
 
 __global__ void __launch_bounds__(256) scaled_sum_kernel(const float* __restrict__ x, long long n, float scale,
-                                                         float* __restrict__ out) {
+                                                         float* __restrict__ part) {
   float acc = 0.f;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     acc += x[i];
@@ -198,7 +200,19 @@ __global__ void __launch_bounds__(256) scaled_sum_kernel(const float* __restrict
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int k = 0; k < 8; ++k) t += sm[k];
-    atomicAdd(out, t * scale);
+    part[blockIdx.x] = t * scale;
+  }
+}
+
+__global__ void __launch_bounds__(256) add_partials_kernel(const float* __restrict__ part, int slices, int rows, int cols,
+                                                           float* __restrict__ dst, long long ld_dst, float* __restrict__ dst2) {
+  const long long n = (long long)rows * cols, stride = n;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float t = 0.f;
+    for (int s = 0; s < slices; ++s) t += part[s * stride + i];
+    const long long r = i / cols, c = i % cols;
+    dst[r * ld_dst + c] += t;
+    if (dst2) dst2[r * ld_dst + c] += t;
   }
 }
 
@@ -293,7 +307,7 @@ int add_vec(const float* a, const float* b, float* out, int n, cudaStream_t stre
 
 int mul_dtanh(const float* d_out, const float* out, float* d_pre, long long n, cudaStream_t stream) {
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   mul_dtanh_kernel<<<blocks, 256, 0, stream>>>(d_out, out, d_pre, n);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
@@ -303,34 +317,43 @@ int mul_dtanh(const float* d_out, const float* out, float* d_pre, long long n, c
 int td_priority(const TdPriorityParams& p, cudaStream_t stream) {
   R2D2_REQUIRE(p.q && p.q_next && p.rew && p.term, "null input");
   R2D2_REQUIRE(p.L > 0 && p.B > 0 && p.A > 0, "shape");
-  if (p.loss_sum) R2D2_CUDA_TRY(cudaMemsetAsync(p.loss_sum, 0, sizeof(float), stream));
+  const int col_blocks = ceil_div(p.B, 32);
+  float* loss_part = nullptr;     // one partial loss per column block, summed in block order
+  if (p.loss_sum) {
+    R2D2_CUDA_TRY(cudaMemsetAsync(p.loss_sum, 0, sizeof(float), stream));
+    R2D2_TRY(partials_scratch(col_blocks, stream, &loss_part));
+  }
   const size_t smem = (size_t)TD1_WARPS * 2 * 32 * p.A * sizeof(float);
   if (p.td_sq && smem <= 48 * 1024) {   // the path's configuration: two line-coalesced passes over L x B x A and L x B
-    td_elem_kernel<<<dim3(ceil_div(p.B, 32), ceil_div(p.L, TD1_WARPS)), TD1_WARPS * 32, smem, stream>>>(p);
+    td_elem_kernel<<<dim3(col_blocks, ceil_div(p.L, TD1_WARPS)), TD1_WARPS * 32, smem, stream>>>(p);
     count_launch();
     if (p.priority || p.loss_sum) {
-      td_reduce_kernel<<<ceil_div(p.B, 32), TD2_WARPS * 32, 0, stream>>>(p);
+      td_reduce_kernel<<<col_blocks, TD2_WARPS * 32, 0, stream>>>(p, loss_part);
       count_launch();
     }
   } else {
-    td_priority_column_kernel<<<ceil_div(p.B, 32), TD_WARPS * 32, 0, stream>>>(p);
+    td_priority_column_kernel<<<col_blocks, TD_WARPS * 32, 0, stream>>>(p, loss_part);
     count_launch();
   }
   R2D2_CUDA_TRY(cudaGetLastError());
+  if (p.loss_sum) R2D2_TRY(add_partials(loss_part, col_blocks, 1, 1, p.loss_sum, 1, nullptr, stream));
   return R2D2_OK;
 }
 
 int colsum(const float* x, long long ld, int M, int N, float* out, float* out2, cudaStream_t stream) {
   R2D2_REQUIRE(x && out && M > 0 && N > 0, "colsum args");
   const int col_blocks = ceil_div(N, 32);
-  int row_blocks = ceil_div(4 * 148, col_blocks);
+  int row_blocks = ceil_div(4 * num_sms(), col_blocks);
   if (row_blocks > ceil_div(M, 64)) row_blocks = ceil_div(M, 64);
   if (row_blocks < 1) row_blocks = 1;
   const int rows_per_block = ceil_div(M, row_blocks);
-  colsum_kernel<<<dim3(col_blocks, ceil_div(M, rows_per_block)), 256, 0, stream>>>(x, ld, M, N, rows_per_block, out, out2);
+  const int slices = ceil_div(M, rows_per_block);
+  float* part = nullptr;
+  R2D2_TRY(partials_scratch((size_t)slices * N, stream, &part));
+  colsum_kernel<<<dim3(col_blocks, slices), 256, 0, stream>>>(x, ld, M, N, rows_per_block, part);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
-  return R2D2_OK;
+  return add_partials(part, slices, 1, N, out, N, out2, stream);
 }
 
 int adam_step(float* param, const float* grad, float* m, float* v, long long n, int step, float lr, float beta1,
@@ -341,7 +364,7 @@ int adam_step(float* param, const float* grad, float* m, float* v, long long n, 
   const float step_size = (float)((double)lr / bc1);
   const float inv_bc2_sqrt = (float)(1.0 / sqrt(bc2));
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   adam_kernel<<<blocks, 256, 0, stream>>>(param, grad, m, v, n, grad_scale, beta1, beta2, step_size, inv_bc2_sqrt, eps);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
@@ -350,7 +373,7 @@ int adam_step(float* param, const float* grad, float* m, float* v, long long n, 
 
 int fill_f32(float* x, long long n, float value, cudaStream_t stream) {
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   fill_kernel<<<blocks, 256, 0, stream>>>(x, n, value);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
@@ -360,8 +383,43 @@ int fill_f32(float* x, long long n, float value, cudaStream_t stream) {
 int scaled_sum(const float* x, long long n, float scale, float* out, cudaStream_t stream) {
   R2D2_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float), stream));
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 4) blocks = 148 * 4;
-  scaled_sum_kernel<<<blocks, 256, 0, stream>>>(x, n, scale, out);
+  if (blocks > num_sms() * 4) blocks = num_sms() * 4;
+  float* part = nullptr;
+  R2D2_TRY(partials_scratch(blocks, stream, &part));
+  scaled_sum_kernel<<<blocks, 256, 0, stream>>>(x, n, scale, part);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return add_partials(part, blocks, 1, 1, out, 1, nullptr, stream);
+}
+
+namespace {
+struct PartialsBuf { float* ptr = nullptr; size_t floats = 0; };
+std::mutex g_partials_mutex;
+std::map<std::pair<int, cudaStream_t>, PartialsBuf> g_partials;
+}  // namespace
+
+int partials_scratch(size_t floats, cudaStream_t stream, float** out) {
+  int dev = 0;
+  R2D2_CUDA_TRY(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(g_partials_mutex);
+  PartialsBuf& b = g_partials[std::make_pair(dev, stream)];
+  if (b.floats < floats) {
+    if (b.ptr) { R2D2_CUDA_TRY(cudaDeviceSynchronize()); R2D2_CUDA_TRY(cudaFree(b.ptr)); b.ptr = nullptr; b.floats = 0; }
+    const size_t want = floats + floats / 4 + (1u << 16);
+    R2D2_CUDA_TRY(cudaMalloc(&b.ptr, want * sizeof(float)));
+    b.floats = want;
+  }
+  *out = b.ptr;
+  return R2D2_OK;
+}
+
+int add_partials(const float* part, int slices, int rows, int cols, float* dst, long long ld_dst, float* dst2,
+                 cudaStream_t stream) {
+  R2D2_REQUIRE(part && dst && slices >= 1 && rows >= 1 && cols >= 1 && ld_dst >= cols, "add_partials args");
+  const long long n = (long long)rows * cols;
+  int blocks = (int)((n + 255) / 256);
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+  add_partials_kernel<<<blocks, 256, 0, stream>>>(part, slices, rows, cols, dst, ld_dst, dst2);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;

@@ -34,4 +34,12 @@ int adam_step(float* param, const float* grad, float* m, float* v, long long n, 
 int fill_f32(float* x, long long n, float value, cudaStream_t stream);
 int scaled_sum(const float* x, long long n, float scale, float* out, cudaStream_t stream);
 
+// Deterministic accumulation.  A kernel that would add many partial results into one place writes them instead into
+// slices of a scratch buffer (grow-only, one per device and stream, valid until the next call on the same stream), and
+// add_partials adds the slices in slice order, so that every run sums in the same order and gets the same bits:
+//   dst[r * ld_dst + c] += sum_{s < slices} part[(s * rows + r) * cols + c]   (and the same sum into dst2 if given)
+int partials_scratch(size_t floats, cudaStream_t stream, float** out);
+int add_partials(const float* part, int slices, int rows, int cols, float* dst, long long ld_dst, float* dst2,
+                 cudaStream_t stream);
+
 }  // namespace r2d2

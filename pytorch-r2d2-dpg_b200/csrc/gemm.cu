@@ -58,7 +58,7 @@ __device__ __forceinline__ void store_split4(__nv_bfloat16* hi_plane, __nv_bfloa
 
 template <int LAYOUT>
 __global__ void __launch_bounds__(GEMM_THREADS)
-gemm_bf16x3_kernel(GemmParams p, int vecA, int vecB, int vecA2, int vecB2) {
+gemm_bf16x3_kernel(GemmParams p, int vecA, int vecB, int vecA2, int vecB2, long long c_split_stride) {
   using G = TileGeom<LAYOUT>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __nv_bfloat16* smem = reinterpret_cast<__nv_bfloat16*>(smem_raw);
@@ -184,7 +184,9 @@ gemm_bf16x3_kernel(GemmParams p, int vecA, int vecB, int vecA2, int vecB2) {
 
   // ---- epilogue ----
   const int g = lane >> 2, c = lane & 3;
-  const bool vec_c = ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0) && (p.ldc % 2 == 0) && p.split_k == 1;
+  // split-K: slice blockIdx.z of the partial products (c_split_stride floats apart), summed in order by the caller
+  float* const C = p.C + (long long)blockIdx.z * c_split_stride;
+  const bool vec_c = ((reinterpret_cast<uintptr_t>(C) & 7) == 0) && (p.ldc % 2 == 0);
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
 #pragma unroll
@@ -207,11 +209,8 @@ gemm_bf16x3_kernel(GemmParams p, int vecA, int vecB, int vecA2, int vecB2) {
           v0 += z[0];
           if (has1) v1 += z[1];
         }
-        float* cp = p.C + (long long)row * p.ldc + col;
-        if (p.split_k > 1) {
-          atomicAdd(cp, v0);
-          if (has1) atomicAdd(cp + 1, v1);
-        } else if (vec_c && has1) {
+        float* cp = C + (long long)row * p.ldc + col;
+        if (vec_c && has1) {
           *reinterpret_cast<float2*>(cp) = make_float2(v0, v1);
         } else {
           cp[0] = v0;
@@ -233,11 +232,20 @@ int launch_gemm(const GemmParams& p, cudaStream_t stream) {
   auto aligned = [](const float* ptr, long long ld) {
     return ptr != nullptr && ((reinterpret_cast<uintptr_t>(ptr) & 15) == 0) && (ld % 4 == 0);
   };
-  dim3 grid(ceil_div(p.N, BN), ceil_div(p.M, BM), p.split_k);
+  GemmParams q = p;
+  int slices = 1;
+  if (p.split_k > 1) {   // partial products into slices, then added into C in slice order (same bits every run)
+    const int nk = ceil_div(p.K, BK) + ceil_div(p.K2, BK), per_split = ceil_div(nk, p.split_k);
+    slices = ceil_div(nk, per_split);                    // every slice z < slices owns at least one k tile
+    R2D2_TRY(partials_scratch((size_t)slices * p.M * p.N, stream, &q.C));
+    q.ldc = p.N;
+  }
+  dim3 grid(ceil_div(p.N, BN), ceil_div(p.M, BM), slices);
   gemm_bf16x3_kernel<LAYOUT><<<grid, GEMM_THREADS, G::SMEM_BYTES, stream>>>(
-      p, aligned(p.A, p.lda), aligned(p.B, p.ldb), aligned(p.A2, p.lda2), aligned(p.B2, p.ldb2));
+      q, aligned(p.A, p.lda), aligned(p.B, p.ldb), aligned(p.A2, p.lda2), aligned(p.B2, p.ldb2), (long long)p.M * p.N);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
+  if (p.split_k > 1) return add_partials(q.C, slices, p.M, p.N, p.C, p.ldc, nullptr, stream);
   return R2D2_OK;
 }
 
@@ -266,7 +274,7 @@ bool gemm_emits_operand_image(int M, int N, int K_total) {
   if (gemm_get_impl() != 1 || N <= 32 || N % 32 != 0) return false;
   if (gemm_get_impl_skinny_mma() && K_total <= 32) return true;                 // small-K streaming kernel (gemm_thin.cu)
   const bool skinny = (K_total < 64) || (M < 32);
-  return !(skinny && gemm_get_impl_skinny_mma());                              // tcgen05 epilogue (gemm_tc.cu)
+  return !(skinny && gemm_get_impl_skinny_mma());                              // wgmma epilogue (gemm_tc.cu)
 }
 
 int gemm_suggest_split_k(int M, int N, int K) {
@@ -274,8 +282,8 @@ int gemm_suggest_split_k(int M, int N, int K) {
   if (gemm_get_impl() == 1 && !(skinny && g_skinny_mma)) return gemm_tc_suggest_split_k(M, N, K);
   long long tiles = (long long)ceil_div(M, BM) * ceil_div(N, BN);
   int k_tiles = ceil_div(K, BK);
-  if (tiles >= 148 || k_tiles < 16) return 1;
-  int want = (int)ceil_div_ll(2 * 148, tiles);
+  if (tiles >= num_sms() || k_tiles < 16) return 1;
+  int want = (int)ceil_div_ll(2 * num_sms(), tiles);
   int max_by_k = k_tiles / 8;  // keep >= 8 k-tiles (256 k) per split
   int s = want < max_by_k ? want : max_by_k;
   if (s < 1) s = 1;
@@ -310,16 +318,16 @@ static int gemm_f32_dispatch(const GemmParams& p, GemmLayout layout, cudaStream_
   R2D2_REQUIRE((p.epilogue != EPI_MUL_DTANH && p.epilogue != EPI_ADD_Z) || p.Z, "epilogue needs Z");
   R2D2_REQUIRE(ceil_div(p.M, BM) <= 65535, "M too large for grid.y");
   // skinny problems (K < 64: obs/act inputs; N < 32: heads, dW1/dW3 blocks) are launch/latency bound: the single-launch
-  // mma.sync kernel beats pack + pack + tcgen05 there (tools/gemm_bench.py); everything else goes to the tcgen05 path
+  // mma.sync kernel beats pack + pack + wgmma there (tools/gemm_bench.py); everything else goes to the wgmma path
   const bool skinny = (p.K + p.K2 < 64) || (p.N < 32) || (p.M < 32);
   if (gemm_get_impl() == 1 && gemm_get_impl_skinny_mma()) {   // default mode: degenerate shapes -> fp32 streaming kernels
     bool handled = false;
     R2D2_TRY(gemm_thin_try(p, layout, stream, &handled));
     if (handled) { *colsums_done = true; return R2D2_OK; }
   }
-  R2D2_REQUIRE(!p.bias2 || gemm_supports_bias2(p.M, p.N, p.K + p.K2), "bias2 needs the tcgen05 path (gemm_supports_bias2)");
+  R2D2_REQUIRE(!p.bias2 || gemm_supports_bias2(p.M, p.N, p.K + p.K2), "bias2 needs the wgmma path (gemm_supports_bias2)");
   R2D2_REQUIRE((!p.C_img_k && !p.C_img_mn) || (layout == GEMM_NT && gemm_emits_operand_image(p.M, p.N, p.K + p.K2)),
-               "C_img_* is produced by the small-K streaming kernel and the tcgen05 epilogue only (see gemm_emits_operand_image)");
+               "C_img_* is produced by the small-K streaming kernel and the wgmma epilogue only (see gemm_emits_operand_image)");
   if (gemm_get_impl() == 1 && !(skinny && gemm_get_impl_skinny_mma())) {
     static int dbg = -1;
     if (dbg < 0) { const char* e = getenv("R2D2_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }

@@ -29,38 +29,38 @@ struct GemmParams {
   float* C = nullptr;        long long ldc = 0;
   int M = 0, N = 0, K = 0;
   const float* bias = nullptr;          // [N]
-  const float* bias2 = nullptr;         // [N] second bias added to the first (b_ih + b_hh); tcgen05 path only, see
+  const float* bias2 = nullptr;         // [N] second bias added to the first (b_ih + b_hh); wgmma path only, see
                                         // gemm_supports_bias2
   const float* Z = nullptr;  long long ldz = 0;   // [M,N] aux for the epilogue
   int epilogue = EPI_NONE;
-  int split_k = 1;           // >1: partial products are atomically added into C (C must be pre-zeroed)
-  const unsigned char* A_img = nullptr;   // tcgen05 path: A already in packed tile-major form (gemm_tc.cu image of this
+  int split_k = 1;           // >1: K split over CTAs; the partial products are added into C in split order
+  const unsigned char* A_img = nullptr;   // wgmma path: A already in packed tile-major form (gemm_tc.cu image of this
                              // call's layout and tiling, e.g. written by the BPTT scan); A / lda are ignored
   unsigned char* C_img_k = nullptr;      // NT, N % 32 == 0 (gemm_emits_operand_image): also write C as the K-major packed operand image
                              // [ceil(M/128)][N/32][16 KB] for a following product that contracts over N
   unsigned char* C_img_mn = nullptr;     // same, MN-major image [ceil(N/128)][ceil(M/32)][16 KB]: C as the B operand of a TN
                              // product that contracts over C's rows (z1 in dW_ih)
-  const unsigned char* B_img = nullptr;   // tcgen05 path: B already packed (image of this call's layout and tiling)
+  const unsigned char* B_img = nullptr;   // wgmma path: B already packed (image of this call's layout and tiling)
   float* colsum_a = nullptr;             // TN only: also ADD the column sums of A[K,M] (M values) / B[K,N] (N values) here:
   float* colsum_b = nullptr;             // the bias gradient that goes with a weight gradient reads the same rows
-  int reuse_packed_a = 0;    // tcgen05 path: A (pointer, shape, layout) is the operand the previous gemm_f32 call packed
+  int reuse_packed_a = 0;    // wgmma path: A (pointer, shape, layout) is the operand the previous gemm_f32 call packed
                              // and its contents have not changed since -> skip the pack pass (dW_hh then dW_ih of a chain)
   int debug_flags = 0;       // dev only (env R2D2_GEMM_DEBUG): 1 = producers skip fetch+convert, 2 = skip MMAs, 4 = skip epilogue stores
 };
 
 int gemm_f32(const GemmParams& p, GemmLayout layout, cudaStream_t stream);
 // true when gemm_f32 will honour GemmParams::C_img_k / C_img_mn for an NT product with these sizes (the small-K streaming
-// kernel or the tcgen05 epilogue is selected)
+// kernel or the wgmma epilogue is selected)
 bool gemm_emits_operand_image(int M, int N, int K_total);
-// true when gemm_f32 will take this NT product on the tcgen05 path, which honours GemmParams::bias2
+// true when gemm_f32 will take this NT product on the wgmma path, which honours GemmParams::bias2
 bool gemm_supports_bias2(int M, int N, int K);
-// picks a split-K factor so that a skinny-output wgrad GEMM fills the 148 SMs
+// picks a split-K factor so that a skinny-output wgrad GEMM fills the SMs
 int gemm_suggest_split_k(int M, int N, int K);
 
-// implementation: 1 = tcgen05/TMEM kernel (default), 0 = mma.sync v1 kernel; env R2D2_GEMM_IMPL = "tc" | "mma"
+// implementation: 1 = wgmma kernel (default), 0 = mma.sync kernel; env R2D2_GEMM_IMPL = "tc" | "mma"
 void gemm_set_impl(int impl);
 int gemm_get_impl();
-// with the tcgen05 implementation selected, skinny problems still take the single-launch mma.sync kernel (default on)
+// with the wgmma implementation selected, skinny problems still take the single-launch mma.sync kernel (default on)
 void gemm_set_impl_skinny_mma(int on);
 int gemm_get_impl_skinny_mma();
 int gemm_f32_tc(const GemmParams& p, GemmLayout layout, cudaStream_t stream);

@@ -1,28 +1,26 @@
-// gemm_f32 on the 5th-gen tensor cores (sm_100a):
+// gemm_f32 on the Hopper tensor cores (sm_90a, wgmma):
 //
 //  1. operand images: every operand is bf16 hi/lo planes stored TILE-MAJOR in exactly the shared-memory image the MMA
-//     wants - one 16 KB block per (128-row tile, 32-deep k tile) = hi plane (8 KB) + lo plane (8 KB) in UMMA
-//     core-matrix order, zero padded.  Producers that can write it directly do (GemmParams::A_img / B_img: the BPTT
-//     scan for dG, the l1 kernel for z1); otherwise pack_operand_kernel converts the fp32 tensor (any leading
-//     dimension, ragged edges) in an HBM-bound elementwise pass (8 B/element).
-//  2. gemm_packed_kernel<NBT>: per CTA one 128 x (128 NBT) output tile.  A producer thread streams the tile images with
-//     1-D bulk copies (cp.async.bulk ... mbarrier::complete_tx, no tensor map, no per-element work) through a 2-3
-//     stage ring; one elected thread issues tcgen05.mma (M=128, N<=128, K=16; passes lo*hi + hi*lo + hi*hi) into one
-//     TMEM accumulator per B tile; eight epilogue warps read them back with tcgen05.ld, transpose 32 x 32 blocks
-//     through the idle stage buffers and apply bias / tanh / dtanh / +Z or the split-K reduction with line-coalesced
-//     global accesses.  <= 96 KB smem + <= 256 TMEM columns per CTA -> two CTAs per SM overlap each other's epilogue.
+//     wants - one 16 KB block per (128-row tile, 32-deep k tile) = hi plane (8 KB) + lo plane (8 KB) in core-matrix
+//     order (no swizzle), zero padded.  Producers that can write it directly do (GemmParams::A_img / B_img, the l1
+//     kernel for z1); otherwise pack_operand_kernel converts the fp32 tensor (any leading dimension, ragged edges) in an
+//     HBM-bound elementwise pass (8 B/element).
+//  2. gemm_packed_kernel: per CTA one 128 x 128 output tile.  A producer thread streams the tile images with 1-D bulk
+//     copies (cp.async.bulk ... mbarrier::complete_tx, no tensor map, no per-element work) through a 4-stage ring; two
+//     consumer warpgroups each issue wgmma.m64n128k16 (passes lo*hi + hi*lo + hi*hi) into register accumulators and
+//     apply bias / tanh / dtanh / +Z or the split-K reduction straight from the accumulator fragments.
 //
-// Why images instead of fp32 operands: staging fp32 through shared memory inside the GEMM (cp.async -> ld.shared ->
-// split -> st.shared) cost 60% of the kernel (ablation in profiles/r01_summary.md); the image is the same byte count
-// as the fp32 operand and is re-read ~N/256 (A) or ~M/128 (B) times from L2.
+// Why images instead of fp32 operands: the image is the same byte count as the fp32 operand, is re-read ~N/128 (A)
+// or ~M/128 (B) times from L2, and needs no conversion inside the GEMM's main loop.
 #include <stdlib.h>
 
 #include <map>
 #include <mutex>
 #include <utility>
 
+#include "elementwise.cuh"
 #include "gemm.cuh"
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 namespace r2d2 {
 namespace {
@@ -30,16 +28,11 @@ namespace {
 constexpr int TBM = 128, TBN = 128, TBK = 32;
 constexpr int PLANE_BYTES = 128 * TBK * 2;     // 8 KB: one bf16 plane of a 128 x 32 operand tile
 constexpr int TILE_BYTES = 2 * PLANE_BYTES;    // 16 KB: hi plane + lo plane of one operand tile
-constexpr int PACKED_GEMM_THREADS = 320;       // warp 0 producer, warp 1 MMA, warps 2..9 epilogue
-// NBT = B tiles (of 128 columns) per CTA.  NBT = 2 halves the number of times the A images are pulled from L2 (the
-// kernel is bound by the L2 -> shared-memory path, profiles/r01_summary.md); both shapes keep ~96 KB of stages and
-// at most 256 TMEM columns per CTA so that two CTAs share an SM and overlap each other's epilogue.
-template <int NBT> struct PackedCfg {
-  static constexpr int STAGES = NBT == 1 ? 3 : 2;
-  static constexpr int STAGE_BYTES = (1 + NBT) * TILE_BYTES;
-  static constexpr int OFF_BARS = STAGES * STAGE_BYTES;
-  static constexpr int SMEM = OFF_BARS + 128;
-};
+constexpr int PACKED_GEMM_THREADS = 384;       // warpgroup 0 producer, warpgroups 1..2 wgmma + epilogue
+constexpr int STAGES = 4;
+constexpr int STAGE_BYTES = 2 * TILE_BYTES;    // A tile + B tile
+constexpr int OFF_BARS = STAGES * STAGE_BYTES;
+constexpr int PACKED_SMEM = OFF_BARS + 128;
 
 // ---- operand tile image (shared with the MMA descriptors below) --------------------------------------------------
 // a tile is 512 groups of 8 elements; group `id` lives at byte id*16 of each plane.
@@ -83,7 +76,7 @@ __global__ void __launch_bounds__(256) pack_operand_kernel(const float* __restri
 }
 
 __device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
-  while (!tc::mbar_try_wait(bar, parity)) {}
+  while (!sm90::mbar_try_wait(bar, parity)) {}
 }
 
 struct PackedGemmParams {
@@ -96,230 +89,162 @@ struct PackedGemmParams {
   const float* bias2;
   const float* Z; long long ldz;
   int epilogue, split_k;
-  int a_mn, b_mn;            // operand majors (1 = MN-major)
+  long long c_split_stride;  // split_k > 1: CTA z writes its partial product to C + z * c_split_stride
   int debug_flags;
   unsigned char* c_img_k;    // optional: C also leaves as packed operand images (N % 32 == 0, split_k == 1), see epilogue
   unsigned char* c_img_mn;
 };
 
-template <int NBT>
-__global__ void __launch_bounds__(PACKED_GEMM_THREADS, 2) gemm_packed_kernel(PackedGemmParams p) {
-  using CFG = PackedCfg<NBT>;
-  constexpr int TSTAGES = CFG::STAGES, STAGE_BYTES = CFG::STAGE_BYTES;
+// 3 warpgroups: warpgroup 0 = producer (one elected thread), warpgroups 1 and 2 = consumers, each owning 64 rows of the
+// 128 x 128 output tile as wgmma register accumulators.
+template <bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(PACKED_GEMM_THREADS, 1) gemm_packed_kernel(PackedGemmParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + CFG::OFF_BARS);   // [TSTAGES] bytes landed
-  uint64_t* empty = full + TSTAGES;                                     // [TSTAGES] MMAs retired
-  uint64_t* accum_full = empty + TSTAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_full + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BARS);   // [STAGES] bytes landed
+  uint64_t* empty = full + STAGES;                                  // [STAGES] both consumer warpgroups done reading
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int w_u = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int m_tile = blockIdx.y, n_blk = blockIdx.x;
-  const int m0 = m_tile * TBM, n0 = n_blk * TBN * NBT;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);
+  const int m_tile = blockIdx.y, n_tile = blockIdx.x;
+  const int m0 = m_tile * TBM, n0 = n_tile * TBN;
   const int per_split = (p.k_tiles + p.split_k - 1) / p.split_k;
   const int t_begin = blockIdx.z * per_split;
   const int t_end = min(p.k_tiles, t_begin + per_split);
   if (t_begin >= t_end) return;
   const int n_tiles = t_end - t_begin;
-  int n_eff[NBT], nb_live = 0;                       // columns of each B tile (rounded up to the MMA granule), live tiles
-#pragma unroll
-  for (int j = 0; j < NBT; ++j) {
-    int e = min(TBN, p.N - n0 - j * TBN);
-    n_eff[j] = e > 0 ? ((e + 15) & ~15) : 0;
-    if (e > 0) nb_live = j + 1;
-  }
 
   if (tid == 0) {
-    for (int s = 0; s < TSTAGES; ++s) { tc::mbar_init(&full[s], 1); tc::mbar_init(&empty[s], 1); }
-    tc::mbar_init(accum_full, 1);
+    for (int s = 0; s < STAGES; ++s) { sm90::mbar_init(&full[s], 1); sm90::mbar_init(&empty[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (w_u == 1) { __syncwarp(); tc::tmem_alloc(tmem_slot, TBN * NBT); }
-  tc::fence_before_thread_sync();
   __syncthreads();
-  tc::fence_after_thread_sync();
-  const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot, 0);
 
-  if (w_u == 0) {
+  if (wg == 0) {
     // ================= producer: one 16 KB bulk copy per operand tile and k tile =================
-    if (tc::elect_one()) {
+    if (tid < 32 && sm90::elect_one()) {
       const unsigned char* a_src = p.pa + ((size_t)m_tile * p.k_tiles + t_begin) * TILE_BYTES;
-      const unsigned char* b_src = p.pb + ((size_t)(n_blk * NBT) * p.k_tiles + t_begin) * TILE_BYTES;
-      const uint32_t smem_base = tc::smem_u32(smem);
+      const unsigned char* b_src = p.pb + ((size_t)n_tile * p.k_tiles + t_begin) * TILE_BYTES;
+      const uint32_t smem_base = sm90::smem_u32(smem);
       for (int i = 0; i < n_tiles; ++i) {
-        const int s = i % TSTAGES;
-        mbar_wait_spin(&empty[s], ((i / TSTAGES) & 1) ^ 1);
-        const uint32_t bar = tc::smem_u32(&full[s]);
-        tc::mbar_arrive_expect_tx(&full[s], (uint32_t)((1 + nb_live) * TILE_BYTES));
-        tc::bulk_copy_g2s(smem_base + s * STAGE_BYTES, a_src + (size_t)i * TILE_BYTES, TILE_BYTES, bar);
-#pragma unroll
-        for (int j = 0; j < NBT; ++j)
-          if (j < nb_live)
-            tc::bulk_copy_g2s(smem_base + s * STAGE_BYTES + (1 + j) * TILE_BYTES,
-                              b_src + ((size_t)j * p.k_tiles + i) * TILE_BYTES, TILE_BYTES, bar);
+        const int s = i % STAGES;
+        mbar_wait_spin(&empty[s], ((i / STAGES) & 1) ^ 1);
+        const uint32_t bar = sm90::smem_u32(&full[s]);
+        sm90::mbar_arrive_expect_tx(&full[s], 2 * TILE_BYTES);
+        sm90::bulk_copy_g2s(smem_base + s * STAGE_BYTES, a_src + (size_t)i * TILE_BYTES, TILE_BYTES, bar);
+        sm90::bulk_copy_g2s(smem_base + s * STAGE_BYTES + TILE_BYTES, b_src + (size_t)i * TILE_BYTES, TILE_BYTES, bar);
       }
     }
-    __syncwarp();
-  } else if (w_u == 1) {
-    // ================= MMA issuer =================
-    const uint32_t idesc_base = ((p.a_mn ? 1u : 0u) << 15) | ((p.b_mn ? 1u : 0u) << 16);
-    const uint64_t da0 = p.a_mn ? tc::make_smem_desc(tc::smem_u32(smem), 2048, 128) : tc::make_smem_desc(tc::smem_u32(smem), 128, 512);
-    const uint64_t db0 = p.b_mn ? tc::make_smem_desc(tc::smem_u32(smem), 2048, 128) : tc::make_smem_desc(tc::smem_u32(smem), 128, 512);
-    const int a_ks = p.a_mn ? 4096 : 256, b_ks = p.b_mn ? 4096 : 256;   // byte advance per K=16 step
-    for (int i = 0; i < n_tiles; ++i) {
-      const int s = i % TSTAGES;
-      mbar_wait_spin(&full[s], (i / TSTAGES) & 1);
-      __syncwarp();
-      tc::fence_after_thread_sync();
-      if (tc::elect_one()) {
-        const uint64_t dsa = da0 + (uint64_t)((s * STAGE_BYTES) >> 4);
-#pragma unroll
-        for (int j = 0; j < NBT; ++j) {
-          if (j >= nb_live) continue;
-          const uint32_t idesc = tc::make_idesc_bf16_f32(TBM, n_eff[j]) | idesc_base;
-          const uint64_t dsb = db0 + (uint64_t)((s * STAGE_BYTES + (1 + j) * TILE_BYTES) >> 4);
-          const uint32_t d = tmem_base + j * TBN;
-#pragma unroll
-          for (int ks = 0; ks < TBK / 16; ++ks) {
-            const uint64_t a_hi = dsa + (uint64_t)((ks * a_ks) >> 4);
-            const uint64_t a_lo = a_hi + (uint64_t)(PLANE_BYTES >> 4);
-            const uint64_t b_hi = dsb + (uint64_t)((ks * b_ks) >> 4);
-            const uint64_t b_lo = b_hi + (uint64_t)(PLANE_BYTES >> 4);
-            if (p.debug_flags & 2) continue;
-            tc::mma_bf16_ss(d, a_lo, b_hi, idesc, (i | ks) != 0);
-            tc::mma_bf16_ss(d, a_hi, b_lo, idesc, true);
-            tc::mma_bf16_ss(d, a_hi, b_hi, idesc, true);
-          }
-        }
-        tc::mma_commit(&empty[s]);
-        if (i + 1 == n_tiles) tc::mma_commit(accum_full);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ================= epilogue: warps 2..9; TMEM lane quarter = warp % 4, column half = (warp - 2) / 4 ==========
-    // tcgen05.ld hands every lane one ROW of the tile; stored like that, each lane would write its own 32-byte piece
-    // of a different cache line (measured: the x*W_ih^T product was bound by those partial-line writes).  So every
-    // warp transposes 32 x 32 blocks through a private 4.5 KB slot of the (now idle) stage buffers and does bias /
-    // activation / Z reads / stores with lane = column: 128 contiguous bytes per row, 4 rows per instruction.
-    mbar_wait_spin(accum_full, 0);
-    __syncwarp();
-    tc::fence_after_thread_sync();
-    const int q = w_u & 3, half = (w_u - 2) >> 2;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    const bool vec_c = ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && (p.ldc % 4 == 0);
-    const bool vec_z = p.Z && ((reinterpret_cast<uintptr_t>(p.Z) & 15) == 0) && (p.ldz % 4 == 0);
-    const bool vec_b = p.bias && ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
-    const int n_tot = (nb_live - 1) * TBN + n_eff[nb_live - 1];     // accumulator columns in use
-    constexpr int HALF_COLS = TBN * NBT / 2, SLD = 36;
-    const int c_begin = half * HALF_COLS, c_end = min(n_tot, c_begin + HALF_COLS);
-    float* stg = reinterpret_cast<float*>(smem) + (w_u - 2) * 32 * SLD;
-    const int cc = lane & 7, rr = lane >> 3;
-    for (int c0 = c_begin; c0 < c_end; c0 += 32) {
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (c0 + 8 * k < c_end) {                                // warp-uniform; c_end is a multiple of 16
-          float v[8];
-          tc::tmem_ld_32x32b_x8(lane_base + (uint32_t)(c0 + 8 * k), v);
-          *reinterpret_cast<float4*>(&stg[lane * SLD + 8 * k]) = make_float4(v[0], v[1], v[2], v[3]);
-          *reinterpret_cast<float4*>(&stg[lane * SLD + 8 * k + 4]) = make_float4(v[4], v[5], v[6], v[7]);
-        }
-      }
-      __syncwarp();
-      const int col = n0 + c0 + cc * 4;
-      const int nv = min(4, p.N - col);                          // <= 0: nothing to write for this lane
-      const bool live = (c0 + cc * 4 < c_end) && nv > 0 && !(p.debug_flags & 4);
-      float bv[4] = {0.f, 0.f, 0.f, 0.f};
-      if (live && p.bias) {
-        if (vec_b && nv == 4) { const float4 t = __ldg(reinterpret_cast<const float4*>(p.bias + col)); bv[0] = t.x; bv[1] = t.y; bv[2] = t.z; bv[3] = t.w; }
-        else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) if (j < nv) bv[j] = __ldg(p.bias + col + j);
-        }
-        if (p.bias2) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) if (j < nv) bv[j] += __ldg(p.bias2 + col + j);
-        }
-      }
-      const bool img = p.c_img_k != nullptr || p.c_img_mn != nullptr;   // kernel-uniform
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int r = it * 4 + rr, row = m0 + q * 32 + r;
-        if (!img && (!live || row >= p.M)) continue;
-        if (img) {
-          // C also leaves as the bf16 hi/lo operand image(s) of the product(s) that consume it next (tile format at the
-          // top of this file): a 16-byte piece = 8 consecutive columns of one row; lanes cc / cc^1 hold its two halves.
-          // Every lane takes part in the shuffles; rows >= M are written as zeros (a reduction index in the MN-major image).
-          const bool ok = live && row < p.M;
-          float v[4] = {0.f, 0.f, 0.f, 0.f};
-          if (ok) {
-            const float4 a = *reinterpret_cast<const float4*>(&stg[r * SLD + cc * 4]);
-            v[0] = a.x + bv[0]; v[1] = a.y + bv[1]; v[2] = a.z + bv[2]; v[3] = a.w + bv[3];
-            if (p.epilogue == EPI_TANH) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) v[j] = tanhf(v[j]);
-            }
-            *reinterpret_cast<float4*>(p.C + (long long)row * p.ldc + col) = make_float4(v[0], v[1], v[2], v[3]);
-          }
-          uint32_t h0, h1, l0, l1;
-          split_pack2(v[0], v[1], h0, l0);
-          split_pack2(v[2], v[3], h1, l1);
-          const uint32_t ph0 = __shfl_xor_sync(0xffffffffu, h0, 1), ph1 = __shfl_xor_sync(0xffffffffu, h1, 1);
-          const uint32_t pl0 = __shfl_xor_sync(0xffffffffu, l0, 1), pl1 = __shfl_xor_sync(0xffffffffu, l1, 1);
-          if ((cc & 1) == 0 && (c0 + cc * 4 < c_end) && col < p.N && row < ((p.M + 31) & ~31)) {
-            const uint4 hi = make_uint4(h0, h1, ph0, ph1), lo = make_uint4(l0, l1, pl0, pl1);
-            if (p.c_img_k && row < p.M) {
-              unsigned char* d = p.c_img_k + ((size_t)(row >> 7) * (p.N >> 5) + (col >> 5)) * TILE_BYTES +
-                                 ((((row & 127) >> 3) * 32) + ((col & 31) >> 3) * 8 + (row & 7)) * 16;
-              *reinterpret_cast<uint4*>(d) = hi;
-              *reinterpret_cast<uint4*>(d + PLANE_BYTES) = lo;
-            }
-            if (p.c_img_mn) {
-              unsigned char* d = p.c_img_mn + ((size_t)(col >> 7) * ((p.M + 31) >> 5) + (row >> 5)) * TILE_BYTES +
-                                 ((((row & 31) >> 3) * 128) + ((col & 127) >> 3) * 8 + (row & 7)) * 16;
-              *reinterpret_cast<uint4*>(d) = hi;
-              *reinterpret_cast<uint4*>(d + PLANE_BYTES) = lo;
-            }
-          }
-          continue;
-        }
-        const float4 a = *reinterpret_cast<const float4*>(&stg[r * SLD + cc * 4]);
-        float v[4] = {a.x + bv[0], a.y + bv[1], a.z + bv[2], a.w + bv[3]};
-        if (p.epilogue == EPI_TANH) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) v[j] = tanhf(v[j]);
-        } else if (p.epilogue == EPI_MUL_DTANH || p.epilogue == EPI_ADD_Z) {
-          const float* z = p.Z + (long long)row * p.ldz + col;
-          float zz[4] = {0.f, 0.f, 0.f, 0.f};
-          if (vec_z && nv == 4) { const float4 t = *reinterpret_cast<const float4*>(z); zz[0] = t.x; zz[1] = t.y; zz[2] = t.z; zz[3] = t.w; }
-          else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) if (j < nv) zz[j] = z[j];
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) v[j] = (p.epilogue == EPI_MUL_DTANH) ? v[j] * (1.f - zz[j] * zz[j]) : v[j] + zz[j];
-        }
-        float* cp = p.C + (long long)row * p.ldc + col;
-        if (p.split_k > 1) {
-          if (vec_c && nv == 4) {
-            asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(cp), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) if (j < nv) atomicAdd(cp + j, v[j]);
-          }
-        } else if (vec_c && nv == 4) {
-          *reinterpret_cast<float4*>(cp) = make_float4(v[0], v[1], v[2], v[3]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) if (j < nv) cp[j] = v[j];
-        }
-      }
-      __syncwarp();
-    }
-    tc::fence_before_thread_sync();
+    return;
   }
-  __syncthreads();
-  if (w_u == 1) { __syncwarp(); tc::tmem_dealloc(tmem_base, TBN * NBT); }
+
+  // ================= consumers: rows [64 (wg - 1), 64 wg) of the tile =================
+  const int half = wg - 1, t = tid & 127;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  // tile image layouts (top of this file): K-major LBO 128 / SBO 512, MN-major LBO 2048 / SBO 128
+  const uint32_t a_lbo = A_MN ? 2048 : 128, a_sbo = A_MN ? 128 : 512;
+  const uint32_t b_lbo = B_MN ? 2048 : 128, b_sbo = B_MN ? 128 : 512;
+  const uint32_t a_ks = A_MN ? 4096 : 256, b_ks = B_MN ? 4096 : 256;     // byte advance per K=16 step
+  const uint32_t a_half = half * 8 * a_sbo;                               // 64 rows = eight 8-row groups
+  const uint32_t smem_base = sm90::smem_u32(smem);
+  for (int i = 0; i < n_tiles; ++i) {
+    const int s = i % STAGES;
+    mbar_wait_spin(&full[s], (i / STAGES) & 1);
+    const uint32_t sa = smem_base + s * STAGE_BYTES + a_half, sb = smem_base + s * STAGE_BYTES + TILE_BYTES;
+    if (!(p.debug_flags & 2)) {
+      sm90::wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < TBK / 16; ++ks) {
+        const uint64_t a_hi = sm90::make_smem_desc(sa + ks * a_ks, a_lbo, a_sbo);
+        const uint64_t a_lo = sm90::make_smem_desc(sa + ks * a_ks + PLANE_BYTES, a_lbo, a_sbo);
+        const uint64_t b_hi = sm90::make_smem_desc(sb + ks * b_ks, b_lbo, b_sbo);
+        const uint64_t b_lo = sm90::make_smem_desc(sb + ks * b_ks + PLANE_BYTES, b_lbo, b_sbo);
+        sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_lo, b_hi);
+        sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_lo);
+        sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_hi);
+      }
+      sm90::wgmma_commit();
+      sm90::wgmma_wait_all();
+    }
+    __syncwarp();
+    if (t == 0) sm90::mbar_arrive(&empty[s]);
+  }
+
+  // ================= epilogue straight from the accumulator fragments =================
+  // fragment j of a thread: rows r and r + 8, columns c, c + 1 with r = 16 (t / 32) + (t % 32) / 4, c = 8 j + 2 (t % 4)
+  const int r_base = m0 + half * 64 + 16 * (t >> 5) + (lane >> 2);
+  const int c_off = 2 * (lane & 3);
+  float* const C = p.C + (long long)blockIdx.z * p.c_split_stride;
+  const bool vec_c = ((reinterpret_cast<uintptr_t>(C) & 7) == 0) && (p.ldc % 2 == 0);
+  const bool img = p.c_img_k != nullptr || p.c_img_mn != nullptr;   // kernel-uniform
+  if (p.debug_flags & 4) return;
+#pragma unroll
+  for (int j = 0; j < TBN / 8; ++j) {
+    const int col = n0 + 8 * j + c_off;
+    const bool c0ok = col < p.N, c1ok = col + 1 < p.N;
+    float b0 = 0.f, b1 = 0.f;
+    if (p.bias) {
+      if (c0ok) b0 = __ldg(p.bias + col) + (p.bias2 ? __ldg(p.bias2 + col) : 0.f);
+      if (c1ok) b1 = __ldg(p.bias + col + 1) + (p.bias2 ? __ldg(p.bias2 + col + 1) : 0.f);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r_base + 8 * h;
+      float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+      if (img) {
+        // C also leaves as the bf16 hi/lo operand image(s) of the product(s) that consume it next: a 16-byte piece = 8
+        // consecutive columns of one row, held by the 4 lanes of a quad.  Every lane takes part in the shuffles; rows
+        // >= M are written as zeros (a reduction index in the MN-major image).
+        const bool ok = row < p.M && c0ok;
+        if (ok) {
+          if (p.epilogue == EPI_TANH) { v0 = tanhf(v0); v1 = tanhf(v1); }
+          *reinterpret_cast<float2*>(p.C + (long long)row * p.ldc + col) = make_float2(v0, v1);   // N % 32 == 0
+        } else {
+          v0 = v1 = 0.f;
+        }
+        uint32_t hw, lw;
+        split_pack2(v0, v1, hw, lw);
+        const int q0 = lane & ~3;
+        const uint4 hi = make_uint4(__shfl_sync(0xffffffffu, hw, q0), __shfl_sync(0xffffffffu, hw, q0 + 1),
+                                    __shfl_sync(0xffffffffu, hw, q0 + 2), __shfl_sync(0xffffffffu, hw, q0 + 3));
+        const uint4 lo = make_uint4(__shfl_sync(0xffffffffu, lw, q0), __shfl_sync(0xffffffffu, lw, q0 + 1),
+                                    __shfl_sync(0xffffffffu, lw, q0 + 2), __shfl_sync(0xffffffffu, lw, q0 + 3));
+        const int cg = n0 + 8 * j;   // first column of the 16-byte piece
+        if ((lane & 3) == 0 && cg < p.N && row < ((p.M + 31) & ~31)) {
+          if (p.c_img_k && row < p.M) {
+            unsigned char* d = p.c_img_k + ((size_t)(row >> 7) * (p.N >> 5) + (cg >> 5)) * TILE_BYTES +
+                               ((((row & 127) >> 3) * 32) + ((cg & 31) >> 3) * 8 + (row & 7)) * 16;
+            *reinterpret_cast<uint4*>(d) = hi;
+            *reinterpret_cast<uint4*>(d + PLANE_BYTES) = lo;
+          }
+          if (p.c_img_mn) {
+            unsigned char* d = p.c_img_mn + ((size_t)(cg >> 7) * ((p.M + 31) >> 5) + (row >> 5)) * TILE_BYTES +
+                               ((((row & 31) >> 3) * 128) + ((cg & 127) >> 3) * 8 + (row & 7)) * 16;
+            *reinterpret_cast<uint4*>(d) = hi;
+            *reinterpret_cast<uint4*>(d + PLANE_BYTES) = lo;
+          }
+        }
+        continue;
+      }
+      if (row >= p.M || !c0ok) continue;
+      if (p.epilogue == EPI_TANH) {
+        v0 = tanhf(v0); v1 = tanhf(v1);
+      } else if (p.epilogue == EPI_MUL_DTANH || p.epilogue == EPI_ADD_Z) {
+        const float* z = p.Z + (long long)row * p.ldz + col;
+        const float z0 = z[0], z1 = c1ok ? z[1] : 0.f;
+        if (p.epilogue == EPI_MUL_DTANH) { v0 *= 1.f - z0 * z0; v1 *= 1.f - z1 * z1; }
+        else { v0 += z0; v1 += z1; }
+      }
+      float* cp = C + (long long)row * p.ldc + col;
+      if (vec_c && c1ok) {
+        *reinterpret_cast<float2*>(cp) = make_float2(v0, v1);
+      } else {
+        cp[0] = v0;
+        if (c1ok) cp[1] = v1;
+      }
+    }
+  }
 }
 
 // grow-only scratch for the packed operand images, one set per (device, stream): kernels of one stream are ordered,
@@ -362,10 +287,10 @@ int launch_pack(const float* src, long long ld, int mn_lim, int k_lim, bool mn_m
 }  // namespace
 
 int gemm_tc_suggest_split_k(int M, int N, int K) {
-  long long tiles = (long long)ceil_div(M, TBM) * (N > TBN ? ceil_div(N, 2 * TBN) : 1);
+  long long tiles = (long long)ceil_div(M, TBM) * ceil_div(N, TBN);
   int k_tiles = ceil_div(K, TBK);
-  if (tiles >= 2 * 148 || k_tiles < 16) return 1;
-  int want = (int)ceil_div_ll(2 * 148, tiles);
+  if (tiles >= num_sms() || k_tiles < 16) return 1;
+  int want = (int)ceil_div_ll(2 * num_sms(), tiles);
   int max_by_k = k_tiles / 8;
   int s = want < max_by_k ? want : max_by_k;
   if (s < 1) s = 1;
@@ -373,16 +298,26 @@ int gemm_tc_suggest_split_k(int M, int N, int K) {
   return s;
 }
 
-int gemm_f32_tc(const GemmParams& p, GemmLayout layout, cudaStream_t stream) {
+template <bool A_MN, bool B_MN>
+int launch_packed(const PackedGemmParams& q, int m_tiles, int n_tiles, int slices, cudaStream_t stream) {
   static PerDeviceOnce once;
   if (once.need()) {
-    R2D2_CUDA_TRY(cudaFuncSetAttribute(gemm_packed_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, PackedCfg<1>::SMEM));
-    R2D2_CUDA_TRY(cudaFuncSetAttribute(gemm_packed_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, PackedCfg<2>::SMEM));
+    R2D2_CUDA_TRY(cudaFuncSetAttribute(gemm_packed_kernel<A_MN, B_MN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       PACKED_SMEM));
   }
+  dim3 grid(n_tiles, m_tiles, slices);
+  gemm_packed_kernel<A_MN, B_MN><<<grid, PACKED_GEMM_THREADS, PACKED_SMEM, stream>>>(q);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return R2D2_OK;
+}
+
+int gemm_f32_tc(const GemmParams& p, GemmLayout layout, cudaStream_t stream) {
   const bool a_mn = (layout == GEMM_TN), b_mn = (layout != GEMM_NT);
   const int m_tiles = ceil_div(p.M, TBM), n_tiles = ceil_div(p.N, TBN);
   const int kt1 = ceil_div(p.K, TBK), kt2 = p.K2 > 0 ? ceil_div(p.K2, TBK) : 0;
   const int k_tiles = kt1 + kt2;
+  R2D2_REQUIRE(m_tiles <= 65535, "M too large for grid.y");
   StreamScratch* sc = nullptr;
   R2D2_TRY(scratch_for(stream, &sc));
   Scratch& g_pack_a = sc->a;
@@ -406,27 +341,25 @@ int gemm_f32_tc(const GemmParams& p, GemmLayout layout, cudaStream_t stream) {
   PackedGemmParams q;
   q.pa = p.A_img ? p.A_img : g_pack_a.ptr; q.pb = p.B_img ? p.B_img : g_pack_b.ptr; q.k_tiles = k_tiles; q.C = p.C; q.ldc = p.ldc; q.M = p.M; q.N = p.N;
   q.bias = p.bias; q.bias2 = p.bias ? p.bias2 : nullptr; q.Z = p.Z; q.ldz = p.ldz; q.epilogue = p.epilogue; q.split_k = p.split_k;
-  q.a_mn = a_mn; q.b_mn = b_mn; q.debug_flags = p.debug_flags;
+  q.debug_flags = p.debug_flags;
   q.c_img_k = p.C_img_k; q.c_img_mn = p.C_img_mn;
+  q.c_split_stride = 0;
+  int slices = 1;
+  if (p.split_k > 1) {   // partial products into slices, then added into C in slice order (same bits every run)
+    slices = ceil_div(k_tiles, ceil_div(k_tiles, p.split_k));   // every slice z < slices owns at least one k tile
+    R2D2_TRY(partials_scratch((size_t)slices * p.M * p.N, stream, &q.C));
+    q.ldc = p.N;
+    q.c_split_stride = (long long)p.M * p.N;
+  }
   if (p.C_img_k || p.C_img_mn) {
     R2D2_REQUIRE(p.N % 32 == 0 && p.split_k == 1 && (p.epilogue == EPI_NONE || p.epilogue == EPI_TANH) &&
-                     (reinterpret_cast<uintptr_t>(p.C) & 15) == 0 && p.ldc % 4 == 0,
-                 "operand image from the tcgen05 epilogue: N % 32 == 0, no split-K, bias / tanh epilogue, 16-byte aligned C");
+                     (reinterpret_cast<uintptr_t>(p.C) & 7) == 0 && p.ldc % 2 == 0,
+                 "operand image from the wgmma epilogue: N % 32 == 0, no split-K, bias / tanh epilogue, 8-byte aligned C");
   }
-  static int force_nbt = -1;
-  if (force_nbt < 0) { const char* e = getenv("R2D2_GEMM_NBT"); force_nbt = e ? atoi(e) : 0; }
-  // two B tiles per CTA when the A images would otherwise be re-read many times (N >= 512) or the CTA count is set by
-  // split-K anyway; a 256-wide product with a long K keeps 128-wide tiles (twice the CTAs: measured 52 vs 58 us)
-  const bool wide = n_tiles > 1 && (n_tiles >= 4 || p.split_k > 1);
-  if ((wide && force_nbt != 1) || (n_tiles > 1 && force_nbt == 2)) {
-    dim3 grid(ceil_div(n_tiles, 2), m_tiles, p.split_k);
-    gemm_packed_kernel<2><<<grid, PACKED_GEMM_THREADS, PackedCfg<2>::SMEM, stream>>>(q);
-  } else {
-    dim3 grid(n_tiles, m_tiles, p.split_k);
-    gemm_packed_kernel<1><<<grid, PACKED_GEMM_THREADS, PackedCfg<1>::SMEM, stream>>>(q);
-  }
-  count_launch();
-  R2D2_CUDA_TRY(cudaGetLastError());
+  if (a_mn) R2D2_TRY((launch_packed<true, true>(q, m_tiles, n_tiles, slices, stream)));      // TN
+  else if (b_mn) R2D2_TRY((launch_packed<false, true>(q, m_tiles, n_tiles, slices, stream)));   // NN
+  else R2D2_TRY((launch_packed<false, false>(q, m_tiles, n_tiles, slices, stream)));          // NT
+  if (p.split_k > 1) return add_partials(q.C, slices, p.M, p.N, p.C, p.ldc, nullptr, stream);
   return R2D2_OK;
 }
 

@@ -2,21 +2,22 @@
 //
 // A third of the GEMM launches of one iteration have a dimension of 6..23 (obs / action widths, models.py:17-19,
 // :62-64): x*W1^T (K = 17 | 17+6), the heads (N = 6), their dgrads and the dW1 / dW3 blocks.  On a 128-wide tensor
-// core tile they are >90% padding and ran at 16-36 us each (profiles/r01_summary.md) although they only stream
-// 2-32 MB.  Here every one is a single HBM-bound pass in exact fp32:
+// core tile they are >90% padding although they only stream 2-32 MB.  Here every one is a single HBM-bound pass in
+// exact fp32:
 //   thin_smallk : C[M,N] = epi(A[M,K] W (+ A2[M,K2] W2) + bias),  K + K2 <= 32   (NT / NN)
 //   thin_smalln : C[M,N] = epi(A[M,K] W + bias),                  N <= 32        (NT / NN)
 //   thin_tn     : C[M,N] += A[K,M]^T B[K,N],                      M <= 32 or N <= 32, reduction over K rows
+#include "elementwise.cuh"
 #include "gemm.cuh"
 
 #include <stdlib.h>
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 namespace r2d2 {
 namespace {
 
 __device__ __forceinline__ float apply_epilogue(float v, int epilogue, float z) {
-  if (epilogue == EPI_TANH) return tc::tanh_fast(v);
+  if (epilogue == EPI_TANH) return sm90::tanh_fast(v);
   if (epilogue == EPI_MUL_DTANH) return v * (1.f - z * z);
   if (epilogue == EPI_ADD_Z) return v + z;
   return v;
@@ -263,8 +264,7 @@ __global__ void __launch_bounds__(SN_THREADS) thin_smalln_kernel(GemmParams p, i
 // ------------------------------------------------------------------------------------------------
 // Small-N products whose K is 128 / 256 / 512 (the heads at H = 128..512: N = 1..32 outputs per row).  The kernel
 // above keeps 32 accumulators per lane and re-reads the whole [NP][K] weight tile from shared memory for every ROW
-// (64 KB of shared-memory traffic per row at K = 512: it ran at the shared-memory roof, 104 us for the 64000 x 17 x 512
-// head of cfg-3).  Here a warp owns FOUR rows: lane = 8 * row + j, lane j of a row loads the 16-byte pieces
+// (64 KB of shared-memory traffic per row at K = 512: it runs at the shared-memory roof).  Here a warp owns FOUR rows: lane = 8 * row + j, lane j of a row loads the 16-byte pieces
 // j, j + 8, j + 16, ... of that row (the 8 lanes of a row read 128 contiguous bytes per instruction, 4 full lines per
 // warp instruction) and keeps them in registers; for every output column the 8 lanes of a row multiply their pieces
 // with the matching weight pieces (shared memory: 8 distinct 16-byte addresses per instruction, broadcast over the
@@ -313,7 +313,7 @@ __global__ void __launch_bounds__(256) thin_rowdot_kernel(GemmParams p) {
 
 // Second version: the kernel above is bound by the shared-memory pipe - a 128-bit shared load is served one quarter
 // warp per clock and every quarter (= one row) re-reads the same 8 weight pieces, so the [N][K] tile crosses the pipe once
-// per ROW (69 groups x 17 columns x 16 loads x 4 clocks = 75 k clocks = 40 us per SM of the 70 us at cfg-3).  Here all 32
+// per ROW (69 groups x 17 columns x 16 loads x 4 clocks = 75 k clocks per SM at cfg-3).  Here all 32
 // lanes share one k-slice layout (lane j holds the 16-byte pieces j, j + 32, ... of each of the warp's FOUR rows), so a
 // weight load feeds four rows: the tile crosses the pipe once per four rows.  The 4 x 32 partial sums are reduced with a
 // transposing butterfly: 2 + 1 exchanges halve the rows per lane, 3 more add the 8 lanes of a row (6 shuffles per column).
@@ -398,7 +398,7 @@ int launch_thin_rowdot(const GemmParams& p, cudaStream_t stream) {
   }
   const int groups = ceil_div(p.M, 4);
   int grid = ceil_div(groups, 8);
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > num_sms() * 4) grid = num_sms() * 4;
   if (v1) thin_rowdot_kernel<NN, KI><<<grid, 256, smem, stream>>>(p);
   else thin_rowdot4_kernel<NN, KI><<<grid, 256, smem, stream>>>(p);
   count_launch();
@@ -409,16 +409,17 @@ int launch_thin_rowdot(const GemmParams& p, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------------
 // TN with one small output dimension: X[K rows][P] is the wide operand (thread = one of its columns), Y[K rows][Q<=32]
 // the narrow one (staged per 32-row chunk in shared memory, read as broadcast float4).  X rows are fetched sixteen at a
-// time (the kernel is latency bound otherwise).  Accumulates into C with atomics once per block (split-K contract
-// of gemm_f32: C pre-zeroed by the caller); the block result goes through shared memory so that the atomics walk C
-// in address order whichever side is the narrow one.
+// time (the kernel is latency bound otherwise).  Block column x writes its partial product as slice x of a dense
+// C-shaped buffer (the block result goes through shared memory so that the stores walk C in address order whichever
+// side is the narrow one); the launcher adds the slices into C in order (split-K contract of gemm_f32: C += A^T B).
+// The optional column sums leave the same way: slice x of [P] (X) and of [Q] (Y, blocks with y == 0 only).
 // ------------------------------------------------------------------------------------------------
 constexpr int TN_THREADS = 256, TN_CHUNK = 32, TN_BATCH = 16;
 
 template <int QP>
 __global__ void __launch_bounds__(TN_THREADS) thin_tn_kernel(const float* __restrict__ X, long long ldx, int P,
                                                              const float* __restrict__ Y, long long ldy, int Q, int K,
-                                                             float* __restrict__ C, long long ldc, int small_is_m,
+                                                             float* __restrict__ C_part, int small_is_m,
                                                              float* __restrict__ colsum_x, float* __restrict__ colsum_y) {
   __shared__ __align__(16) float Ys[TN_CHUNK][QP];
   __shared__ float Out[TN_THREADS][QP + 1];
@@ -462,8 +463,9 @@ __global__ void __launch_bounds__(TN_THREADS) thin_tn_kernel(const float* __rest
       }
     }
   }
-  if (colsum_x && pon) atomicAdd(colsum_x + pc, xsum);
-  if (do_ysum) atomicAdd(colsum_y + tid, ysum);
+  if (colsum_x && pon) colsum_x[(size_t)blockIdx.x * P + pc] = xsum;
+  if (do_ysum) colsum_y[(size_t)blockIdx.x * Q + tid] = ysum;
+  float* const C = C_part + (size_t)blockIdx.x * P * Q;   // dense slice: [Q][P] or [P][Q]
 #pragma unroll
   for (int q = 0; q < QP; ++q) Out[tid][q] = acc[q];
   __syncthreads();
@@ -471,12 +473,12 @@ __global__ void __launch_bounds__(TN_THREADS) thin_tn_kernel(const float* __rest
   if (small_is_m) {   // C[q][p]: p fastest
     for (int idx = tid; idx < Q * pn; idx += TN_THREADS) {
       const int q = idx / pn, pp = idx % pn;
-      atomicAdd(C + (long long)q * ldc + p0 + pp, Out[pp][q]);
+      C[(long long)q * P + p0 + pp] = Out[pp][q];
     }
   } else {            // C[p][q]: q fastest
     for (int idx = tid; idx < pn * Q; idx += TN_THREADS) {
       const int pp = idx / Q, q = idx % Q;
-      atomicAdd(C + (long long)(p0 + pp) * ldc + q, Out[pp][q]);
+      C[(long long)(p0 + pp) * Q + q] = Out[pp][q];
     }
   }
 }
@@ -489,13 +491,22 @@ template <int QP>
 int launch_thin_tn(const float* X, long long ldx, int P, const float* Y, long long ldy, int Q, int K, float* C,
                    long long ldc, int small_is_m, float* colsum_x, float* colsum_y, cudaStream_t stream) {
   const int chunks = ceil_div(K, TN_CHUNK), py = ceil_div(P, TN_THREADS);
-  int gx = 888 / py;                                   // ~6 resident blocks per SM
+  int gx = 6 * num_sms() / py;                         // ~6 resident blocks per SM
   if (gx < 1) gx = 1;
   if (gx > chunks) gx = chunks;
   gx = ceil_div(chunks, ceil_div(chunks, gx));         // equal number of chunks per block
-  thin_tn_kernel<QP><<<dim3(gx, py), TN_THREADS, 0, stream>>>(X, ldx, P, Y, ldy, Q, K, C, ldc, small_is_m, colsum_x, colsum_y);
+  const size_t c_floats = (size_t)gx * P * Q, x_floats = colsum_x ? (size_t)gx * P : 0, y_floats = colsum_y ? (size_t)gx * Q : 0;
+  float* part = nullptr;
+  R2D2_TRY(partials_scratch(c_floats + x_floats + y_floats, stream, &part));
+  float* part_x = colsum_x ? part + c_floats : nullptr;
+  float* part_y = colsum_y ? part + c_floats + x_floats : nullptr;
+  thin_tn_kernel<QP><<<dim3(gx, py), TN_THREADS, 0, stream>>>(X, ldx, P, Y, ldy, Q, K, part, small_is_m, part_x, part_y);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
+  if (small_is_m) R2D2_TRY(add_partials(part, gx, Q, P, C, ldc, nullptr, stream));
+  else R2D2_TRY(add_partials(part, gx, P, Q, C, ldc, nullptr, stream));
+  if (colsum_x) R2D2_TRY(add_partials(part_x, gx, 1, P, colsum_x, P, nullptr, stream));
+  if (colsum_y) R2D2_TRY(add_partials(part_y, gx, 1, Q, colsum_y, Q, nullptr, stream));
   return R2D2_OK;
 }
 
@@ -507,7 +518,7 @@ int launch_thin_smalln(const GemmParams& p, cudaStream_t stream) {
     R2D2_CUDA_TRY(cudaFuncSetAttribute(thin_smalln_kernel<NN, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int groups = ceil_div(p.M, 32 / NP);
   int grid = ceil_div(groups, SN_THREADS / 32);
-  if (grid > 148 * 6) grid = 148 * 6;
+  if (grid > num_sms() * 6) grid = num_sms() * 6;
   thin_smalln_kernel<NN, NP><<<grid, SN_THREADS, smem, stream>>>(p, kpad);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
@@ -555,7 +566,7 @@ int gemm_thin_try(const GemmParams& p, GemmLayout layout, cudaStream_t stream, b
     R2D2_REQUIRE(!(p.C_img_k || p.C_img_mn) || (p.N % 32 == 0), "operand image needs N % 32 == 0");
     *handled = true;
     const int row_tiles = ceil_div(p.M, SK_ROWS), ny = ceil_div(p.N, SK_COLS);
-    int gx = 444 / ny;                                 // 3 resident blocks per SM (registers)
+    int gx = 3 * num_sms() / ny;                       // 3 resident blocks per SM (registers)
     if (gx < 1) gx = 1;
     if (gx > row_tiles) gx = row_tiles;                // tiles go round-robin over the resident blocks: SM loads differ by <= 1 tile
     const int vec_c = aligned16(p.C, p.ldc) ? 1 : 0, vec_z = aligned16(p.Z, p.ldz) ? 1 : 0;

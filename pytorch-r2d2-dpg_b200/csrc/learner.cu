@@ -71,8 +71,6 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
   l->ws_c2 = ChainWs::carve(take(ws_c2), l->critic_sh, L, B, 1);
   l->ws_ta.inference_only = true;  // target nets: no BPTT, the scan keeps only what the heads read (learner.py:94-95,106)
   l->ws_tc.inference_only = true;
-  l->ws_c1.keep_z1_image = true;   // chains whose weights get gradients: the l1 kernel also leaves z1 as the B operand of dW_ih
-  l->ws_a1.keep_z1_image = true;
   {   // R2D2_OVERLAP_INPUTS=0 disables the side stream (A/B)
     const char* e = getenv("R2D2_OVERLAP_INPUTS");
     l->overlap_inputs = !(e && e[0] == '0');
@@ -137,7 +135,7 @@ int learner_target_phase(Learner* l, int slot, cudaStream_t st) {
   R2D2_TRY(net_forward_inputs(l->actor_sh, Pa_t, l->ws_ta, b.obs, nullptr, Tt, B, st));
   if (l->overlap_inputs) {
     // fork: input projections that need the batch and weights nothing in this phase changes are issued on a
-    // low-priority side stream right where the first persistent scan starts: the scans occupy 7 x 16 of the 148 SMs
+    // low-priority side stream right where the first persistent scan starts: the scans occupy whole clusters of SMs
     // and the projections take the rest.  Same slot: the online critic chain of this batch (stored actions).  The
     // actor's DPG chain of the iteration in flight: when its weights are final - always when running ahead (the caller
     // completes the previous optimiser step first), else unless the caller defers that step (overlap_actor_inputs).

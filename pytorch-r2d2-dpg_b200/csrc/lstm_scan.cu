@@ -1,8 +1,11 @@
-// Persistent LSTM scan kernels (forward + BPTT) for sm_100a.
+// Persistent LSTM scan kernels (forward + BPTT) for sm_90a.
 //
-// Decomposition (H in {32,64,128,256}):  a thread-block cluster of C = H/32 CTAs owns NB batch
+// Decomposition (H in {32,64,128,256,512}):  a thread-block cluster of C = H/32 CTAs owns NB batch
 // rows for the whole chain.  CTA `rank` owns hidden units [32*rank, 32*rank+32): its 128 gate rows of
-// W_hh stay resident in REGISTERS as bf16 hi/lo MMA fragments for the whole launch (loaded once);
+// W_hh stay resident as bf16 hi/lo MMA fragments for the whole launch (loaded once) - in REGISTERS up to H = 256;
+// at H = 512 (cluster of 16, non-portable size) the slice is 256 KB, more than the register file or the 227 KB of
+// shared memory of one CTA, so the lo plane stays in registers and the hi plane lives in shared memory in fragment
+// order (one conflict-free 16-byte load per thread and k-step);
 // per step the only traffic is the h_t all-gather inside the cluster through distributed shared
 // memory plus one hardware cluster barrier.  Batch is split across clusters (grid = C * ceil(B/NB)).
 //   forward : D[gate rows(128) x NB] = W_slice[128 x H] * h_{s-1}^T           (swap-AB: M = gate rows)
@@ -31,18 +34,24 @@ __device__ __forceinline__ float accurate_sigmoid(float x) { return 1.0f / (1.0f
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
+// W_hh hi plane in shared memory (H = 512): the register file cannot hold both planes of a 128 x 512 slice
+template <int H> __host__ __device__ constexpr bool w_hi_in_smem() { return H > 256; }
+
 template <int H, int NB>
 struct FwdSmem {
   static constexpr int HLD = H + 8;                        // bf16 row stride of the h operand tile
+  static constexpr int W_BYTES = w_hi_in_smem<H>() ? (H / 16) * 8 * 32 * 16 : 0;   // hi fragments [ks][warp][lane][16 B]
   static constexpr int HB_ELEMS = 2 * 2 * NB * HLD;        // [buf][plane][n][k]
   static constexpr int GT_ELEMS = NB * GT_LD;              // fp32
   static constexpr int HS_ELEMS = 2 * NB * UNITS_PER_CTA;  // bf16 staging [plane][n][unit]
-  static constexpr int BYTES = HB_ELEMS * 2 + GT_ELEMS * 4 + HS_ELEMS * 2;
+  static constexpr int BYTES = W_BYTES + HB_ELEMS * 2 + GT_ELEMS * 4 + HS_ELEMS * 2;
+  static_assert(BYTES <= 232448, "forward scan tile does not fit in 227 KB of shared memory");
 };
 
 template <int H, int NB>
 __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdParams p) {
   constexpr int C = H / 32, KS = H / 16, NT = NB / 8;
+  constexpr bool WS = w_hi_in_smem<H>();
   using SM = FwdSmem<H, NB>;
   constexpr int HLD = SM::HLD;
   cg::cluster_group cluster = cg::this_cluster();
@@ -53,12 +62,13 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
   const int B = p.B, S = p.T * p.repeat;
 
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  __nv_bfloat16* hb = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  float* gt = reinterpret_cast<float*>(smem_raw + SM::HB_ELEMS * 2);
-  __nv_bfloat16* hstage = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::HB_ELEMS * 2 + SM::GT_ELEMS * 4);
+  uint4* w_hi_s = reinterpret_cast<uint4*>(smem_raw);   // H = 512 only
+  __nv_bfloat16* hb = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES);
+  float* gt = reinterpret_cast<float*>(smem_raw + SM::W_BYTES + SM::HB_ELEMS * 2);
+  __nv_bfloat16* hstage = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES + SM::HB_ELEMS * 2 + SM::GT_ELEMS * 4);
 
-  // ---- W_hh slice -> register-resident A fragments (rows: local r = gate*32 + unit; warp w owns r in [16w,16w+16))
-  uint32_t a_hi[KS][4], a_lo[KS][4];
+  // ---- W_hh slice -> resident A fragments (rows: local r = gate*32 + unit; warp w owns r in [16w,16w+16))
+  uint32_t a_hi[WS ? 1 : KS][4], a_lo[KS][4];
   {
     const int gate = w >> 1;
     const int u_lo = (w & 1) * 16 + g;  // local unit of fragment row g; row g+8 -> unit u_lo+8
@@ -71,10 +81,17 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
       float2 v1 = __ldg(reinterpret_cast<const float2*>(w_r1 + k));
       float2 v2 = __ldg(reinterpret_cast<const float2*>(w_r0 + k + 8));
       float2 v3 = __ldg(reinterpret_cast<const float2*>(w_r1 + k + 8));
-      split_pack2(v0.x, v0.y, a_hi[ks][0], a_lo[ks][0]);
-      split_pack2(v1.x, v1.y, a_hi[ks][1], a_lo[ks][1]);
-      split_pack2(v2.x, v2.y, a_hi[ks][2], a_lo[ks][2]);
-      split_pack2(v3.x, v3.y, a_hi[ks][3], a_lo[ks][3]);
+      uint32_t h[4];
+      split_pack2(v0.x, v0.y, h[0], a_lo[ks][0]);
+      split_pack2(v1.x, v1.y, h[1], a_lo[ks][1]);
+      split_pack2(v2.x, v2.y, h[2], a_lo[ks][2]);
+      split_pack2(v3.x, v3.y, h[3], a_lo[ks][3]);
+      if constexpr (WS) {
+        w_hi_s[(ks * 8 + w) * 32 + lane] = make_uint4(h[0], h[1], h[2], h[3]);
+      } else {
+#pragma unroll
+        for (int f = 0; f < 4; ++f) a_hi[ks][f] = h[f];
+      }
     }
   }
 
@@ -129,6 +146,14 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
     const __nv_bfloat16* hb_lo = hb + (cur * 2 + 1) * NB * HLD;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
+      uint32_t ah[4];
+      if constexpr (WS) {
+        const uint4 v = w_hi_s[(ks * 8 + w) * 32 + lane];
+        ah[0] = v.x; ah[1] = v.y; ah[2] = v.z; ah[3] = v.w;
+      } else {
+#pragma unroll
+        for (int f = 0; f < 4; ++f) ah[f] = a_hi[ks][f];
+      }
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
         const int off = (nt * 8 + g) * HLD + ks * 16 + 2 * c;
@@ -138,8 +163,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
         bl[0] = *reinterpret_cast<const uint32_t*>(hb_lo + off);
         bl[1] = *reinterpret_cast<const uint32_t*>(hb_lo + off + 8);
         mma_bf16_16816(acc[nt], a_lo[ks], bh);
-        mma_bf16_16816(acc[nt], a_hi[ks], bl);
-        mma_bf16_16816(acc[nt], a_hi[ks], bh);
+        mma_bf16_16816(acc[nt], ah, bl);
+        mma_bf16_16816(acc[nt], ah, bh);
       }
     }
     // fragment -> gate tile gt[n][local row]
@@ -167,10 +192,12 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
         const float cn = fg * cst[e] + ig * gg;
         const float hn = og * tanhf(cn);
         cst[e] = cn;
-        float* go = p.gates + ((size_t)s * B + b) * gstride + ug;
-        go[0] = ig; go[H] = fg; go[2 * H] = gg; go[3 * H] = og;
+        if (!p.no_save) {   // gates and c are read by the BPTT only
+          float* go = p.gates + ((size_t)s * B + b) * gstride + ug;
+          go[0] = ig; go[H] = fg; go[2 * H] = gg; go[3 * H] = og;
+          p.cs[((size_t)(s + 1) * B + b) * H + ug] = cn;
+        }
         p.hs[((size_t)(s + 1) * B + b) * H + ug] = hn;
-        p.cs[((size_t)(s + 1) * B + b) * H + ug] = cn;
         if (p.head_in && (s % p.repeat) == p.repeat - 1)
           p.head_in[((size_t)t * B + b) * H + ug] = tanhf(hn);
         split_bf16(hn, hi, lo);
@@ -205,7 +232,10 @@ struct BwdSmem {
   static constexpr int DG_ELEMS = 2 * NB * DG_LD;               // bf16 [plane][n][local gate row]
   static constexpr int PS_LD = NB + 2;                          // 2-way instead of 16-way bank conflicts on the unit-strided reads
   static constexpr int PS_ELEMS = 2 * C * UNITS_PER_CTA * PS_LD; // fp32 [buf][src rank][unit][n]
-  static constexpr int BYTES = DG_ELEMS * 2 + PS_ELEMS * 4;
+  static constexpr int MT = (H / 16 + 7) / 8;
+  static constexpr int W_BYTES = w_hi_in_smem<H>() ? MT * 8 * 8 * 32 * 16 : 0;   // hi fragments [i][ks][warp][lane][16 B]
+  static constexpr int BYTES = W_BYTES + DG_ELEMS * 2 + PS_ELEMS * 4;
+  static_assert(BYTES <= 232448, "BPTT scan tile does not fit in 227 KB of shared memory");
 };
 
 template <int H, int NB>
@@ -214,6 +244,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
   constexpr int M_TILES = H / 16;
   constexpr int MT = (M_TILES + 7) / 8;  // m-tiles per warp
   constexpr int KS = ROWS_PER_CTA / 16;  // 8
+  constexpr bool WS = w_hi_in_smem<H>();
   using SM = BwdSmem<H, NB>;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
@@ -223,16 +254,18 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
   const int B = p.B, S = p.T * p.repeat;
 
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  __nv_bfloat16* dgs = reinterpret_cast<__nv_bfloat16*>(smem_raw);
-  float* ps = reinterpret_cast<float*>(smem_raw + SM::DG_ELEMS * 2);
+  uint4* w_hi_s = reinterpret_cast<uint4*>(smem_raw);   // H = 512 only
+  __nv_bfloat16* dgs = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES);
+  float* ps = reinterpret_cast<float*>(smem_raw + SM::W_BYTES + SM::DG_ELEMS * 2);
 
   // ---- W_hh slice (transposed use): A(m = j output unit, k = local gate row r) = W_hh[grow(r)][j]
-  uint32_t a_hi[MT][KS][4], a_lo[MT][KS][4];
+  uint32_t a_hi[WS ? 1 : MT][WS ? 1 : KS][4], a_lo[MT][KS][4];
 #pragma unroll
   for (int i = 0; i < MT; ++i) {
     const int mi = w * MT + i;
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
+      uint32_t h[4];
 #pragma unroll
       for (int f = 0; f < 4; ++f) {
         float v0 = 0.f, v1 = 0.f;
@@ -243,11 +276,18 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
           v0 = __ldg(p.whh + row0 * H + j);
           v1 = __ldg(p.whh + (row0 + 1) * H + j);  // r even -> r+1 stays in the same gate block
         }
-        split_pack2(v0, v1, a_hi[i][ks][f], a_lo[i][ks][f]);
+        split_pack2(v0, v1, h[f], a_lo[i][ks][f]);
+      }
+      if constexpr (WS) {
+        w_hi_s[((i * KS + ks) * 8 + w) * 32 + lane] = make_uint4(h[0], h[1], h[2], h[3]);
+      } else {
+#pragma unroll
+        for (int f = 0; f < 4; ++f) a_hi[i][ks][f] = h[f];
       }
     }
   }
 
+  __syncthreads();   // W_hh hi fragments in shared memory (H = 512) before the first MMA
   const int ug = rank * 32 + lane;
   const size_t gstride = (size_t)4 * H;
   float dcn[NT], keep[NT][4];
@@ -323,19 +363,30 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
       const __nv_bfloat16* d_lo = dgs + NB * DG_LD;
 #pragma unroll
       for (int ks = 0; ks < KS; ++ks) {
+        uint32_t bh[NT][2], bl[NT][2];
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) {
           const int off = (nt * 8 + g) * DG_LD + ks * 16 + 2 * c;
-          uint32_t bh[2], bl[2];
-          bh[0] = *reinterpret_cast<const uint32_t*>(d_hi + off);
-          bh[1] = *reinterpret_cast<const uint32_t*>(d_hi + off + 8);
-          bl[0] = *reinterpret_cast<const uint32_t*>(d_lo + off);
-          bl[1] = *reinterpret_cast<const uint32_t*>(d_lo + off + 8);
+          bh[nt][0] = *reinterpret_cast<const uint32_t*>(d_hi + off);
+          bh[nt][1] = *reinterpret_cast<const uint32_t*>(d_hi + off + 8);
+          bl[nt][0] = *reinterpret_cast<const uint32_t*>(d_lo + off);
+          bl[nt][1] = *reinterpret_cast<const uint32_t*>(d_lo + off + 8);
+        }
 #pragma unroll
-          for (int i = 0; i < MT; ++i) {
-            mma_bf16_16816(acc[i][nt], a_lo[i][ks], bh);
-            mma_bf16_16816(acc[i][nt], a_hi[i][ks], bl);
-            mma_bf16_16816(acc[i][nt], a_hi[i][ks], bh);
+        for (int i = 0; i < MT; ++i) {
+          uint32_t ah[4];
+          if constexpr (WS) {
+            const uint4 v = w_hi_s[((i * KS + ks) * 8 + w) * 32 + lane];
+            ah[0] = v.x; ah[1] = v.y; ah[2] = v.z; ah[3] = v.w;
+          } else {
+#pragma unroll
+            for (int f = 0; f < 4; ++f) ah[f] = a_hi[i][ks][f];
+          }
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) {
+            mma_bf16_16816(acc[i][nt], a_lo[i][ks], bh[nt]);
+            mma_bf16_16816(acc[i][nt], ah, bl[nt]);
+            mma_bf16_16816(acc[i][nt], ah, bh[nt]);
           }
         }
       }
@@ -362,8 +413,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
 }
 
 // ------------------------------------------------------------------------------------------------
-// generic path (any H): one GEMM + one pointwise kernel per step.  Correct for every size; used
-// only when the cluster kernels do not cover H (e.g. H = 512 until its kernel lands).
+// per-step path (any H): one GEMM + one pointwise kernel per step.  Correct for every size; used when the cluster
+// kernels do not cover H (H not a multiple of 32 in 32..512) and as the A/B reference (lstm_scan_set_impl(0)).
 // ------------------------------------------------------------------------------------------------
 __global__ void lstm_cell_fwd_pointwise(const float* __restrict__ gpre, const float* __restrict__ c_prev,
                                         float* __restrict__ gates, float* __restrict__ h_out,
@@ -476,91 +527,131 @@ int scan_backward_generic(const ScanBwdParams& p, cudaStream_t stream) {
   return R2D2_OK;
 }
 
-template <typename Kern, typename Params>
-int launch_cluster(Kern kern, const Params& p, int cluster_size, int n_clusters, int smem_bytes, cudaStream_t stream) {
+template <typename Kern>
+int set_cluster_attributes(Kern kern, int cluster_size, int smem_bytes) {
   R2D2_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+  if (cluster_size > 8) R2D2_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  return R2D2_OK;
+}
+
+cudaLaunchConfig_t cluster_config(int cluster_size, int n_clusters, int smem_bytes, cudaStream_t stream,
+                                  cudaLaunchAttribute* attr) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(cluster_size * n_clusters);
   cfg.blockDim = dim3(SCAN_THREADS);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = cluster_size;
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  return cfg;
+}
+
+template <typename Kern, typename Params>
+int launch_cluster(Kern kern, const Params& p, int cluster_size, int n_clusters, int smem_bytes, cudaStream_t stream) {
+  R2D2_TRY(set_cluster_attributes(kern, cluster_size, smem_bytes));
+  cudaLaunchAttribute attr[1];
+  cudaLaunchConfig_t cfg = cluster_config(cluster_size, n_clusters, smem_bytes, stream, attr);
   R2D2_CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, p));
   count_launch();
   return R2D2_OK;
 }
 
-// batch columns per cluster: the smallest tile that still fits one wave of clusters (per-step cost is
-// dominated by fixed latencies, so more, narrower clusters win as long as they are co-resident)
-int pick_nb(int B, int H) {
-  const int avail = 148 / (H / 32);
-  const int opts[3] = {8, 16, 32};
-  for (int i = 0; i < 3; ++i)
-    if (ceil_div(B, opts[i]) <= avail) return opts[i];
-  return 32;
+// clusters of this kernel the device keeps resident at once (GPC geometry decides, not the SM count alone)
+template <typename Kern>
+int resident_clusters(Kern kern, int cluster_size, int smem_bytes, int* out) {
+  R2D2_TRY(set_cluster_attributes(kern, cluster_size, smem_bytes));
+  cudaLaunchAttribute attr[1];
+  cudaLaunchConfig_t cfg = cluster_config(cluster_size, 1, smem_bytes, nullptr, attr);
+  R2D2_CUDA_TRY(cudaOccupancyMaxActiveClusters(out, kern, &cfg));
+  return R2D2_OK;
+}
+
+// Batch columns per cluster: the smallest tile whose clusters are all resident in one wave (per-step cost is
+// dominated by fixed latencies, so more, narrower clusters win as long as they are co-resident); the widest tile
+// that fits in shared memory otherwise (32 rows up to H = 256, 16 at H = 512).
+template <int H, typename K8, typename K16, typename K32>
+int pick_nb(int B, K8 k8, int smem8, K16 k16, int smem16, K32 k32, int smem32, int* nb) {
+  int fit = 0;
+  R2D2_TRY(resident_clusters(k8, H / 32, smem8, &fit));
+  if (ceil_div(B, 8) <= fit) { *nb = 8; return R2D2_OK; }
+  R2D2_TRY(resident_clusters(k16, H / 32, smem16, &fit));
+  if (ceil_div(B, 16) <= fit || !k32) { *nb = 16; return R2D2_OK; }
+  *nb = 32;
+  (void)smem32;
+  return R2D2_OK;
 }
 
 template <int H>
 int fwd_dispatch(const ScanFwdParams& p, cudaStream_t stream) {
-  const int nb = pick_nb(p.B, H);
+  constexpr bool WIDE = !w_hi_in_smem<H>();   // a 32-row tile fits next to the weights only below H = 512
+  constexpr int NB3 = WIDE ? 32 : 16;
+  int nb = 0;
+  R2D2_TRY(pick_nb<H>(p.B, lstm_scan_fwd_kernel<H, 8>, FwdSmem<H, 8>::BYTES, lstm_scan_fwd_kernel<H, 16>,
+                      FwdSmem<H, 16>::BYTES, WIDE ? lstm_scan_fwd_kernel<H, NB3> : nullptr, FwdSmem<H, NB3>::BYTES, &nb));
   if (nb == 8)
     return launch_cluster(lstm_scan_fwd_kernel<H, 8>, p, H / 32, ceil_div(p.B, 8), FwdSmem<H, 8>::BYTES, stream);
   if (nb == 16)
     return launch_cluster(lstm_scan_fwd_kernel<H, 16>, p, H / 32, ceil_div(p.B, 16), FwdSmem<H, 16>::BYTES, stream);
-  return launch_cluster(lstm_scan_fwd_kernel<H, 32>, p, H / 32, ceil_div(p.B, 32), FwdSmem<H, 32>::BYTES, stream);
+  return launch_cluster(lstm_scan_fwd_kernel<H, NB3>, p, H / 32, ceil_div(p.B, NB3), FwdSmem<H, NB3>::BYTES, stream);
 }
 template <int H>
 int bwd_dispatch(const ScanBwdParams& p, cudaStream_t stream) {
-  const int nb = pick_nb(p.B, H);
+  constexpr bool WIDE = !w_hi_in_smem<H>();
+  constexpr int NB3 = WIDE ? 32 : 16;
+  int nb = 0;
+  R2D2_TRY(pick_nb<H>(p.B, lstm_scan_bwd_kernel<H, 8>, BwdSmem<H, 8>::BYTES, lstm_scan_bwd_kernel<H, 16>,
+                      BwdSmem<H, 16>::BYTES, WIDE ? lstm_scan_bwd_kernel<H, NB3> : nullptr, BwdSmem<H, NB3>::BYTES, &nb));
   if (nb == 8)
     return launch_cluster(lstm_scan_bwd_kernel<H, 8>, p, H / 32, ceil_div(p.B, 8), BwdSmem<H, 8>::BYTES, stream);
   if (nb == 16)
     return launch_cluster(lstm_scan_bwd_kernel<H, 16>, p, H / 32, ceil_div(p.B, 16), BwdSmem<H, 16>::BYTES, stream);
-  return launch_cluster(lstm_scan_bwd_kernel<H, 32>, p, H / 32, ceil_div(p.B, 32), BwdSmem<H, 32>::BYTES, stream);
+  return launch_cluster(lstm_scan_bwd_kernel<H, NB3>, p, H / 32, ceil_div(p.B, NB3), BwdSmem<H, NB3>::BYTES, stream);
 }
 
 }  // namespace
 
-// v1 (mma.sync) cluster kernels: weights as register fragments, up to 256 hidden units
-static bool v1_cluster_supported(int H) { return H == 32 || H == 64 || H == 128 || H == 256; }
-// tcgen05 kernels: up to 512 hidden units (cluster of 16 CTAs, W_hh lo plane partly in shared memory)
-bool lstm_scan_cluster_supported(int H) { return v1_cluster_supported(H) || H == 512; }
-bool lstm_scan_backward_emits_images(int H) { return lstm_scan_cluster_supported(H) && lstm_scan_get_impl() == 1; }
+bool lstm_scan_cluster_supported(int H) { return H == 32 || H == 64 || H == 128 || H == 256 || H == 512; }
 
 static int g_scan_impl = -1;
 void lstm_scan_set_impl(int impl) { g_scan_impl = impl ? 1 : 0; }
 int lstm_scan_get_impl() {
   if (g_scan_impl < 0) {
     const char* e = getenv("R2D2_SCAN_IMPL");
-    g_scan_impl = (e && (e[0] == 'm' || e[0] == '0')) ? 0 : 1;
+    g_scan_impl = (e && (e[0] == 's' || e[0] == '0')) ? 0 : 1;
   }
   return g_scan_impl;
 }
+static bool use_cluster_kernels(int H) { return lstm_scan_cluster_supported(H) && lstm_scan_get_impl() == 1; }
 
-size_t lstm_scan_fwd_scratch_floats(int B, int H) {   // the per-step path is the A/B fallback wherever v1 has no kernel
-  return v1_cluster_supported(H) ? 0 : (size_t)B * 4 * H;
+// the cluster kernels synchronise with hardware cluster barriers only: there is no bounded wait that could time out
+int lstm_scan_error_status(int* out, cudaStream_t stream) {
+  R2D2_REQUIRE(out, "null");
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
+  *out = 0;
+  return R2D2_OK;
 }
-size_t lstm_scan_bwd_scratch_floats(int B, int H) {
-  return v1_cluster_supported(H) ? 0 : (size_t)2 * B * H;
-}
+
+// the per-step path can be selected for every hidden size (lstm_scan_set_impl(0)), so its scratch is always reserved
+size_t lstm_scan_fwd_scratch_floats(int B, int H) { return (size_t)B * 4 * H; }
+size_t lstm_scan_bwd_scratch_floats(int B, int H) { return (size_t)2 * B * H; }
 
 int lstm_scan_forward(const ScanFwdParams& p, cudaStream_t stream) {
   R2D2_REQUIRE(p.gin && p.whh && p.gates && p.hs && p.cs, "null pointer");
   R2D2_REQUIRE(p.T > 0 && p.B > 0 && p.H > 0 && p.repeat >= 1, "shape");
   R2D2_REQUIRE(p.repeat == 1 || p.gates != p.gin, "gates must not alias gin when repeat > 1");
-  if (lstm_scan_cluster_supported(p.H) && lstm_scan_get_impl() == 1) return lstm_scan_forward_tc(p, stream);
-  switch (p.H) {
-    case 32: return fwd_dispatch<32>(p, stream);
-    case 64: return fwd_dispatch<64>(p, stream);
-    case 128: return fwd_dispatch<128>(p, stream);
-    case 256: return fwd_dispatch<256>(p, stream);
-    default: break;
+  if (use_cluster_kernels(p.H)) {
+    switch (p.H) {
+      case 32: return fwd_dispatch<32>(p, stream);
+      case 64: return fwd_dispatch<64>(p, stream);
+      case 128: return fwd_dispatch<128>(p, stream);
+      case 256: return fwd_dispatch<256>(p, stream);
+      case 512: return fwd_dispatch<512>(p, stream);
+      default: break;
+    }
   }
   return scan_forward_generic(p, p.scratch, stream);
 }
@@ -569,16 +660,15 @@ int lstm_scan_backward(const ScanBwdParams& p, cudaStream_t stream) {
   R2D2_REQUIRE(p.gates && p.hs && p.cs && p.whh && p.dgates, "null pointer");
   R2D2_REQUIRE(p.T > 0 && p.B > 0 && p.H > 0 && p.repeat >= 1, "shape");
   R2D2_REQUIRE(p.repeat == 1 || (p.dgin && p.dgin != p.dgates), "dgin buffer required when repeat > 1");
-  if (lstm_scan_cluster_supported(p.H) && lstm_scan_get_impl() == 1) return lstm_scan_backward_tc(p, stream);  // bias sums fused
-  int rc;
-  switch (p.H) {
+  int rc = R2D2_OK;
+  switch (use_cluster_kernels(p.H) ? p.H : 0) {
     case 32: rc = bwd_dispatch<32>(p, stream); break;
     case 64: rc = bwd_dispatch<64>(p, stream); break;
     case 128: rc = bwd_dispatch<128>(p, stream); break;
     case 256: rc = bwd_dispatch<256>(p, stream); break;
+    case 512: rc = bwd_dispatch<512>(p, stream); break;
     default: rc = scan_backward_generic(p, stream); break;
   }
-  R2D2_REQUIRE(!p.skip_fp32, "skip_fp32 needs the tcgen05 scan (lstm_scan_backward_emits_images)");
   R2D2_TRY(rc);
   if (p.dbias) {  // sum_t dgin_t == sum_s dgates_s
     const float* src = p.repeat > 1 ? p.dgin : p.dgates;

@@ -17,13 +17,9 @@ struct ScanFwdParams {
   float* cs = nullptr;          // [S+1,B,H]
   float* head_in = nullptr;     // optional [T,B,H]: tanh(h) at steps s % repeat == repeat-1 (actor head input)
   int T = 0, B = 0, H = 0, repeat = 1;   // S = T*repeat; repeat=2 reproduces the double actor step (learner.py:122-123)
-  float* scratch = nullptr;     // generic path only: [B,4H]
-  int rows_per_cluster = 0;     // set by the tcgen05 dispatcher: batch rows owned by one cluster (<= its N tile)
-  long long* trace = nullptr;   // debug: [grid][S][8] globaltimer stamps written by thread 0 of every CTA (tcgen05 kernel)
-  unsigned char* xchg = nullptr;   // set by the tcgen05 dispatcher (H = 512): global scratch of the h_t exchange through L2
-  int no_save = 0;                 // 1: chain is never back-propagated (target nets): gates / cs need not be stored (hs, head_in
-                                   // still are); honoured by the H = 512 kernel, ignored elsewhere
-  int dbg = 0;                     // dev only (env R2D2_SCAN_DBG, honoured by the trace build of the H = 512 kernel)
+  float* scratch = nullptr;     // per-step path: [B,4H]
+  int no_save = 0;              // 1: chain is never back-propagated (target nets): the cluster kernels store neither gates
+                                // nor cs[1..S] (hs and head_in are stored)
 };
 
 struct ScanBwdParams {
@@ -37,42 +33,24 @@ struct ScanBwdParams {
   float* dgates = nullptr;         // [S,B,4H] dLoss/d(pre-activation gates) (may alias gates)
   float* dgin = nullptr;           // [T,B,4H] sum over the `repeat` steps sharing an input row (== dgates if repeat==1)
   int T = 0, B = 0, H = 0, repeat = 1;
-  float* scratch = nullptr;        // generic path only: [2,B,H] (dh_rec, dc)
+  float* scratch = nullptr;        // per-step path: [2,B,H] (dh_rec, dc)
   float* dbias = nullptr;          // optional [4H]: column sums of dgates over all steps and rows are ADDED here
   float* dbias2 = nullptr;         // optional second copy (b_ih and b_hh receive the same gradient)
-  // tcgen05 path only: the scan can write dG directly as the packed bf16 hi/lo operand images of the three GEMMs that
-  // consume it (tile formats of gemm_tc.cu), so that no pack pass and no fp32 round trip is needed:
-  unsigned char* img_k = nullptr;       // dgin   as A of dgin * W_ih  : K-major tiles  [ceil(T*B/128)][4H/32][16 KB]
-  unsigned char* img_mn_dg = nullptr;   // dgates as A of dgates^T * h : MN-major tiles [4H/128][ceil(S*B/32)][16 KB]
-  unsigned char* img_mn_gin = nullptr;  // dgin   as A of dgin^T * z1  : MN-major tiles [4H/128][ceil(T*B/32)][16 KB]
-                                        // (pass img_mn_dg again when repeat == 1: the two tensors coincide)
-  int skip_fp32 = 0;                    // 1: do not store fp32 dgates / dgin (every consumer reads the images)
-  int rows_per_cluster = 0;        // set by the tcgen05 dispatcher
-  unsigned char* xchg = nullptr;   // set by the tcgen05 dispatcher (H = 512): global scratch of the partial-sum exchange through L2
-  int dbg = 0;                     // dev only (env R2D2_SCAN_DBG): 1 = skip the dG stores, 2 = skip the saved-activation loads
-  long long* trace = nullptr;      // debug: [grid][S][8] globaltimer stamps (H = 512 kernel, tools/trace_bwd.py)
-  int row_begin = 0, row_end = 0;  // set by the tcgen05 dispatcher: batch rows [row_begin, row_end) of THIS launch (0, 0 = all)
 };
 
-// true when lstm_scan_backward will honour img_* (persistent tcgen05 kernels selected for this hidden size)
-bool lstm_scan_backward_emits_images(int H);
-
-// true when the persistent cluster kernels cover this hidden size (H in {32,64,128,256})
+// true when persistent cluster kernels cover this hidden size (H in {32,64,128,256,512})
 bool lstm_scan_cluster_supported(int H);
 int lstm_scan_forward(const ScanFwdParams& p, cudaStream_t stream);
 int lstm_scan_backward(const ScanBwdParams& p, cudaStream_t stream);
-// generic-path scratch requirements in floats (0 when the cluster kernels cover H)
+// per-step path scratch requirements in floats (reserved for every H: the path can be selected at run time)
 size_t lstm_scan_fwd_scratch_floats(int B, int H);
 size_t lstm_scan_bwd_scratch_floats(int B, int H);
 
-// implementation of the cluster kernels: 1 = tcgen05/TMEM (default), 0 = mma.sync (v1, kept for A/B checks).
-// Initialised from the environment variable R2D2_SCAN_IMPL ("tc" | "mma") on first use.
+// 1 = persistent cluster kernels where they cover H (default), 0 = per-step path (one GEMM + one cell kernel per step)
+// for every H, the A/B reference.  Initialised from the environment variable R2D2_SCAN_IMPL ("cluster" | "step").
 void lstm_scan_set_impl(int impl);
 int lstm_scan_get_impl();
-int lstm_scan_forward_tc(const ScanFwdParams& p, cudaStream_t stream);
-int lstm_scan_backward_tc(const ScanBwdParams& p, cudaStream_t stream);
-// nonzero if a bounded mbarrier wait of a tcgen05 scan kernel ever timed out (protocol bug); synchronises the stream
+// nonzero if a scan kernel reported a protocol error; synchronises the stream
 int lstm_scan_error_status(int* out, cudaStream_t stream);
-int lstm_scan_max_active_clusters(int H, int nb, int backward);
 
 }  // namespace r2d2

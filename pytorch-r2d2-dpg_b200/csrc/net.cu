@@ -24,12 +24,7 @@ size_t ChainWs::floats(const NetShape& s, int T, int B, int repeat) {
   const size_t sb = lstm_scan_bwd_scratch_floats(B, s.hidden);
   if (sb > sc) sc = sb;
   n += align64(sc + 64);
-  if (lstm_scan_cluster_supported(s.hidden)) {   // operand images, 4 bytes per element like the fp32 tensors they replace
-    n += align64(pad_to(TB, 128) * 4 * H);
-    n += align64(pad_to(S * B, 32) * 4 * H);
-    if (repeat > 1) n += align64(pad_to(TB, 32) * 4 * H);
-    n += align64(pad_to(TB, 32) * pad_to(H, 128));
-  }
+  n += align64(pad_to(TB, 128) * H);           // z1 operand image (bf16 hi + lo: 4 bytes per element)
   return n;
 }
 
@@ -52,12 +47,7 @@ ChainWs ChainWs::carve(float* base, const NetShape& s, int T, int B, int repeat)
   const size_t sb = lstm_scan_bwd_scratch_floats(B, s.hidden);
   if (sb > sc) sc = sb;
   w.scratch = take(sc + 64);
-  if (lstm_scan_cluster_supported(s.hidden)) {
-    w.img_k = reinterpret_cast<unsigned char*>(take(pad_to(TB, 128) * 4 * H));
-    w.img_mn_dg = reinterpret_cast<unsigned char*>(take(pad_to(S * B, 32) * 4 * H));
-    w.img_mn_gin = (repeat > 1) ? reinterpret_cast<unsigned char*>(take(pad_to(TB, 32) * 4 * H)) : w.img_mn_dg;
-    w.img_z_mn = reinterpret_cast<unsigned char*>(take(pad_to(TB, 32) * pad_to(H, 128)));
-  }
+  w.img_k = reinterpret_cast<unsigned char*>(take(pad_to(TB, 128) * H));
   return w;
 }
 
@@ -80,20 +70,12 @@ int net_forward_inputs(const NetShape& s, const NetParams& P, const ChainWs& ws,
     g.A = obs; g.lda = O; g.B = P.w1; g.ldb = I; g.K = O;
     if (s.critic) { g.A2 = act; g.lda2 = A; g.B2 = P.w1 + O; g.ldb2 = I; g.K2 = A; }
     g.C = ws.z1; g.ldc = H; g.M = M; g.N = H; g.bias = P.b1; g.epilogue = EPI_TANH;
-    // the l1 kernel can write z1 a second time as the packed A operand of the W_ih product (the BPTT image buffer is
-    // idle during the forward pass)
+    // the l1 kernel can write z1 a second time as the packed A operand of the W_ih product
     z1_img = ws.img_k != nullptr && gemm_emits_operand_image(M, H, I);
     if (z1_img) g.C_img_k = ws.img_k;
-    if (z1_img && ws.keep_z1_image && ws.img_z_mn) {   // second copy as the B operand of dW_ih (BPTT of this chain)
-      g.C_img_mn = ws.img_z_mn;
-      if (M % 32 != 0) {   // rows of the last 32-row tile that no batch row maps to are part of a reduction: zeros
-        const size_t kt = (size_t)(M + 31) / 32;
-        R2D2_CUDA_TRY(cudaMemset2DAsync(ws.img_z_mn + (kt - 1) * 16384, kt * 16384, 0, 16384, (size_t)(H + 127) / 128, stream));
-      }
-    }
     R2D2_TRY(gemm_f32(g, GEMM_NT, stream));
   }
-  const bool two_bias = gemm_supports_bias2(M, 4 * H, H);   // the tcgen05 epilogue adds both biases itself
+  const bool two_bias = gemm_supports_bias2(M, 4 * H, H);   // the wgmma epilogue adds both biases itself
   if (!two_bias) R2D2_TRY(add_vec(P.bih, P.bhh, ws.bias_sum, 4 * H, stream));
   {  // gin = z1 * W_ih^T + (b_ih + b_hh)   (input half of LSTMCell, models.py:37,80) for all rows at once
     GemmParams g;
@@ -157,7 +139,6 @@ int net_backward(const NetShape& s, const NetParams& P, const NetParams* G, cons
     R2D2_TRY(gemm_f32(g, GEMM_NN, stream));
   }
   float* dgin = (repeat > 1) ? ws.gin : ws.gates;
-  const bool use_img = ws.img_k != nullptr && lstm_scan_backward_emits_images(H) && gemm_get_impl() != 0;
   {
     ScanBwdParams bp;
     bp.gates = ws.gates; bp.hs = ws.hs; bp.cs = ws.cs; bp.whh = P.whh;
@@ -165,26 +146,18 @@ int net_backward(const NetShape& s, const NetParams& P, const NetParams* G, cons
     bp.dgates = ws.gates; bp.dgin = dgin;
     bp.T = T; bp.B = B; bp.H = H; bp.repeat = repeat; bp.scratch = ws.scratch;
     if (G) { bp.dbias = G->bih; bp.dbias2 = G->bhh; }   // db_ih = db_hh = sum of dG, accumulated inside the scan
-    if (use_img) {   // dG leaves the scan as the packed operands of the three GEMMs below: no pack pass, no fp32 copy
-      bp.img_k = ws.img_k;
-      if (G) { bp.img_mn_dg = ws.img_mn_dg; bp.img_mn_gin = ws.img_mn_gin; }
-      bp.skip_fp32 = 1;
-    }
     R2D2_TRY(lstm_scan_backward(bp, stream));
   }
   if (G) {
     {  // dW_hh = sum_s dG_s^T h_{s-1}
       GemmParams g;
       g.A = ws.gates; g.lda = 4 * H; g.B = ws.hs; g.ldb = H; g.K = S * B;
-      if (use_img) g.A_img = ws.img_mn_dg;
       g.C = G->whh; g.ldc = H; g.M = 4 * H; g.N = H; g.split_k = gemm_suggest_split_k(4 * H, H, S * B);
       R2D2_TRY(gemm_f32(g, GEMM_TN, stream));
     }
     {  // dW_ih = sum_t dGin_t^T z1_t
       GemmParams g;
       g.A = dgin; g.lda = 4 * H; g.B = ws.z1; g.ldb = H; g.K = M;
-      if (use_img) g.A_img = ws.img_mn_gin;
-      if (use_img && ws.keep_z1_image && ws.img_z_mn && gemm_emits_operand_image(M, H, I)) g.B_img = ws.img_z_mn;
       g.C = G->wih; g.ldc = H; g.M = 4 * H; g.N = H; g.split_k = gemm_suggest_split_k(4 * H, H, M);
       g.reuse_packed_a = (repeat == 1);   // same dG operand as the dW_hh product just above
       R2D2_TRY(gemm_f32(g, GEMM_TN, stream));
@@ -193,7 +166,6 @@ int net_backward(const NetShape& s, const NetParams& P, const NetParams* G, cons
   {  // d(pre-l1) = (dGin * W_ih) * (1 - z1^2), in place over z1
     GemmParams g;
     g.A = dgin; g.lda = 4 * H; g.B = P.wih; g.ldb = H; g.K = 4 * H;
-    if (use_img) g.A_img = ws.img_k;
     g.C = ws.z1; g.ldc = H; g.M = M; g.N = H; g.Z = ws.z1; g.ldz = H; g.epilogue = EPI_MUL_DTANH;
     R2D2_TRY(gemm_f32(g, GEMM_NN, stream));
   }

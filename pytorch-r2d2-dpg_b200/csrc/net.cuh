@@ -42,13 +42,8 @@ struct ChainWs {
   float* d_pre = nullptr;     // [T,B,A]
   float* bias_sum = nullptr;  // [4H] b_ih + b_hh
   float* scratch = nullptr;   // generic scan path
-  // packed bf16 hi/lo images of dG written by the BPTT scan (tcgen05 path; null when the hidden size has no cluster kernel)
-  unsigned char* img_k = nullptr;       // dgin, K-major tiles (A of the data-gradient product)
-  unsigned char* img_mn_dg = nullptr;   // dgates, MN-major tiles (A of dW_hh)
-  unsigned char* img_mn_gin = nullptr;  // dgin, MN-major tiles (A of dW_ih); == img_mn_dg when repeat == 1
-  unsigned char* img_z_mn = nullptr;    // z1, MN-major tiles (B of dW_ih), written by the l1 kernel when `keep_z1_image`
+  unsigned char* img_k = nullptr;       // z1 as the packed K-major A operand of z1 * W_ih^T (written by the l1 kernel)
   bool inference_only = false;          // set by the owner of a chain that is never back-propagated (target nets)
-  bool keep_z1_image = false;           // set by the owner of a chain whose weights get gradients (learner: critic, actor)
   static size_t floats(const NetShape& s, int T, int B, int repeat);
   static ChainWs carve(float* base, const NetShape& s, int T, int B, int repeat);
 };

@@ -143,7 +143,7 @@ int peer_reduce(PeerExchange& x, int block, cudaStream_t stream) {
   if (!x.reduce_pending[block]) return R2D2_OK;
   const long long slice_vec = x.lay.padded[block] / 4 / x.world;
   int grid = (int)((slice_vec + 511) / 512);
-  if (grid > 148) grid = 148;
+  if (grid > num_sms()) grid = num_sms();
   if (grid < 1) grid = 1;
   peer_reduce_kernel<<<grid, 512, 0, stream>>>(x.ptrs, x.world, x.rank, x.lay.off_flags, block, x.lay.off_grads[block],
                                               x.lay.off_sums[block], slice_vec, x.epoch[block]);

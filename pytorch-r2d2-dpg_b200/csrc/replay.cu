@@ -151,7 +151,7 @@ __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
 
 int grid_for(long long total) {
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   if (blocks < 1) blocks = 1;
   return (int)blocks;
 }

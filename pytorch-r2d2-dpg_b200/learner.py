@@ -2,7 +2,7 @@
 `.update_target_model()`, `learner_process(n_actors)` (learner.py:18-67) with the same attributes,
 hyper-parameter literals, cwd-relative ./model_data and ./memory_data protocol and checkpoint keys -
 so the reference's r2d2.py launcher runs unchanged - while every iteration of the loop body
-(learner.py:84-139) executes in libr2d2_b200 (hand-written sm_100a CUDA):
+(learner.py:84-139) executes in libr2d2_b200 (hand-written sm_90a CUDA):
 
     memory.sample()          -> DeviceReplay.sample_into   (sum-tree draw + gather kernels, HBM resident)
     burn-in / unrolls / BPTT -> LearnerEngine.step         (persistent cluster LSTM scans + tensor-core GEMMs)

@@ -1,6 +1,6 @@
 """Actor-side rows of the path on the GPU (SURVEY 8f N2): the n-step reward pre-sum and the initial sequence
 priorities that every reference actor computes per finished episode at batch 1 on its own nets
-(/root/reference/actor.py:74-76 `calc_nstep_reward`, :78-107 `calc_priorities`), batched over episodes:
+(reference actor.py:74-76 `calc_nstep_reward`, :78-107 `calc_priorities`), batched over episodes:
 
     B = episodes, time-major zero-padded rows -> three persistent chains from the zero state
     (online critic on the stored actions, target actor, target critic on the target actor's actions:

@@ -87,7 +87,7 @@ def init_reference_params(cfg: PathConfig, critic: bool, generator: torch.Genera
 class LearnerEngine:
     def __init__(self, cfg: PathConfig, device=None, seed: int = 1):
         if not torch.cuda.is_available():
-            raise nv.NativeError("LearnerEngine needs a CUDA device (B200); there is no CPU fallback")
+            raise nv.NativeError("LearnerEngine needs a CUDA device (H100); there is no CPU fallback")
         self.lib = nv.lib()
         self.cfg = cfg
         self._pending_finish = False          # a deferred phase 3 (data-parallel "defer" mode), see step() / flush()

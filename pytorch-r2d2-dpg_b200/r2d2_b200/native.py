@@ -80,11 +80,6 @@ SIGNATURES = {
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "r2d2_lstm_scan_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p,
                                         c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "r2d2_debug_scan_forward_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
-                                              c_void_p, c_void_p]),
-    "r2d2_debug_scan_backward_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                               c_int, c_void_p, c_void_p]),
-    "r2d2_debug_max_active_clusters": (c_int, [c_int, c_int, c_int]),
     "r2d2_set_gemm_impl": (c_int, [c_int]),
     "r2d2_get_gemm_impl": (c_int, []),
     "r2d2_set_scan_impl": (c_int, [c_int]),

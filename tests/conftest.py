@@ -14,7 +14,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -32,8 +32,15 @@ def pytest_collection_modifyitems(config, items):
 
 
 def load_golden(name):
-    z = np.load(os.path.join(GOLDEN, name), allow_pickle=False)
-    return {k: z[k] for k in z.files}
+    """Fixture `name`; a large one is stored as <stem>.part0.npz, <stem>.part1.npz, ... (oracle/make_golden.py)."""
+    stem = name[:-len(".npz")]
+    parts = sorted((f for f in os.listdir(GOLDEN) if f.startswith(stem + ".part") and f.endswith(".npz")),
+                   key=lambda f: int(f[len(stem) + 5:-4]))
+    out = {}
+    for f in parts or [name]:
+        z = np.load(os.path.join(GOLDEN, f), allow_pickle=False)
+        out.update({k: z[k] for k in z.files})
+    return out
 
 
 def golden_params(g, prefix):

@@ -1,4 +1,4 @@
-"""Next-row N2 (SURVEY 8f): actor-side n-step reward pre-sum and initial priorities (/root/reference/actor.py:74-107).
+"""Next-row N2 (SURVEY 8f): actor-side n-step reward pre-sum and initial priorities (reference actor.py:74-107).
 
  * CPU: the numpy restatement (oracle/actor_oracle.py) against the fixture the UNMODIFIED reference produced
    (tests/golden/ref_actor_prio.npz, oracle/make_golden.py gen_actor_priorities) - pins the checker;

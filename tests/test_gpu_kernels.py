@@ -60,7 +60,7 @@ GEMM_CASES = [
 
 @pytest.fixture(params=["tc", "mma", "default"])
 def gemm_impl(request, nv):
-    # 2: tcgen05 path for every shape; 0: mma.sync v1 kernel; 1 (default): tcgen05 + the fp32 streaming kernels of
+    # 2: wgmma path for every shape; 0: mma.sync kernel; 1 (default): wgmma + the fp32 streaming kernels of
     # gemm_thin.cu for shapes with a dimension <= 32
     nv.lib().r2d2_set_gemm_impl({"tc": 2, "mma": 0, "default": 1}[request.param])
     yield request.param
@@ -150,7 +150,8 @@ NET_CASES = [
 
 @pytest.fixture(params=["tc", "mma"])
 def scan_impl(request, nv):
-    """Run the chain tests on both scan implementations: tcgen05/TMEM (default) and the mma.sync v1 kernels."""
+    """Run the chain tests on both scan implementations: the persistent cluster kernels (default; the hidden sizes they
+    do not cover fall through to the per-step path) and the per-step path (one GEMM + one cell kernel per step)."""
     lib = nv.lib()
     lib.r2d2_set_scan_impl(1 if request.param == "tc" else 0)
     yield request.param

@@ -103,9 +103,8 @@ def test_cfg2_full_size_against_port(eng_mod):
 
 @pytest.mark.parametrize("batch", [24, 512])
 def test_cfg3_hidden_512_against_port(eng_mod, batch):
-    """BASELINE.json configs[2] (obs=376 act=17 hidden=512 seq_len=80 burn_in=40): the cluster-of-16 tcgen05 scan
-    (W_hh hi plane in tensor memory, lo plane split between tensor and shared memory) at the full batch of 512 and at a
-    batch that fills a single 16-row tile, against the CPU port of the reference on the same synthetic batch."""
+    """BASELINE.json configs[2] (obs=376 act=17 hidden=512 seq_len=80 burn_in=40): the H = 512 chains at the full batch
+    of 512 and at a small batch of 24, against the CPU port of the reference on the same synthetic batch."""
     import ctypes
     from r2d2_b200 import native as nv
     pc = ref_port.PathConfig(obs=376, act=17, hidden=512, batch=batch, burn_in=40, learning=80, n_step=5)
@@ -294,3 +293,47 @@ def test_pipelined_step_matches_sequential(eng_mod, hidden, batch):
     torch.cuda.synchronize()
     for net in ("actor", "critic"):
         assert rel_l2(pip.flat[net].cpu().numpy(), seq.flat[net].cpu().numpy()) < 1e-5, net
+
+
+@pytest.mark.parametrize("hidden,batch", [(256, 64), (512, 32)])
+def test_replay_fed_run_is_bitwise_reproducible(eng_mod, hidden, batch):
+    """Two runs of the same seeded replay-fed loop (draw from the sum tree, pipelined step, priority write-back) give the
+    same bits: split-K weight gradients, bias column sums and loss sums are added in a fixed order, so the priorities
+    and with them the next draws cannot drift apart between runs."""
+    kw = dict(obs=11, act=3, hidden=hidden, batch=batch, burn_in=10, learning=20, n_step=3)
+    cfg = eng_mod.PathConfig(**kw)
+    ep_len = 120
+
+    def run():
+        rng = np.random.default_rng(5)
+        n_rows = ep_len + cfg.n_step
+        rp = eng_mod.DeviceReplay(cfg, capacity_rows=24 * n_rows)
+        for _ in range(24):
+            term = np.zeros(n_rows, np.float32)
+            term[ep_len:] = 1
+            rp.add_episode(rng.standard_normal((n_rows, cfg.obs)).astype(np.float32),
+                           rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32),
+                           rng.standard_normal(n_rows).astype(np.float32), term,
+                           (0.1 * rng.standard_normal((ep_len, 4, 2, cfg.hidden))).astype(np.float32),
+                           rng.uniform(0.01, 1, ep_len - (cfg.burn_in + cfg.learning)).astype(np.float32))
+        eng = eng_mod.LearnerEngine(cfg, seed=7)
+        gen = torch.Generator(device="cuda").manual_seed(11)
+
+        def hook(e, used):
+            rp.update_priorities(used.leaf_idx, used.priority)
+            rp.sample_into(e, generator=gen)
+
+        rp.sample_into(eng, generator=gen)
+        for _ in range(6):
+            eng.step(prefetch=hook)
+        torch.cuda.synchronize()
+        out = {k: getattr(eng, k).clone() for k in ("q_value", "target_q_value", "priority", "losses", "leaf_idx")}
+        for net in ("actor", "critic"):
+            out.update({f"{net}.{k}": v.clone() for k, v in eng.views(net).items()})
+        rp.close()
+        eng.close()
+        return out
+
+    a, b = run(), run()
+    for k in a:
+        assert torch.equal(a[k], b[k]), k

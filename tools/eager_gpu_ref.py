@@ -1,4 +1,4 @@
-"""Context number (SURVEY 8d): the reference learner iteration in PyTorch EAGER mode on one B200 - the only
+"""Context number (SURVEY 8d): the reference learner iteration in PyTorch EAGER mode on one H100 - the only
 pre-existing GPU implementation of this path (oracle/ref_port.py with its modules and batch moved to cuda).
 Not part of bench.py's contract; prints one JSON line."""
 import json, os, sys, time
@@ -38,5 +38,5 @@ if __name__ == "__main__":
         lr.iteration(batch_np, keep_tensors=False)
         torch.cuda.synchronize(); times.append(time.perf_counter() - t0)
     sec = sorted(times[2:])[len(times[2:]) // 2]
-    print(json.dumps({"impl": "reference port, PyTorch eager on 1x B200 (fp32, TF32 off)", "config": c,
+    print(json.dumps({"impl": "reference port, PyTorch eager on 1x H100 (fp32, TF32 off)", "config": c,
                       "sec_per_iteration": sec, "seq_steps_per_s": c["batch"] * c["learning"] / sec, "all": [round(t, 4) for t in times]}))

@@ -1,4 +1,4 @@
-"""Time r2d2_gemm_f32 on the learner's shapes (dev tool): us and fp32-equivalent TFLOP/s, tcgen05 vs mma.sync."""
+"""Time r2d2_gemm_f32 on the learner's shapes (dev tool): us and fp32-equivalent TFLOP/s, wgmma vs mma.sync."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "pytorch-r2d2-dpg_b200")]
