@@ -29,11 +29,9 @@ __device__ __forceinline__ float apply_epilogue(float v, int epilogue, float z) 
 // ------------------------------------------------------------------------------------------------
 constexpr int SK_ROWS = 32, SK_COLS = 256, SK_KMAX = 32, SK_THREADS = 256, SK_WLD = SK_COLS + 4;
 
-__device__ __forceinline__ void cp_async_4(float* smem_dst, const float* gsrc) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+using sm90::cp_async_4;
+using sm90::cp_async_commit;
+using sm90::cp_async_wait_all;
 
 template <bool NN>
 __global__ void __launch_bounds__(SK_THREADS) thin_smallk_kernel(GemmParams p, int vec_c, int vec_z) {

@@ -6,17 +6,34 @@
 // at H = 512 (cluster of 16, non-portable size) the slice is 256 KB, more than the register file or the 227 KB of
 // shared memory of one CTA, so the lo plane stays in registers and the hi plane lives in shared memory in fragment
 // order (one conflict-free 16-byte load per thread and k-step);
-// per step the only traffic is the h_t all-gather inside the cluster through distributed shared
-// memory plus one hardware cluster barrier.  Batch is split across clusters (grid = C * ceil(B/NB)).
+// per step the only traffic is the h_t all-gather (forward) or the dh reduce-scatter (BPTT) inside the cluster through
+// distributed shared memory.  It is point to point: every transfer completes the transaction count of one mbarrier of
+// the receiving CTA per (buffer, source CTA), and a CTA waits for each source's data just before it uses it, so there
+// is no per-step cluster barrier.  Batch is split across clusters (grid = C * ceil(B/NB)).
 //   forward : D[gate rows(128) x NB] = W_slice[128 x H] * h_{s-1}^T           (swap-AB: M = gate rows)
 //   backward: P[H x NB] = W_slice^T[H x 128] * dG_s^T  -> reduce-scatter of fp32 partials via DSMEM
 // Tensor cores: mma.sync bf16, 3 passes (hi*hi, lo*hi, hi*lo), fp32 accumulate.
+//
+// Hand-off protocol (both kernels).  bar[buf][src] (arrival count 1) completes when this CTA has armed it with the
+// byte count of one slice (arrive.expect_tx) and CTA `src` has delivered those bytes (complete_tx).  The data for step
+// s >= 1 (forward) / iteration it >= 1 (BPTT) sits in buffer b = s & 1; buffer b is filled for the steps b+1, b+3,
+// ..., so step s uses phase (s-1)/2 of bar[b][*] and waits on parity ((s-1) >> 1) & 1.  A barrier is armed once after
+// init and re-armed by this CTA after all of its threads have passed the wait of the phase before (the __syncthreads
+// that follows the waits), so it is never armed twice in one phase.
+// Why no write-after-read hazard remains: CTA d writes step s+1's slice into my buffer b only after its own step-s
+// MMAs (forward) / pointwise (BPTT) consumed the slice I sent at step s, and I send that slice only after a
+// __syncthreads that follows my reads of buffer b at step s-1; a peer is therefore never more than one step ahead of
+// the buffer it writes.  The same chain shows that the next phase of bar[b][d] cannot complete before every thread
+// of mine has observed the current one, so parity waits are unambiguous.
+// Every wait is bounded (wait_slice): on expiry it records a status word read by lstm_scan_error_status and carries on,
+// so a protocol error is reported and the launch still ends.
 #include <cooperative_groups.h>
 #include <stdlib.h>
 
 #include "gemm.cuh"
 #include "lstm_scan.cuh"
 #include "elementwise.cuh"
+#include "sm90.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -28,8 +45,34 @@ constexpr int UNITS_PER_CTA = 32;
 constexpr int ROWS_PER_CTA = 128;         // 4 gates x 32 units
 constexpr int GT_LD = ROWS_PER_CTA + 4;   // fp32 gate tile [NB][132]: conflict-free fragment writes / unit reads
 constexpr int DG_LD = ROWS_PER_CTA + 8;   // bf16 dG tile [NB][136]
+constexpr unsigned long long kWaitLimitNs = 4000000000ull;
+
+__device__ unsigned g_scan_status = 0;   // 1 = a bounded hand-off wait expired (sticky until read)
 
 __device__ __forceinline__ float accurate_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+
+// waits until phase `parity` of `bar` has completed, for at most kWaitLimitNs; on expiry it sets g_scan_status and
+// returns as if the data had arrived.  Once a wait has expired the run is lost and later waits do not stall it further.
+__device__ __forceinline__ void wait_slice(uint64_t* bar, uint32_t parity) {
+  if (sm90::mbar_try_wait(bar, parity)) return;
+  if (*reinterpret_cast<volatile unsigned*>(&g_scan_status)) return;
+  const unsigned long long t0 = global_ns();
+  while (!sm90::mbar_try_wait(bar, parity)) {
+    if (global_ns() - t0 > kWaitLimitNs) {
+      atomicExch(&g_scan_status, 1u);
+      return;
+    }
+  }
+}
+
+// phase parity of the hand-off barriers used at step (iteration) s >= 1: see the protocol note at the top
+__device__ __forceinline__ uint32_t slice_parity(int s) { return (uint32_t)((s - 1) >> 1) & 1u; }
 
 // ------------------------------------------------------------------------------------------------
 // forward
@@ -39,12 +82,17 @@ template <int H> __host__ __device__ constexpr bool w_hi_in_smem() { return H > 
 
 template <int H, int NB>
 struct FwdSmem {
-  static constexpr int HLD = H + 8;                        // bf16 row stride of the h operand tile
+  static constexpr int C = H / 32;
+  static constexpr int HROW = UNITS_PER_CTA + 8;           // 80-byte rows: g * 20 words mod 32 are distinct, so the
+                                                           // B-fragment loads are free of bank conflicts
+  static constexpr int SLICE = 2 * NB * HROW;              // bf16 h_t slice of one source CTA [plane][n][unit]: one bulk copy
   static constexpr int W_BYTES = w_hi_in_smem<H>() ? (H / 16) * 8 * 32 * 16 : 0;   // hi fragments [ks][warp][lane][16 B]
-  static constexpr int HB_ELEMS = 2 * 2 * NB * HLD;        // [buf][plane][n][k]
+  static constexpr int HB_ELEMS = 2 * C * SLICE;           // h operand [buf][src][plane][n][unit]
   static constexpr int GT_ELEMS = NB * GT_LD;              // fp32
-  static constexpr int HS_ELEMS = 2 * NB * UNITS_PER_CTA;  // bf16 staging [plane][n][unit]
-  static constexpr int BYTES = W_BYTES + HB_ELEMS * 2 + GT_ELEMS * 4 + HS_ELEMS * 2;
+  static constexpr int HS_ELEMS = SLICE;                   // bf16 staging of this CTA's slice
+  static constexpr int BAR_OFF = W_BYTES + HB_ELEMS * 2 + GT_ELEMS * 4 + HS_ELEMS * 2;
+  static constexpr int BYTES = BAR_OFF + 2 * C * 8;        // + mbarriers [buf][src]
+  static_assert((SLICE * 2) % 16 == 0 && BAR_OFF % 16 == 0, "bulk copies need 16-byte granules");
   static_assert(BYTES <= 232448, "forward scan tile does not fit in 227 KB of shared memory");
 };
 
@@ -53,7 +101,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
   constexpr int C = H / 32, KS = H / 16, NT = NB / 8;
   constexpr bool WS = w_hi_in_smem<H>();
   using SM = FwdSmem<H, NB>;
-  constexpr int HLD = SM::HLD;
+  constexpr int HROW = SM::HROW, SLICE = SM::SLICE;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   const int b0 = (blockIdx.x / C) * NB;
@@ -66,6 +114,37 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
   __nv_bfloat16* hb = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES);
   float* gt = reinterpret_cast<float*>(smem_raw + SM::W_BYTES + SM::HB_ELEMS * 2);
   __nv_bfloat16* hstage = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES + SM::HB_ELEMS * 2 + SM::GT_ELEMS * 4);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + SM::BAR_OFF);   // [buf][src]
+
+  // ---- initial state (before the weights, while few registers are live): full h0 tile -> hb[0]; own units -> hs[0], cs[0], c registers
+  for (int idx = tid; idx < NB * H; idx += SCAN_THREADS) {
+    const int n = idx / H, k = idx % H, b = b0 + n;
+    float v = (b < B && p.h0) ? __ldg(p.h0 + (size_t)b * H + k) : 0.f;
+    __nv_bfloat16 hi, lo;
+    split_bf16(v, hi, lo);
+    __nv_bfloat16* row = hb + (0 * C + k / UNITS_PER_CTA) * SLICE + n * HROW + k % UNITS_PER_CTA;
+    row[0] = hi;
+    row[NB * HROW] = lo;
+  }
+  const int ug = rank * 32 + lane;  // global hidden unit owned by this thread in the pointwise phase
+  float cst[NT];
+#pragma unroll
+  for (int e = 0; e < NT; ++e) {
+    const int b = b0 + w + 8 * e;
+    cst[e] = 0.f;
+    if (b < B) {
+      float hv = p.h0 ? __ldg(p.h0 + (size_t)b * H + ug) : 0.f;
+      float cv = p.c0 ? __ldg(p.c0 + (size_t)b * H + ug) : 0.f;
+      p.hs[(size_t)b * H + ug] = hv;
+      p.cs[(size_t)b * H + ug] = cv;
+      cst[e] = cv;
+    }
+  }
+  if (tid < 2 * C) {
+    sm90::mbar_init(bar + tid, 1);
+    sm90::fence_mbar_init_cluster();
+    sm90::mbar_arrive_expect_tx(bar + tid, SLICE * 2);
+  }
 
   // ---- W_hh slice -> resident A fragments (rows: local r = gate*32 + unit; warp w owns r in [16w,16w+16))
   uint32_t a_hi[WS ? 1 : KS][4], a_lo[KS][4];
@@ -94,47 +173,25 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
       }
     }
   }
-
-  // ---- initial state: full h0 tile -> hb[0]; own units -> hs[0], cs[0], c registers
-  for (int idx = tid; idx < NB * H; idx += SCAN_THREADS) {
-    const int n = idx / H, k = idx % H, b = b0 + n;
-    float v = (b < B && p.h0) ? __ldg(p.h0 + (size_t)b * H + k) : 0.f;
-    __nv_bfloat16 hi, lo;
-    split_bf16(v, hi, lo);
-    hb[(0 * 2 + 0) * NB * HLD + n * HLD + k] = hi;
-    hb[(0 * 2 + 1) * NB * HLD + n * HLD + k] = lo;
-  }
-  const int ug = rank * 32 + lane;  // global hidden unit owned by this thread in the pointwise phase
-  float cst[NT];
-#pragma unroll
-  for (int e = 0; e < NT; ++e) {
-    const int b = b0 + w + 8 * e;
-    cst[e] = 0.f;
-    if (b < B) {
-      float hv = p.h0 ? __ldg(p.h0 + (size_t)b * H + ug) : 0.f;
-      float cv = p.c0 ? __ldg(p.c0 + (size_t)b * H + ug) : 0.f;
-      p.hs[(size_t)b * H + ug] = hv;
-      p.cs[(size_t)b * H + ug] = cv;
-      cst[e] = cv;
-    }
-  }
   __syncthreads();
-  cluster.sync();  // every CTA of the cluster has started: remote shared memory may be written from here on
+  cluster.sync();  // every CTA of the cluster has started and armed its barriers: remote transfers may start
 
   const size_t gstride = (size_t)4 * H;
   for (int s = 0; s < S; ++s) {
     const int cur = s & 1, nxt = cur ^ 1;
     const int t = s / p.repeat;
 
-    // prefetch this step's input projection for the elements this thread finishes (hides HBM/L2 latency behind the MMAs)
-    float gpre[NT][4];
+    // this step's input projection -> the gate tile, for the elements whose MMA fragment this thread adds below:
+    // the copies run behind the MMAs without holding registers (gates may alias gin: each element is read here
+    // before the pointwise phase of this step overwrites it)
 #pragma unroll
-    for (int e = 0; e < NT; ++e) {
-      const int b = b0 + w + 8 * e;
+    for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        gpre[e][q] = (b < B) ? p.gin[((size_t)t * B + b) * gstride + q * H + ug] : 0.f;  // plain load: gates may alias gin
-    }
+      for (int f = 0; f < 4; ++f) {
+        const int n = nt * 8 + 2 * c + (f & 1), r = 16 * w + g + (f >> 1) * 8, b = b0 + n;
+        if (b < B) sm90::cp_async_4(gt + n * GT_LD + r, p.gin + ((size_t)t * B + b) * gstride + (r >> 5) * H + rank * 32 + (r & 31));
+      }
+    sm90::cp_async_commit();
 
     // ---- tensor-core part: acc[128 x NB] = W_slice * h_{s-1}^T
     float acc[NT][4];
@@ -142,10 +199,16 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
     for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[nt][e] = 0.f;
-    const __nv_bfloat16* hb_hi = hb + (cur * 2 + 0) * NB * HLD;
-    const __nv_bfloat16* hb_lo = hb + (cur * 2 + 1) * NB * HLD;
+    const __nv_bfloat16* hb_cur = hb + cur * C * SLICE;
+    uint64_t* bar_cur = bar + cur * C;
+    const uint32_t parity = slice_parity(s);
 #pragma unroll
     for (int ks = 0; ks < KS; ++ks) {
+      // k-steps 2d, 2d+1 read the slice of source CTA d: wait for it here, so that the MMAs on the slices that
+      // arrived first overlap the arrival of the later ones (step 0 reads h0, written by this CTA)
+      if ((ks & 1) == 0 && s > 0) wait_slice(bar_cur + ks / 2, parity);
+      const __nv_bfloat16* hb_hi = hb_cur + (ks / 2) * SLICE;
+      const __nv_bfloat16* hb_lo = hb_hi + NB * HROW;
       uint32_t ah[4];
       if constexpr (WS) {
         const uint4 v = w_hi_s[(ks * 8 + w) * 32 + lane];
@@ -156,7 +219,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
       }
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
-        const int off = (nt * 8 + g) * HLD + ks * 16 + 2 * c;
+        const int off = (nt * 8 + g) * HROW + (ks & 1) * 16 + 2 * c;
         uint32_t bh[2], bl[2];
         bh[0] = *reinterpret_cast<const uint32_t*>(hb_hi + off);
         bh[1] = *reinterpret_cast<const uint32_t*>(hb_hi + off + 8);
@@ -167,16 +230,20 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
         mma_bf16_16816(acc[nt], ah, bh);
       }
     }
-    // fragment -> gate tile gt[n][local row]
+    // fragment + input projection -> gate tile gt[n][local row] (rows b >= B hold garbage and are never read)
+    sm90::cp_async_wait_all();
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
       const int n = nt * 8 + 2 * c, r = 16 * w + g;
-      gt[n * GT_LD + r] = acc[nt][0];
-      gt[(n + 1) * GT_LD + r] = acc[nt][1];
-      gt[n * GT_LD + r + 8] = acc[nt][2];
-      gt[(n + 1) * GT_LD + r + 8] = acc[nt][3];
+      gt[n * GT_LD + r] += acc[nt][0];
+      gt[(n + 1) * GT_LD + r] += acc[nt][1];
+      gt[n * GT_LD + r + 8] += acc[nt][2];
+      gt[(n + 1) * GT_LD + r + 8] += acc[nt][3];
     }
+    if (w == 0 && lane < C) sm90::bulk_wait_read_all();   // last step's sends have read hstage
     __syncthreads();
+    // every thread has passed its waits on bar[cur][*]: arm them for the step after next
+    if (s > 0 && tid < C) sm90::mbar_arrive_expect_tx(bar_cur + tid, SLICE * 2);
 
     // ---- pointwise LSTM cell: thread = (unit = lane, batch column n = w + 8e); coalesced along units
 #pragma unroll
@@ -185,10 +252,10 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
       __nv_bfloat16 hi = __float2bfloat16_rn(0.f), lo = hi;
       if (b < B) {
         const float* gr = gt + n * GT_LD + lane;
-        const float ig = accurate_sigmoid(gr[0] + gpre[e][0]);
-        const float fg = accurate_sigmoid(gr[32] + gpre[e][1]);
-        const float gg = tanhf(gr[64] + gpre[e][2]);
-        const float og = accurate_sigmoid(gr[96] + gpre[e][3]);
+        const float ig = accurate_sigmoid(gr[0]);
+        const float fg = accurate_sigmoid(gr[32]);
+        const float gg = tanhf(gr[64]);
+        const float og = accurate_sigmoid(gr[96]);
         const float cn = fg * cst[e] + ig * gg;
         const float hn = og * tanhf(cn);
         cst[e] = cn;
@@ -202,25 +269,23 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_fwd_kernel(ScanFwdP
           p.head_in[((size_t)t * B + b) * H + ug] = tanhf(hn);
         split_bf16(hn, hi, lo);
       }
-      hstage[(0 * NB + n) * UNITS_PER_CTA + lane] = hi;
-      hstage[(1 * NB + n) * UNITS_PER_CTA + lane] = lo;
+      hstage[(0 * NB + n) * HROW + lane] = hi;
+      hstage[(1 * NB + n) * HROW + lane] = lo;
     }
+    sm90::fence_proxy_async_smem();   // the bulk copies below read hstage through the async proxy
     __syncthreads();
 
-    // ---- all-gather of h_s inside the cluster: 16-byte DSMEM stores into every CTA's next operand buffer
-    if (s + 1 < S) {
-      constexpr int VEC_PER_CTA = 2 * NB * 4;  // [plane][n][4 x 16 B]
-      for (int vv = tid; vv < C * VEC_PER_CTA; vv += SCAN_THREADS) {
-        const int d = vv / VEC_PER_CTA, v = vv % VEC_PER_CTA;
-        const int plane = v / (NB * 4), n = (v / 4) % NB, q4 = v % 4;
-        const uint4 val = *reinterpret_cast<const uint4*>(hstage + (plane * NB + n) * UNITS_PER_CTA + q4 * 8);
-        __nv_bfloat16* dst_local = hb + ((nxt * 2 + plane) * NB + n) * HLD + rank * 32 + q4 * 8;
-        __nv_bfloat16* dst = cluster.map_shared_rank(dst_local, d);
-        *reinterpret_cast<uint4*>(dst) = val;
-      }
+    // ---- all-gather of h_s inside the cluster: one bulk copy of this CTA's slice into every CTA's next operand
+    // buffer, completing that CTA's bar[nxt][rank]
+    if (s + 1 < S && w == 0 && lane < C) {
+      const uint32_t slot = sm90::smem_u32(hb + (nxt * C + rank) * SLICE);
+      const uint32_t slot_bar = sm90::smem_u32(bar + nxt * C + rank);
+      sm90::bulk_copy_s2cluster(sm90::map_cluster(slot, lane), sm90::smem_u32(hstage), SLICE * 2,
+                                sm90::map_cluster(slot_bar, lane));
+      sm90::bulk_commit();
     }
-    cluster.sync();
   }
+  cluster.sync();   // no CTA leaves while a peer may still deliver into its shared memory
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -232,9 +297,12 @@ struct BwdSmem {
   static constexpr int DG_ELEMS = 2 * NB * DG_LD;               // bf16 [plane][n][local gate row]
   static constexpr int PS_LD = NB + 2;                          // 2-way instead of 16-way bank conflicts on the unit-strided reads
   static constexpr int PS_ELEMS = 2 * C * UNITS_PER_CTA * PS_LD; // fp32 [buf][src rank][unit][n]
+  static constexpr int PS_BYTES_PER_SRC = UNITS_PER_CTA * NB * 4; // delivered per (buf, src): the pad columns stay unwritten
   static constexpr int MT = (H / 16 + 7) / 8;
   static constexpr int W_BYTES = w_hi_in_smem<H>() ? MT * 8 * 8 * 32 * 16 : 0;   // hi fragments [i][ks][warp][lane][16 B]
-  static constexpr int BYTES = W_BYTES + DG_ELEMS * 2 + PS_ELEMS * 4;
+  static constexpr int BAR_OFF = W_BYTES + DG_ELEMS * 2 + PS_ELEMS * 4;
+  static constexpr int BYTES = BAR_OFF + 2 * C * 8;              // + mbarriers [buf][src]
+  static_assert(BAR_OFF % 8 == 0, "mbarrier alignment");
   static_assert(BYTES <= 232448, "BPTT scan tile does not fit in 227 KB of shared memory");
 };
 
@@ -257,6 +325,13 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
   uint4* w_hi_s = reinterpret_cast<uint4*>(smem_raw);   // H = 512 only
   __nv_bfloat16* dgs = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES);
   float* ps = reinterpret_cast<float*>(smem_raw + SM::W_BYTES + SM::DG_ELEMS * 2);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + SM::BAR_OFF);   // [buf][src]
+
+  if (tid < 2 * C) {
+    sm90::mbar_init(bar + tid, 1);
+    sm90::fence_mbar_init_cluster();
+    sm90::mbar_arrive_expect_tx(bar + tid, SM::PS_BYTES_PER_SRC);
+  }
 
   // ---- W_hh slice (transposed use): A(m = j output unit, k = local gate row r) = W_hh[grow(r)][j]
   uint32_t a_hi[WS ? 1 : MT][WS ? 1 : KS][4], a_lo[MT][KS][4];
@@ -306,6 +381,13 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
     const int rel = s - p.head_first_step;
     const bool has_head = p.dh_head && rel >= 0 && (rel % p.repeat) == p.repeat - 1;
 
+    // partial dh from every source CTA (iteration 0 has none); summed below in source order 0..C-1
+    if (it > 0) {
+      const uint32_t parity = slice_parity(it);
+#pragma unroll
+      for (int src = 0; src < C; ++src) wait_slice(bar + buf * C + src, parity);
+    }
+
     // ---- pointwise backward of the cell (thread = (unit = lane, n = w + 8e))
 #pragma unroll
     for (int e = 0; e < NT; ++e) {
@@ -349,6 +431,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
       }
     }
     __syncthreads();
+    // every thread has passed its waits on bar[buf][*]: arm them for the iteration after next
+    if (it > 0 && tid < C) sm90::mbar_arrive_expect_tx(bar + buf * C + tid, SM::PS_BYTES_PER_SRC);
 
     if (s > 0) {
       // ---- partial dh_{s-1}[j, n] over this CTA's 128 gate rows
@@ -390,7 +474,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
           }
         }
       }
-      // ---- reduce-scatter: partial rows j go to the CTA that owns unit j (slot = my rank), fp32 via DSMEM
+      // ---- reduce-scatter: partial rows j go to the CTA that owns unit j (slot = my rank), fp32 st.async into its
+      // shared memory, each store completing its bytes on the owner's bar[buf ^ 1][rank]
+      const uint32_t slot_bar = sm90::smem_u32(bar + (buf ^ 1) * C + rank);
 #pragma unroll
       for (int i = 0; i < MT; ++i) {
         const int mi = w * MT + i;
@@ -399,17 +485,19 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
           for (int h2 = 0; h2 < 2; ++h2) {
             const int j = mi * 16 + g + h2 * 8;
             const int owner = j >> 5, jl = j & 31;
-            float* slot_local = ps + (((buf ^ 1) * C + rank) * UNITS_PER_CTA + jl) * SM::PS_LD;
-            float* slot = cluster.map_shared_rank(slot_local, owner);
+            const uint32_t slot = sm90::map_cluster(
+                sm90::smem_u32(ps + (((buf ^ 1) * C + rank) * UNITS_PER_CTA + jl) * SM::PS_LD), owner);
+            const uint32_t owner_bar = sm90::map_cluster(slot_bar, owner);
 #pragma unroll
             for (int nt = 0; nt < NT; ++nt)
-              *reinterpret_cast<float2*>(slot + nt * 8 + 2 * c) = make_float2(acc[i][nt][2 * h2], acc[i][nt][2 * h2 + 1]);
+              sm90::st_async_f2(slot + (nt * 8 + 2 * c) * 4, acc[i][nt][2 * h2], acc[i][nt][2 * h2 + 1], owner_bar);
           }
         }
       }
     }
-    cluster.sync();
+    __syncthreads();   // dgs is rewritten by the next iteration's pointwise phase
   }
+  cluster.sync();   // no CTA leaves while a peer may still deliver into its shared memory
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -627,11 +715,12 @@ int lstm_scan_get_impl() {
 }
 static bool use_cluster_kernels(int H) { return lstm_scan_cluster_supported(H) && lstm_scan_get_impl() == 1; }
 
-// the cluster kernels synchronise with hardware cluster barriers only: there is no bounded wait that could time out
 int lstm_scan_error_status(int* out, cudaStream_t stream) {
   R2D2_REQUIRE(out, "null");
+  unsigned v = 0;
+  R2D2_CUDA_TRY(cudaMemcpyFromSymbolAsync(&v, g_scan_status, sizeof(v), 0, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
-  *out = 0;
+  *out = (int)v;
   return R2D2_OK;
 }
 

@@ -50,7 +50,8 @@ size_t lstm_scan_bwd_scratch_floats(int B, int H);
 // for every H, the A/B reference.  Initialised from the environment variable R2D2_SCAN_IMPL ("cluster" | "step").
 void lstm_scan_set_impl(int impl);
 int lstm_scan_get_impl();
-// nonzero if a scan kernel reported a protocol error; synchronises the stream
+// nonzero if a bounded hand-off wait inside a cluster scan kernel expired (the word stays set for the rest of the
+// process: the results of that launch and of later ones are not to be trusted); synchronises the stream
 int lstm_scan_error_status(int* out, cudaStream_t stream);
 
 }  // namespace r2d2

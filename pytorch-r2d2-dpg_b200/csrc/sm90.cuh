@@ -1,5 +1,6 @@
 // Hopper (sm_90a) primitives used by the packed-operand GEMM: wgmma shared-memory descriptors and the
-// m64n128k16 bf16 wgmma, mbarrier with transaction counts and 1-D bulk copies global -> shared.
+// m64n128k16 bf16 wgmma, mbarrier with transaction counts and 1-D bulk copies global -> shared; and by the LSTM
+// scans: bulk copies and st.async between the CTAs of a cluster that complete on the receiver's mbarrier.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -96,6 +97,41 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst_smem_addr, const void* src_global, uint32_t bytes, uint32_t mbar_smem_addr) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem_addr),
                "l"(src_global), "r"(bytes), "r"(mbar_smem_addr)
+               : "memory");
+}
+
+// 4-byte asynchronous copy global -> shared (LDGSTS); completion per thread with cp_async_wait_all
+__device__ __forceinline__ void cp_async_4(float* smem_dst, const float* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+
+// ---- point-to-point hand-off inside a thread-block cluster (the persistent LSTM scans)
+// makes mbarrier.init visible to the other CTAs of the cluster (a cluster barrier must still follow)
+__device__ __forceinline__ void fence_mbar_init_cluster() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// orders this thread's generic-proxy shared-memory writes before later async-proxy (bulk copy) reads of them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// shared::cta address -> shared::cluster address of the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t map_cluster(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
+}
+// bulk copy own shared memory -> shared memory of a CTA of the cluster, completing `bytes` on that CTA's mbarrier
+__device__ __forceinline__ void bulk_copy_s2cluster(uint32_t dst_cluster_addr, uint32_t src_smem_addr, uint32_t bytes,
+                                                    uint32_t mbar_cluster_addr) {
+  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst_cluster_addr), "r"(src_smem_addr), "r"(bytes), "r"(mbar_cluster_addr)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the source reads of every bulk copy this thread committed are done: the source may be overwritten
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// 8-byte store into shared memory of a CTA of the cluster, completing 8 bytes on that CTA's mbarrier
+__device__ __forceinline__ void st_async_f2(uint32_t dst_cluster_addr, float x, float y, uint32_t mbar_cluster_addr) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+               ::"r"(dst_cluster_addr), "f"(x), "f"(y), "r"(mbar_cluster_addr)
                : "memory");
 }
 
