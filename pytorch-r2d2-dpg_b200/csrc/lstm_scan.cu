@@ -25,6 +25,16 @@
 // __syncthreads that follows my reads of buffer b at step s-1; a peer is therefore never more than one step ahead of
 // the buffer it writes.  The same chain shows that the next phase of bar[b][d] cannot complete before every thread
 // of mine has observed the current one, so parity waits are unambiguous.
+// BPTT activation stage.  None of the BPTT's per-step global inputs (gates[s], cs[s], dh_head) depends on the
+// recurrence, so each thread cp.asyncs step s-1's values for its own cells into stage[plane][n][unit] right after the
+// pointwise phase of step s, and waits for them (cp.async.wait_group 0, no barrier: no thread reads a stage element
+// another thread copied) at the top of the next pointwise phase; the pointwise phase then reads only shared memory.
+// c_new (cs[s+1]) is c_prev of the step before and is carried in a register.
+//  - stage write-after-read: a thread issues the next prefetch only after it has consumed the values it read from
+//    the stage (they are in dgs before the __syncthreads that precedes the prefetch);
+//  - in-place dG (dgates may alias gates): the thread that prefetches gates[s-1][b][q*H+u] is the only writer of
+//    dgates[s-1][b][q*H+u], and it writes it only after its cp.async wait;
+//  - repeat > 1: the keep / dgin accumulation is untouched.
 // Every wait is bounded (wait_slice): on expiry it records a status word read by lstm_scan_error_status and carries on,
 // so a protocol error is reported and the launch still ends.
 #include <cooperative_groups.h>
@@ -300,7 +310,9 @@ struct BwdSmem {
   static constexpr int PS_BYTES_PER_SRC = UNITS_PER_CTA * NB * 4; // delivered per (buf, src): the pad columns stay unwritten
   static constexpr int MT = (H / 16 + 7) / 8;
   static constexpr int W_BYTES = w_hi_in_smem<H>() ? MT * 8 * 8 * 32 * 16 : 0;   // hi fragments [i][ks][warp][lane][16 B]
-  static constexpr int BAR_OFF = W_BYTES + DG_ELEMS * 2 + PS_ELEMS * 4;
+  static constexpr int STAGE_PLANES = 6;                        // gates i, f, g, o; c_prev; dh_head
+  static constexpr int STAGE_ELEMS = STAGE_PLANES * NB * UNITS_PER_CTA;   // fp32 [plane][n][unit], one step
+  static constexpr int BAR_OFF = W_BYTES + DG_ELEMS * 2 + PS_ELEMS * 4 + STAGE_ELEMS * 4;
   static constexpr int BYTES = BAR_OFF + 2 * C * 8;              // + mbarriers [buf][src]
   static_assert(BAR_OFF % 8 == 0, "mbarrier alignment");
   static_assert(BYTES <= 232448, "BPTT scan tile does not fit in 227 KB of shared memory");
@@ -325,15 +337,53 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
   uint4* w_hi_s = reinterpret_cast<uint4*>(smem_raw);   // H = 512 only
   __nv_bfloat16* dgs = reinterpret_cast<__nv_bfloat16*>(smem_raw + SM::W_BYTES);
   float* ps = reinterpret_cast<float*>(smem_raw + SM::W_BYTES + SM::DG_ELEMS * 2);
+  float* stage = ps + SM::PS_ELEMS;                                       // [plane][n][unit]
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + SM::BAR_OFF);   // [buf][src]
+  constexpr int PLANE = NB * UNITS_PER_CTA;
+  constexpr size_t gstride = (size_t)4 * H;
+
+  // step s adds dh_head row (s - head_first_step) / repeat when it is the last repeat of a head row
+  auto head_step = [&](int s) {
+    const int rel = s - p.head_first_step;
+    return p.dh_head && rel >= 0 && (rel % p.repeat) == p.repeat - 1;
+  };
+  // gates, c_prev (and dh_head on head steps) of step s for exactly the cells this thread processes in the pointwise
+  // phase -> stage; the copies land while the MMAs, the reduce-scatter and the dh waits of the step before run.
+  // The addresses are rebuilt from %tid.x at every call: kept live instead, they would cost registers through the W_hh
+  // prologue below, which at H = 512 already runs at the 255-register limit.
+  auto prefetch = [&](int s) {
+    const int rel = s - p.head_first_step;
+    const bool head = head_step(s);
+    unsigned tv;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tv));   // volatile: not hoisted out of the step loop
+    const int lane = tv & 31, w = tv >> 5, ug = rank * 32 + lane;
+#pragma unroll
+    for (int e = 0; e < NT; ++e) {
+      const int n = w + 8 * e, b = b0 + n;
+      if (b < B) {
+        float* st = stage + n * UNITS_PER_CTA + lane;
+        const float* gs = p.gates + ((size_t)s * B + b) * gstride + ug;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) sm90::cp_async_4(st + q * PLANE, gs + q * H);
+        sm90::cp_async_4(st + 4 * PLANE, p.cs + ((size_t)s * B + b) * H + ug);
+        if (head) sm90::cp_async_4(st + 5 * PLANE, p.dh_head + ((size_t)(rel / p.repeat) * B + b) * H + ug);
+      }
+    }
+    sm90::cp_async_commit();
+  };
 
   if (tid < 2 * C) {
     sm90::mbar_init(bar + tid, 1);
     sm90::fence_mbar_init_cluster();
     sm90::mbar_arrive_expect_tx(bar + tid, SM::PS_BYTES_PER_SRC);
   }
+  prefetch(S - 1);   // overlaps the W_hh prologue below
 
   // ---- W_hh slice (transposed use): A(m = j output unit, k = local gate row r) = W_hh[grow(r)][j]
+  // element (j, r) with j = mi * 16 + g + (f & 1) * 8, r = ks * 16 + 2c + (f >> 1) * 8 (local gate rows r, r+1: gate
+  // r / 32 = ks / 2, unit r % 32) sits at a compile-time offset from one per-thread pointer, so the unrolled loads
+  // need no further address registers (and spill less at H = 512)
+  const float* w_t = p.whh + (size_t)(rank * 32 + 2 * c) * H + w * MT * 16 + g;
   uint32_t a_hi[WS ? 1 : MT][WS ? 1 : KS][4], a_lo[MT][KS][4];
 #pragma unroll
   for (int i = 0; i < MT; ++i) {
@@ -345,11 +395,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
       for (int f = 0; f < 4; ++f) {
         float v0 = 0.f, v1 = 0.f;
         if (mi < M_TILES) {
-          const int j = mi * 16 + g + (f & 1) * 8;
-          const int r = ks * 16 + 2 * c + (f >> 1) * 8;  // r, r+1: local gate rows (gate = r/32, unit = r%32)
-          const size_t row0 = (size_t)((r >> 5) * H + rank * 32 + (r & 31));
-          v0 = __ldg(p.whh + row0 * H + j);
-          v1 = __ldg(p.whh + (row0 + 1) * H + j);  // r even -> r+1 stays in the same gate block
+          const float* w0 = w_t + ((ks >> 1) * H + (ks & 1) * 16 + (f >> 1) * 8) * H + i * 16 + (f & 1) * 8;
+          v0 = __ldg(w0);
+          v1 = __ldg(w0 + H);  // r even -> r+1 stays in the same gate block
         }
         split_pack2(v0, v1, h[f], a_lo[i][ks][f]);
       }
@@ -364,11 +412,13 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
 
   __syncthreads();   // W_hh hi fragments in shared memory (H = 512) before the first MMA
   const int ug = rank * 32 + lane;
-  const size_t gstride = (size_t)4 * H;
-  float dcn[NT], keep[NT][4];
+  // c_new of the cell at step s (cs[s+1]) is c_prev of step s+1: it stays in a register, only cs[S] is loaded here
+  float dcn[NT], keep[NT][4], c_new[NT];
 #pragma unroll
   for (int e = 0; e < NT; ++e) {
+    const int b = b0 + w + 8 * e;
     dcn[e] = 0.f;
+    c_new[e] = b < B ? __ldg(p.cs + ((size_t)S * B + b) * H + ug) : 0.f;
 #pragma unroll
     for (int q = 0; q < 4; ++q) keep[e][q] = 0.f;
   }
@@ -378,15 +428,23 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
     const int s = S - 1 - it;
     const int buf = it & 1;
     const int t = s / p.repeat;
-    const int rel = s - p.head_first_step;
-    const bool has_head = p.dh_head && rel >= 0 && (rel % p.repeat) == p.repeat - 1;
+    const bool has_head = head_step(s);
 
-    // partial dh from every source CTA (iteration 0 has none); summed below in source order 0..C-1
+    // partial dh from every source CTA (iteration 0 has none), added in source order 0..C-1 as each one arrives
+    float dh_rec[NT];
+#pragma unroll
+    for (int e = 0; e < NT; ++e) dh_rec[e] = 0.f;
     if (it > 0) {
       const uint32_t parity = slice_parity(it);
 #pragma unroll
-      for (int src = 0; src < C; ++src) wait_slice(bar + buf * C + src, parity);
+      for (int src = 0; src < C; ++src) {
+        wait_slice(bar + buf * C + src, parity);
+        const float* pr = ps + ((buf * C + src) * UNITS_PER_CTA + lane) * SM::PS_LD + w;
+#pragma unroll
+        for (int e = 0; e < NT; ++e) dh_rec[e] += pr[8 * e];
+      }
     }
+    sm90::cp_async_wait_all();   // this step's stage, copied by this thread one iteration earlier
 
     // ---- pointwise backward of the cell (thread = (unit = lane, n = w + 8e))
 #pragma unroll
@@ -394,16 +452,13 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
       const int n = w + 8 * e, b = b0 + n;
       float dg[4] = {0.f, 0.f, 0.f, 0.f};
       if (b < B) {
-        float dh = 0.f;
-        if (it > 0) {
-#pragma unroll
-          for (int src = 0; src < C; ++src) dh += ps[((buf * C + src) * UNITS_PER_CTA + lane) * SM::PS_LD + n];
-        }
-        if (has_head) dh += __ldg(p.dh_head + ((size_t)(rel / p.repeat) * B + b) * H + ug);
-        const float* gs = p.gates + ((size_t)s * B + b) * gstride + ug;
-        const float ig = gs[0], fg = gs[H], gg = gs[2 * H], og = gs[3 * H];
-        const float c_prev = __ldg(p.cs + ((size_t)s * B + b) * H + ug);
-        const float tc = tanhf(__ldg(p.cs + ((size_t)(s + 1) * B + b) * H + ug));
+        const float* st = stage + n * UNITS_PER_CTA + lane;
+        float dh = dh_rec[e];
+        if (has_head) dh += st[5 * PLANE];
+        const float ig = st[0], fg = st[PLANE], gg = st[2 * PLANE], og = st[3 * PLANE];
+        const float c_prev = st[4 * PLANE];
+        const float tc = tanhf(c_new[e]);
+        c_new[e] = c_prev;
         const float dc = dcn[e] + dh * og * (1.f - tc * tc);
         dg[3] = dh * tc * og * (1.f - og);
         dg[0] = dc * gg * ig * (1.f - ig);
@@ -435,6 +490,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
     if (it > 0 && tid < C) sm90::mbar_arrive_expect_tx(bar + buf * C + tid, SM::PS_BYTES_PER_SRC);
 
     if (s > 0) {
+      prefetch(s - 1);
       // ---- partial dh_{s-1}[j, n] over this CTA's 128 gate rows
       float acc[MT][NT][4];
 #pragma unroll
