@@ -5,10 +5,11 @@
 //     order (no swizzle), zero padded.  Producers that can write it directly do (GemmParams::A_img / B_img, the l1
 //     kernel for z1); otherwise pack_operand_kernel converts the fp32 tensor (any leading dimension, ragged edges) in an
 //     HBM-bound elementwise pass (8 B/element).
-//  2. gemm_packed_kernel: per CTA one 128 x 128 output tile.  A producer thread streams the tile images with 1-D bulk
-//     copies (cp.async.bulk ... mbarrier::complete_tx, no tensor map, no per-element work) through a 4-stage ring; two
-//     consumer warpgroups each issue wgmma.m64n128k16 (passes lo*hi + hi*lo + hi*hi) into register accumulators and
-//     apply bias / tanh / dtanh / +Z or the split-K reduction straight from the accumulator fragments.
+//  2. gemm_packed_kernel: per CTA one 128 x 128 output tile, two CTAs per SM.  A producer thread streams the tile images
+//     with 1-D bulk copies (cp.async.bulk ... mbarrier::complete_tx, no tensor map, no per-element work) through a
+//     3-stage ring; two consumer warpgroups each issue wgmma.m64n128k16 (passes lo*hi + hi*lo + hi*hi) into register
+//     accumulators, keeping one k tile of wgmma in flight while they wait for the next, and apply bias / tanh / dtanh /
+//     +Z or the split-K reduction straight from the accumulator fragments.
 //
 // Why images instead of fp32 operands: the image is the same byte count as the fp32 operand, is re-read ~N/128 (A)
 // or ~M/128 (B) times from L2, and needs no conversion inside the GEMM's main loop.
@@ -28,8 +29,11 @@ namespace {
 constexpr int TBM = 128, TBN = 128, TBK = 32;
 constexpr int PLANE_BYTES = 128 * TBK * 2;     // 8 KB: one bf16 plane of a 128 x 32 operand tile
 constexpr int TILE_BYTES = 2 * PLANE_BYTES;    // 16 KB: hi plane + lo plane of one operand tile
-constexpr int PACKED_GEMM_THREADS = 384;       // warpgroup 0 producer, warpgroups 1..2 wgmma + epilogue
-constexpr int STAGES = 4;
+constexpr int PACKED_GEMM_THREADS = 288;       // warpgroups 0..1 wgmma + epilogue, warp 8 producer
+// two CTAs per SM (2 x 96 KB ring, 2 x 288 threads x 96 registers): one CTA's ring fill and epilogue run while the
+// other's wgmmas keep the tensor pipe busy
+constexpr int CTAS_PER_SM = 2;
+constexpr int STAGES = 3;
 constexpr int STAGE_BYTES = 2 * TILE_BYTES;    // A tile + B tile
 constexpr int OFF_BARS = STAGES * STAGE_BYTES;
 constexpr int PACKED_SMEM = OFF_BARS + 128;
@@ -95,10 +99,10 @@ struct PackedGemmParams {
   unsigned char* c_img_mn;
 };
 
-// 3 warpgroups: warpgroup 0 = producer (one elected thread), warpgroups 1 and 2 = consumers, each owning 64 rows of the
-// 128 x 128 output tile as wgmma register accumulators.
+// warpgroups 0 and 1 = consumers, each owning 64 rows of the 128 x 128 output tile as wgmma register accumulators;
+// warp 8 = producer (one elected thread).
 template <bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(PACKED_GEMM_THREADS, 1) gemm_packed_kernel(PackedGemmParams p) {
+__global__ void __launch_bounds__(PACKED_GEMM_THREADS, CTAS_PER_SM) gemm_packed_kernel(PackedGemmParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BARS);   // [STAGES] bytes landed
   uint64_t* empty = full + STAGES;                                  // [STAGES] both consumer warpgroups done reading
@@ -119,9 +123,9 @@ __global__ void __launch_bounds__(PACKED_GEMM_THREADS, 1) gemm_packed_kernel(Pac
   }
   __syncthreads();
 
-  if (wg == 0) {
+  if (wg == 2) {
     // ================= producer: one 16 KB bulk copy per operand tile and k tile =================
-    if (tid < 32 && sm90::elect_one()) {
+    if (sm90::elect_one()) {
       const unsigned char* a_src = p.pa + ((size_t)m_tile * p.k_tiles + t_begin) * TILE_BYTES;
       const unsigned char* b_src = p.pb + ((size_t)n_tile * p.k_tiles + t_begin) * TILE_BYTES;
       const uint32_t smem_base = sm90::smem_u32(smem);
@@ -137,8 +141,8 @@ __global__ void __launch_bounds__(PACKED_GEMM_THREADS, 1) gemm_packed_kernel(Pac
     return;
   }
 
-  // ================= consumers: rows [64 (wg - 1), 64 wg) of the tile =================
-  const int half = wg - 1, t = tid & 127;
+  // ================= consumers: rows [64 wg, 64 wg + 64) of the tile =================
+  const int half = wg, t = tid & 127;
   float acc[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc[i] = 0.f;
@@ -153,6 +157,7 @@ __global__ void __launch_bounds__(PACKED_GEMM_THREADS, 1) gemm_packed_kernel(Pac
     mbar_wait_spin(&full[s], (i / STAGES) & 1);
     const uint32_t sa = smem_base + s * STAGE_BYTES + a_half, sb = smem_base + s * STAGE_BYTES + TILE_BYTES;
     if (!(p.debug_flags & 2)) {
+      sm90::fence_regs(acc);
       sm90::wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < TBK / 16; ++ks) {
@@ -165,11 +170,16 @@ __global__ void __launch_bounds__(PACKED_GEMM_THREADS, 1) gemm_packed_kernel(Pac
         sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_hi);
       }
       sm90::wgmma_commit();
-      sm90::wgmma_wait_all();
+      sm90::wgmma_wait<1>();   // k tile i - 1 is done, k tile i stays in flight
+      sm90::fence_regs(acc);
     }
     __syncwarp();
-    if (t == 0) sm90::mbar_arrive(&empty[s]);
+    if (i > 0 && t == 0) sm90::mbar_arrive(&empty[(i - 1) % STAGES]);
   }
+  sm90::wgmma_wait<0>();
+  sm90::fence_regs(acc);
+  __syncwarp();
+  if (t == 0) sm90::mbar_arrive(&empty[(n_tiles - 1) % STAGES]);
 
   // ================= epilogue straight from the accumulator fragments =================
   // fragment j of a thread: rows r and r + 8, columns c, c + 1 with r = 16 (t / 32) + (t % 32) / 4, c = 8 j + 2 (t % 4)
