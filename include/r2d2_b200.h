@@ -124,6 +124,19 @@ int r2d2_actor_priorities(const float* q, const float* q_next, const float* rew,
                           int B, int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max,
                           float* prio, r2d2_stream_t stream);
 
+/* Actor side, per env step: the four nets of N actor lanes stepped once (Actor.run, actor.py:149-154).
+ * shape: O, A, H (is_critic ignored).  params: flat blocks of actor, target_actor, critic, target_critic (the critics'
+ * I = O + A).  obs [N,O]; state_in, state_out [4,2,N,H] in that net order, (hx, cx) - the replay's state layout;
+ * they must not alias.  mu [N,A] = tanh(l3(tanh(h'))) of the actor, before any exploration noise.  The critics are fed
+ * cat(obs, mu) and the target critic cat(obs, mu_t); the critics' heads are not computed (the reference discards them).
+ * fp32 FMA on the flat weights; lane n's outputs are bitwise independent of N and of the other lanes.  Five kernel
+ * launches on `stream`, no host synchronisation.  Supported: 1 <= N <= 256, H a multiple of 32 up to 512, 1 <= A <= 64;
+ * other shapes return R2D2_ERR_UNSUPPORTED.  workspace: r2d2_policy_workspace_floats(shape, N) floats. */
+size_t r2d2_policy_workspace_floats(const r2d2_net_shape* shape, int N);
+int r2d2_policy_step(const r2d2_net_shape* shape, const float* const params[4], const float* obs,
+                     const float* state_in, float* state_out, float* mu, int N, float* workspace,
+                     r2d2_stream_t stream);
+
 /* torch.optim.Adam defaults (learner.py:50-53,114,128) on a flat buffer; grad is multiplied by grad_scale first. */
 int r2d2_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, int step,
                    float lr, float beta1, float beta2, float eps, float grad_scale, r2d2_stream_t stream);

@@ -7,6 +7,7 @@
 #include "learner.cuh"
 #include "lstm_scan.cuh"
 #include "net.cuh"
+#include "policy.cuh"
 #include "replay.cuh"
 
 namespace r2d2 {
@@ -152,6 +153,18 @@ int r2d2_actor_priorities(const float* q, const float* q_next, const float* rew,
                           int B, int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max,
                           float* prio, r2d2_stream_t stream) {
   return actor_priorities(q, q_next, rew, term, n_rows, B, A, burn_in, learning, n_step, gamma, eta, p_max, prio, S(stream));
+}
+
+size_t r2d2_policy_workspace_floats(const r2d2_net_shape* shape, int N) {
+  return shape && N > 0 ? policy_workspace_floats(shape->obs_size, shape->n_actions, shape->hidden, N) : 0;
+}
+
+int r2d2_policy_step(const r2d2_net_shape* shape, const float* const params[4], const float* obs,
+                     const float* state_in, float* state_out, float* mu, int N, float* workspace,
+                     r2d2_stream_t stream) {
+  R2D2_REQUIRE(shape, "null");
+  return policy_step(shape->obs_size, shape->n_actions, shape->hidden, params, obs, state_in, state_out, mu, N,
+                     workspace, S(stream));
 }
 
 int r2d2_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, int step,

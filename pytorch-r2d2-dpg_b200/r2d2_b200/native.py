@@ -90,6 +90,9 @@ SIGNATURES = {
     "r2d2_nstep_rewards": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "r2d2_actor_priorities": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                       c_float, c_float, c_int, c_void_p, c_void_p]),
+    "r2d2_policy_workspace_floats": (c_size_t, [POINTER(NetShape), c_int]),
+    "r2d2_policy_step": (c_int, [POINTER(NetShape), POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                 c_void_p, c_void_p]),
     "r2d2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_float, c_float, c_float,
                                c_float, c_float, c_void_p]),
     "r2d2_replay_create": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig)]),

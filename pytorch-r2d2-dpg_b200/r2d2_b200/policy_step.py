@@ -1,0 +1,121 @@
+"""Actor side, per env step: the four recurrent nets of N actor lanes stepped once on the GPU (r2d2_policy_step,
+csrc/policy.cu), the batched form of what every reference actor does on the CPU at batch 1 (actor.py:149-154):
+
+    action = actor(x); critic(x, action); target_critic(x, target_actor(x))
+
+`PolicyStepper` keeps the four flat parameter blocks and a ring of recurrent states on the device.  Per env step the
+only host<->device traffic is obs in and mu out; an episode's state history crosses PCIe once, when it is read back
+with `episode_states`.
+"""
+from __future__ import annotations
+
+from ctypes import c_void_p
+
+import numpy as np
+import torch
+
+from . import native as nv
+from .actor_priority import _flat
+
+NETS = ("actor", "target_actor", "critic", "target_critic")   # the replay's state order (actor.py:149,166)
+
+
+def policy_step(params, obs, state_in, state_out, mu, workspace=None):
+    """One step on CUDA tensors: params = 4 flat blocks (NETS order), obs [N,O], state_in / state_out [4,2,N,H],
+    mu [N,A] (written).  Launches on the current stream and does not synchronise."""
+    N, O = obs.shape
+    A, H = mu.shape[1], state_in.shape[3]
+    lib = nv.lib()
+    shape = nv.NetShape(O, A, H, 0)
+    if workspace is None:
+        workspace = torch.empty(max(1, lib.r2d2_policy_workspace_floats(nv.byref(shape), N)), device=obs.device)
+    ptrs = (c_void_p * 4)(*[nv.dptr(p).value for p in params])
+    nv.check(lib.r2d2_policy_step(nv.byref(shape), ptrs, nv.dptr(obs), nv.dptr(state_in), nv.dptr(state_out),
+                                  nv.dptr(mu), N, nv.dptr(workspace), nv.current_stream()))
+
+
+class StateRing:
+    """Recurrent state history of N lanes: `ring[(M + 1), 4, 2, N, H]`, where pool step k reads slot k mod (M + 1) and
+    writes slot k + 1.  A lane's episode that began at step `start[lane]` keeps its states while it has at most
+    M = max_episode_steps steps.  Subclasses implement `load(model_dict)` and `_step(obs, state_in, state_out)`."""
+
+    def __init__(self, obs_size, n_actions, hidden, n_lanes, device, max_episode_steps):
+        self.obs_size, self.n_actions, self.hidden, self.n_lanes = obs_size, n_actions, hidden, n_lanes
+        self.max_episode_steps = int(max_episode_steps)
+        self.device = torch.device(device)
+        self.ring = torch.zeros((self.max_episode_steps + 1, 4, 2, n_lanes, hidden), device=self.device)
+        self.t = 0                                   # steps taken so far
+        self.start = np.zeros(n_lanes, np.int64)    # step at which each lane's current episode began
+
+    def _slot(self, k):
+        return k % (self.max_episode_steps + 1)
+
+    def reset(self, lanes):
+        """Zero state for these lanes (models.py:34-36); their episodes begin at the next step."""
+        s = self._slot(self.t)
+        for lane in lanes:
+            self.ring[s, :, :, lane].zero_()
+            self.start[lane] = self.t
+
+    def current_states(self):
+        """[4,2,N,H] view of the states the next step reads."""
+        return self.ring[self._slot(self.t)]
+
+    def step(self, obs):
+        """obs [N,O] host array -> mu [N,A] host array (the actor's output before exploration noise)."""
+        long_lanes = np.nonzero(self.t - self.start + 1 > self.max_episode_steps)[0]
+        if len(long_lanes):
+            raise RuntimeError("episode of lane %d has outgrown max_episode_steps=%d: raise max_episode_steps"
+                               % (int(long_lanes[0]), self.max_episode_steps))
+        mu = self._step(obs, self.ring[self._slot(self.t)], self.ring[self._slot(self.t + 1)])
+        self.t += 1
+        return mu
+
+    def episode_states(self, lane, first, last):
+        """States of `lane` before steps first .. last-1 -> host float32 [last - first, 4, 2, H]."""
+        if not (self.start[lane] <= first <= last <= self.t):
+            raise ValueError("steps [%d, %d) are not in lane %d's current episode [%d, %d)"
+                             % (first, last, lane, int(self.start[lane]), self.t))
+        a, n = self._slot(first), last - first
+        if a + n <= self.max_episode_steps + 1:
+            st = self.ring[a:a + n, :, :, lane]
+        else:
+            st = torch.cat((self.ring[a:, :, :, lane], self.ring[:a + n - self.max_episode_steps - 1, :, :, lane]))
+        return st.to("cpu", copy=True).numpy()           # never a view of the ring (a CPU ring is reused)
+
+
+class PolicyStepper(StateRing):
+    """r2d2_policy_step for n_lanes lanes on one GPU, with pinned obs / mu staging buffers."""
+
+    def __init__(self, obs_size, n_actions, hidden, n_lanes, device=None, max_episode_steps=1000):
+        if not torch.cuda.is_available():
+            raise nv.NativeError("PolicyStepper needs a CUDA device; there is no CPU fallback")
+        dev = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
+        super().__init__(obs_size, n_actions, hidden, n_lanes, dev, max_episode_steps)
+        lib = nv.lib()
+        counts = [lib.r2d2_net_param_count(nv.byref(nv.NetShape(obs_size, n_actions, hidden, int(k >= 2))))
+                  for k in range(4)]
+        self.params = [torch.zeros(c, device=dev) for c in counts]
+        shape = nv.NetShape(obs_size, n_actions, hidden, 0)
+        self.workspace = torch.empty(lib.r2d2_policy_workspace_floats(nv.byref(shape), n_lanes), device=dev)
+        self.obs_host = torch.empty((n_lanes, obs_size), pin_memory=True)
+        self.mu_host = torch.empty((n_lanes, n_actions), pin_memory=True)
+        self.obs_dev = torch.empty((n_lanes, obs_size), device=dev)
+        self.mu_dev = torch.empty((n_lanes, n_actions), device=dev)
+
+    def load(self, model_dict):
+        """model.pt dict {'actor', 'target_actor', 'critic', 'target_critic'} -> the four flat blocks (plain copies)."""
+        for p, name in zip(self.params, NETS):
+            flat = _flat(model_dict[name], self.device)
+            if flat.numel() != p.numel():
+                raise ValueError("%s: %d parameters, the stepper was built for %d" % (name, flat.numel(), p.numel()))
+            p.copy_(flat)
+
+    def _step(self, obs, state_in, state_out):
+        self.obs_host.numpy()[:] = obs
+        with torch.cuda.device(self.device):
+            self.obs_dev.copy_(self.obs_host, non_blocking=True)
+            policy_step(self.params, self.obs_dev, state_in, state_out, self.mu_dev, self.workspace)
+            self.mu_host.copy_(self.mu_dev, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        return self.mu_host.numpy().copy()
