@@ -111,6 +111,13 @@ int r2d2_scan_status(int* status, r2d2_stream_t stream);
 int r2d2_td_priority(const float* q, const float* q_next, const float* rew, const float* term, int L, int B,
                      int A, int burn_in, int n_step, float gamma, float eta, float* target, float* dq,
                      float* td_sq, float* priority, float* critic_loss, r2d2_stream_t stream);
+/* The same with importance-sampling weights is_weight [B] (DEVICE, from r2d2_replay_sample_weighted; NULL = all 1):
+ * dq = w_b * 2 (q - y) / (L*B*A) and critic_loss = sum w_b td_sq / (L*B).  td_sq and priority stay unweighted (a
+ * sequence's priority does not depend on how it was drawn).  w = 1 gives the bits of r2d2_td_priority. */
+int r2d2_td_priority_weighted(const float* q, const float* q_next, const float* rew, const float* term,
+                              const float* is_weight, int L, int B, int A, int burn_in, int n_step, float gamma, float eta,
+                              float* target, float* dq, float* td_sq, float* priority, float* critic_loss,
+                              r2d2_stream_t stream);
 
 /* Actor-side rows of the path (SURVEY 8f N2), batched over finished episodes (one episode per batch column, time-major,
  * zero padded): n-step discounted reward pre-sum (actor.py:74-76; rows i < n_rows[b] - n_step, later rows copied) and
@@ -158,6 +165,11 @@ typedef struct {
 
 int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg);
 int r2d2_replay_destroy(r2d2_replay_t* r);
+/* Priority exponent alpha in [0, 1] (prioritized replay; default 1 = the raw priority): every leaf the shard writes -
+ * ingest and r2d2_replay_update_priorities - holds p > 0 ? p^alpha : 0, so P(start) = p^alpha / sum p^alpha and rows
+ * that start no sequence stay undrawable even at alpha = 0 (uniform over valid starts).  Callers keep passing raw
+ * priorities.  Only while the shard holds no episode (else R2D2_ERR_STATE); alpha outside [0, 1] is R2D2_ERR_ARG. */
+int r2d2_replay_set_priority_exponent(r2d2_replay_t* r, float alpha);
 
 /* Append one episode (replay_memory.py:141-152).  HOST pointers: obs [n_rows,O], act [n_rows,A], rew [n_rows],
  * term [n_rows] (n_rows includes the n_step pad rows, actor.py:173), states [n_state_rows,4,2,H]
@@ -184,12 +196,21 @@ int r2d2_replay_add_episodes(r2d2_replay_t* r, int n_episodes, const int* n_rows
 int r2d2_replay_sample(r2d2_replay_t* r, const float* u, int batch, long long* leaf_idx, float* obs, float* act,
                        float* rew, float* term, float* states, r2d2_stream_t stream);
 
+/* r2d2_replay_sample plus importance-sampling weights (prioritized replay), DEVICE is_weight [batch]:
+ * is_weight[b] = (min_b' leaf_b' / leaf_b)^beta = (N P_b)^-beta / max_b' (N P_b')^-beta, leaf = the stored p^alpha,
+ * normalised over this batch (the largest weight is exactly 1).  beta in [0, 1]; beta = 0 writes 1 everywhere.
+ * Same draw and gather as r2d2_replay_sample, one extra single-CTA kernel. */
+int r2d2_replay_sample_weighted(r2d2_replay_t* r, const float* u, int batch, float beta, long long* leaf_idx,
+                                float* is_weight, float* obs, float* act, float* rew, float* term, float* states,
+                                r2d2_stream_t stream);
+
 /* The gather half alone, for start rows the caller chose (DEVICE int64 leaf_idx): same outputs as r2d2_replay_sample. */
 int r2d2_replay_gather(r2d2_replay_t* r, const long long* leaf_idx, int batch, float* obs, float* act, float* rew,
                        float* term, float* states, r2d2_stream_t stream);
 
 /* priority[leaf_idx[i]] = prio[i] (DEVICE arrays; on duplicates the highest i wins, like the python
- * loop at learner.py:136-139) and recompute the touched tree paths. */
+ * loop at learner.py:136-139) and recompute the touched tree paths.  The leaf stores prio[i]^alpha under a
+ * priority exponent (r2d2_replay_set_priority_exponent). */
 int r2d2_replay_update_priorities(r2d2_replay_t* r, const long long* leaf_idx, const float* prio, int batch,
                                   r2d2_stream_t stream);
 
@@ -250,6 +271,11 @@ int r2d2_learner_buffers_get(r2d2_learner_t* l, r2d2_learner_buffers* out);
  * finish phase copies the weights into the target nets and that finish phase (the targets would be stale). */
 int r2d2_learner_buffers_get_slot(r2d2_learner_t* l, int slot, r2d2_learner_buffers* out);
 int r2d2_learner_select_batch(r2d2_learner_t* l, int slot);
+/* Importance weights of a batch slot: [B] floats next to leaf_idx / uniforms (fill them with
+ * r2d2_replay_sample_weighted or memcpy; 1 after create).  The critic phase reads the selected slot's weights only
+ * while importance weighting is on; off (the default) it runs the unweighted TD kernels. */
+int r2d2_learner_is_weights(r2d2_learner_t* l, int slot, float** out);
+int r2d2_learner_set_importance_weighting(r2d2_learner_t* l, int on);
 int r2d2_learner_target_phase(r2d2_learner_t* l, int slot, r2d2_stream_t stream);
 /* forget a target phase that ran ahead: the caller is about to overwrite that slot's batch */
 int r2d2_learner_discard_prefetch(r2d2_learner_t* l, r2d2_stream_t stream);

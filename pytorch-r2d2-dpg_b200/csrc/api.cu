@@ -145,6 +145,19 @@ int r2d2_td_priority(const float* q, const float* q_next, const float* rew, cons
   return td_priority(p, S(stream));
 }
 
+int r2d2_td_priority_weighted(const float* q, const float* q_next, const float* rew, const float* term,
+                              const float* is_weight, int L, int B, int A, int burn_in, int n_step, float gamma, float eta,
+                              float* target, float* dq, float* td_sq, float* priority, float* critic_loss,
+                              r2d2_stream_t stream) {
+  TdPriorityParams p;
+  p.q = q; p.q_next = q_next; p.rew = rew; p.term = term; p.target = target; p.dq = dq; p.td_sq = td_sq;
+  p.priority = priority; p.loss_sum = critic_loss; p.L = L; p.B = B; p.A = A; p.burn_in = burn_in; p.n_step = n_step;
+  p.gamma_n = (float)pow((double)gamma, (double)n_step);
+  p.eta = eta;
+  p.is_weight = is_weight;
+  return td_priority(p, S(stream));
+}
+
 int r2d2_nstep_rewards(const float* raw, const int* n_rows, int T, int B, int n_step, float gamma, float* out,
                        r2d2_stream_t stream) {
   return nstep_rewards(raw, n_rows, T, B, n_step, gamma, out, S(stream));
@@ -177,6 +190,9 @@ int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg) {
   return replay_create(reinterpret_cast<Replay**>(out), cfg);
 }
 int r2d2_replay_destroy(r2d2_replay_t* r) { return replay_destroy(reinterpret_cast<Replay*>(r)); }
+int r2d2_replay_set_priority_exponent(r2d2_replay_t* r, float alpha) {
+  return replay_set_priority_exponent(reinterpret_cast<Replay*>(r), alpha);
+}
 int r2d2_replay_add_episode(r2d2_replay_t* r, const float* obs, const float* act, const float* rew,
                             const float* term, const float* states, int n_rows, int n_state_rows,
                             const float* priority, int n_starts, r2d2_stream_t stream) {
@@ -193,6 +209,12 @@ int r2d2_replay_add_episodes(r2d2_replay_t* r, int n_episodes, const int* n_rows
 int r2d2_replay_sample(r2d2_replay_t* r, const float* u, int batch, long long* leaf_idx, float* obs, float* act,
                        float* rew, float* term, float* states, r2d2_stream_t stream) {
   return replay_sample(reinterpret_cast<Replay*>(r), u, batch, leaf_idx, obs, act, rew, term, states, S(stream));
+}
+int r2d2_replay_sample_weighted(r2d2_replay_t* r, const float* u, int batch, float beta, long long* leaf_idx,
+                                float* is_weight, float* obs, float* act, float* rew, float* term, float* states,
+                                r2d2_stream_t stream) {
+  return replay_sample_weighted(reinterpret_cast<Replay*>(r), u, batch, beta, leaf_idx, is_weight, obs, act, rew, term,
+                                states, S(stream));
 }
 int r2d2_replay_gather(r2d2_replay_t* r, const long long* leaf_idx, int batch, float* obs, float* act, float* rew,
                        float* term, float* states, r2d2_stream_t stream) {
@@ -233,6 +255,16 @@ int r2d2_learner_buffers_get_slot(r2d2_learner_t* lh, int slot, r2d2_learner_buf
   const Learner::BatchSlot& b = l->slots[slot];
   o->obs = b.obs; o->act = b.act; o->rew = b.rew; o->term = b.term; o->states = b.states;
   o->leaf_idx = b.leaf_idx; o->uniforms = b.uniforms;
+  return R2D2_OK;
+}
+int r2d2_learner_is_weights(r2d2_learner_t* lh, int slot, float** out) {
+  R2D2_REQUIRE(lh && out && (slot == 0 || slot == 1), "batch slot");
+  *out = reinterpret_cast<Learner*>(lh)->slots[slot].is_weight;
+  return R2D2_OK;
+}
+int r2d2_learner_set_importance_weighting(r2d2_learner_t* l, int on) {
+  R2D2_REQUIRE(l, "null");
+  reinterpret_cast<Learner*>(l)->importance_weighting = on != 0;
   return R2D2_OK;
 }
 int r2d2_learner_select_batch(r2d2_learner_t* l, int slot) {

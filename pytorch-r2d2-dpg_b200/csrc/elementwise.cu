@@ -28,6 +28,9 @@ __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPri
   const float grad_scale = 2.0f / ((float)L * (float)B * (float)A);
   float run_max = -INFINITY, run_sum = 0.f, sq_total = 0.f;
   if (b < B) {
+    // importance weight of sequence b: scales its share of the loss and of dq; td_sq and the priority stay unweighted
+    const float wb = p.is_weight ? __ldg(p.is_weight + b) : 1.0f;
+    const float gs = grad_scale * wb;
     for (int i = w; i < L; i += TD_WARPS) {
       const float r = __ldg(p.rew + (size_t)(p.burn_in + i) * B + b);
       const float d = __ldg(p.term + (size_t)(p.burn_in + i + p.n_step - 1) * B + b);
@@ -39,10 +42,10 @@ __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPri
         const float y = value_rescale(r + cont * __ldg(p.q_next + base + a));
         const float diff = q - y;
         if (p.target) p.target[base + a] = y;
-        if (p.dq) p.dq[base + a] = grad_scale * diff;
+        if (p.dq) p.dq[base + a] = gs * diff;
         sq += diff * diff;
       }
-      sq_total += sq;
+      sq_total += wb * sq;
       const float td = sq * inv_a;
       if (p.td_sq) p.td_sq[(size_t)i * B + b] = td;
       // learner.py:137 `average_td_loss[b:-1:B]` drops flat index L*B-1, i.e. (i=L-1, b=B-1)
@@ -101,12 +104,13 @@ __global__ void __launch_bounds__(TD1_WARPS * 32) td_elem_kernel(TdPriorityParam
     const float r = __ldg(p.rew + (size_t)(p.burn_in + i) * B + b);
     const float d = __ldg(p.term + (size_t)(p.burn_in + i + p.n_step - 1) * B + b);
     const float cont = p.gamma_n * (1.0f - d);
+    const float gs = grad_scale * (p.is_weight ? __ldg(p.is_weight + b) : 1.0f);   // w = 1: exactly grad_scale
     float sq = 0.f;
     for (int a = 0; a < A; ++a) {
       const float y = value_rescale(r + cont * sn_[lane * A + a]);
       const float diff = sq_[lane * A + a] - y;
       sn_[lane * A + a] = y;
-      sq_[lane * A + a] = grad_scale * diff;
+      sq_[lane * A + a] = gs * diff;
       sq += diff * diff;
     }
     p.td_sq[(size_t)i * B + b] = sq / (float)A;
@@ -123,9 +127,10 @@ __global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityPar
   const int L = p.L, B = p.B;
   float run_max = -INFINITY, run_sum = 0.f, tot = 0.f;
   if (b < B) {
+    const float wb = p.is_weight ? __ldg(p.is_weight + b) : 1.0f;   // w = 1: w * td + tot rounds like td + tot
     for (int i = w; i < L; i += TD2_WARPS) {
       const float td = p.td_sq[(size_t)i * B + b];
-      tot += td;
+      tot += wb * td;
       // learner.py:137 `average_td_loss[b:-1:B]` drops flat index L*B-1, i.e. (i=L-1, b=B-1)
       if (!(i == L - 1 && b == B - 1)) { run_max = fmaxf(run_max, td); run_sum += td; }
     }
@@ -141,7 +146,7 @@ __global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityPar
       const int count = L - ((b == B - 1) ? 1 : 0);
       p.priority[b] = p.eta * mx + (1.0f - p.eta) * (sm / (float)count);  // utils.py:17-18
     }
-    tt = warp_sum(tt);   // critic loss = mean over (i, b, a) of diff^2 = sum of td_sq / (L * B)
+    tt = warp_sum(tt);   // critic loss = mean over (i, b, a) of w_b diff^2 = sum of w_b td_sq / (L * B)
     if (lane == 0 && loss_part) loss_part[blockIdx.x] = tt / ((float)L * (float)B);
   }
 }

@@ -13,6 +13,8 @@ struct TdPriorityParams {
   float* td_sq = nullptr;          // [L,B] mean over A of squared TD (optional)
   float* priority = nullptr;       // [B] eta*max + (1-eta)*mean over the [b:-1:B] slice (optional)
   float* loss_sum = nullptr;       // scalar: MSE-mean critic loss (zeroed by the call, optional)
+  const float* is_weight = nullptr; // [B] importance weights w_b (optional): loss = sum w_b td_sq / (L*B), dq scaled by
+                                    // w_b; td_sq and priority stay unweighted.  NULL: every w_b = 1, same bits
   int L = 0, B = 0, A = 0, burn_in = 0, n_step = 0;
   float gamma_n = 0.f;             // gamma ** n_step
   float eta = 0.9f;

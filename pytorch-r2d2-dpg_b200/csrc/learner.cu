@@ -49,6 +49,7 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
   const size_t ws_c1 = ChainWs::floats(l->critic_sh, Tc, B, 1), ws_a1 = ChainWs::floats(l->actor_sh, L, B, 2);
   const size_t ws_c2 = ChainWs::floats(l->critic_sh, L, B, 1);
   total += ws_ta + ws_tc + ws_c1 + ws_a1 + ws_c2;
+  total += 2 * align64(B);   // importance weights of the two slots, carved last: the buffers above keep their offsets
   R2D2_CUDA_TRY(cudaMalloc(&l->arena, total * sizeof(float)));
   R2D2_CUDA_TRY(cudaMemset(l->arena, 0, total * sizeof(float)));
   l->arena_floats = total;
@@ -71,6 +72,12 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
   l->ws_c2 = ChainWs::carve(take(ws_c2), l->critic_sh, L, B, 1);
   l->ws_ta.inference_only = true;  // target nets: no BPTT, the scan keeps only what the heads read (learner.py:94-95,106)
   l->ws_tc.inference_only = true;
+  for (auto& b : l->slots) {
+    b.is_weight = take(B);
+    R2D2_TRY(fill_f32(b.is_weight, B, 1.0f, 0));
+  }
+  R2D2_CUDA_TRY(cudaStreamSynchronize(0));
+  learner_select_batch(l, 0);
   {   // R2D2_OVERLAP_INPUTS=0 disables the side stream (A/B)
     const char* e = getenv("R2D2_OVERLAP_INPUTS");
     l->overlap_inputs = !(e && e[0] == '0');
@@ -104,7 +111,7 @@ int learner_select_batch(Learner* l, int slot) {
   const Learner::BatchSlot& b = l->slots[slot];
   l->cur_slot = slot;
   l->obs = b.obs; l->act = b.act; l->rew = b.rew; l->term = b.term; l->states = b.states; l->uniforms = b.uniforms;
-  l->leaf_idx = b.leaf_idx;
+  l->leaf_idx = b.leaf_idx; l->is_weight = b.is_weight;
   return R2D2_OK;
 }
 
@@ -207,6 +214,7 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
   tp.L = L; tp.B = B; tp.A = A; tp.burn_in = Bn; tp.n_step = n;
   tp.gamma_n = (float)std::pow((double)c.gamma, (double)n);
   tp.eta = c.eta;
+  tp.is_weight = l->importance_weighting ? l->is_weight : nullptr;
   R2D2_TRY(td_priority(tp, st));
 
   R2D2_CUDA_TRY(cudaMemsetAsync(c.critic_grads, 0, sizeof(float) * l->critic_sh.param_count(), st));

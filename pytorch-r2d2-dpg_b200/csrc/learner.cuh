@@ -29,6 +29,7 @@ struct Learner {
   struct BatchSlot {
     float *obs = nullptr, *act = nullptr, *rew = nullptr, *term = nullptr, *states = nullptr, *uniforms = nullptr;
     long long* leaf_idx = nullptr;
+    float* is_weight = nullptr;   // [B] importance weights of the batch (r2d2_replay_sample_weighted), 1 by default
   } slots[2];
   int cur_slot = 0;
   int targets_slot = -1;        // slot whose target-chain outputs (q_next) are current; -1: none
@@ -37,6 +38,8 @@ struct Learner {
   bool target_phase_standalone = false;
   float *obs = nullptr, *act = nullptr, *rew = nullptr, *term = nullptr, *states = nullptr, *uniforms = nullptr;
   long long* leaf_idx = nullptr;
+  float* is_weight = nullptr;
+  bool importance_weighting = false;   // the TD kernels read is_weight (off: NULL, the unweighted loss)
   // intermediates / results
   float *act_tc = nullptr, *q = nullptr, *q_next = nullptr, *target = nullptr, *dq = nullptr, *mu = nullptr,
         *q_pi = nullptr, *dq_pi = nullptr, *dpre_actor = nullptr, *td_sq = nullptr, *priority = nullptr,

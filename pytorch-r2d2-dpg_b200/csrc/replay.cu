@@ -18,27 +18,30 @@ namespace r2d2 {
 
 namespace {
 
+// kLeafValue: also return the value of the drawn leaf (the weighted draw turns it into an importance weight)
+template <bool kLeafValue>
 __global__ void __launch_bounds__(256) tree_sample_kernel(TreeView tv, const float* __restrict__ u, int batch,
-                                                          long long* __restrict__ leaf) {
+                                                          long long* __restrict__ leaf, float* __restrict__ leaf_val) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= batch) return;
   const int top = tv.levels - 1;
   const float total = tv.lvl[top][0];
   float r = __fmul_rn(u[i], total);
   long long idx = 0;
+  float v = 0.f;   // value of the picked child; after the level-1 pass that is the leaf itself
   for (int l = top; l >= 1; --l) {
     const float4* ch4 = reinterpret_cast<const float4*>(tv.lvl[l - 1] + idx * TREE_K);
     float c[TREE_K];
 #pragma unroll
     for (int k = 0; k < TREE_K / 4; ++k) {
-      const float4 v = ch4[k];
-      c[4 * k] = v.x; c[4 * k + 1] = v.y; c[4 * k + 2] = v.z; c[4 * k + 3] = v.w;
+      const float4 v4 = ch4[k];
+      c[4 * k] = v4.x; c[4 * k + 1] = v4.y; c[4 * k + 2] = v4.z; c[4 * k + 3] = v4.w;
     }
     int pick = -1;
 #pragma unroll
     for (int k = 0; k < TREE_K; ++k) {
       if (pick < 0) {
-        if (r < c[k]) pick = k;
+        if (r < c[k]) { pick = k; if (kLeafValue) v = c[k]; }
         else r = __fsub_rn(r, c[k]);
       }
     }
@@ -49,10 +52,44 @@ __global__ void __launch_bounds__(256) tree_sample_kernel(TreeView tv, const flo
         if (c[k] > 0.f) { pick = k; cl = c[k]; }
       if (pick < 0) pick = 0;
       r = __fmul_rn(cl, 0.99999994f);
+      if (kLeafValue) v = cl;
     }
     idx = idx * TREE_K + pick;
   }
   leaf[i] = idx;
+  if (kLeafValue) leaf_val[i] = v;
+}
+
+// Leaf stored for a priority p under the exponent alpha.  Zero stays zero (rows that start no sequence must stay
+// undrawable, also at alpha = 0 where powf(0, 0) would be 1).
+__device__ __forceinline__ float raise_priority(float p, float alpha) { return p > 0.f ? powf(p, alpha) : 0.f; }
+
+__global__ void __launch_bounds__(256) raise_leaves_kernel(float* __restrict__ leaves, long long n, float alpha) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i < n) leaves[i] = raise_priority(leaves[i], alpha);
+}
+
+// Single CTA, in place: w[b] holds the drawn leaf value and becomes (min_b' w[b'] / w[b])^beta = (N P_b)^-beta
+// normalised by its batch maximum.  The min is order-independent, so the weights do not depend on the thread
+// schedule and the smallest leaf of the batch gets exactly 1.  Every index is read and written by the same thread.
+// A leaf of 0 (only an all-zero tree can hand one out) gets weight 1 and takes no part in the min.
+constexpr int IS_WEIGHT_THREADS = 256;
+__global__ void __launch_bounds__(IS_WEIGHT_THREADS) is_weight_kernel(float* __restrict__ w, int batch, float beta) {
+  __shared__ float s_min[IS_WEIGHT_THREADS / 32];
+  float m = INFINITY;
+  for (int b = threadIdx.x; b < batch; b += blockDim.x)
+    if (w[b] > 0.f) m = fminf(m, w[b]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = s_min[0];
+#pragma unroll
+  for (int k = 1; k < IS_WEIGHT_THREADS / 32; ++k) m = fminf(m, s_min[k]);
+  for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+    const float leaf = w[b];
+    w[b] = (beta == 0.f || !(leaf > 0.f)) ? 1.0f : powf(__fdiv_rn(m, leaf), beta);
+  }
 }
 
 __device__ __forceinline__ float node_sum(const float* __restrict__ children) {
@@ -69,8 +106,10 @@ __device__ __forceinline__ float node_sum(const float* __restrict__ children) {
 // single CTA: write the batch's leaves (highest batch index wins on duplicates, learner.py:136-139
 // executes the writes in batch order), then refresh every ancestor level by level.  The leaf indices sit in shared
 // memory: the last-writer test is a broadcast scan of the later entries (B^2 / 2 shared reads instead of global ones).
+// kExponent: the shard stores p^alpha (r2d2_replay_set_priority_exponent); without it the leaf is prio[i] as given.
+template <bool kExponent>
 __global__ void __launch_bounds__(1024) tree_update_kernel(TreeView tv, const long long* __restrict__ leaf,
-                                                           const float* __restrict__ prio, int batch) {
+                                                           const float* __restrict__ prio, int batch, float alpha) {
   extern __shared__ long long s_leaf[];
   for (int i = threadIdx.x; i < batch; i += blockDim.x) s_leaf[i] = leaf[i];
   __syncthreads();
@@ -79,7 +118,10 @@ __global__ void __launch_bounds__(1024) tree_update_kernel(TreeView tv, const lo
     bool winner = true;
     for (int j = i + 1; j < batch; ++j)
       if (s_leaf[j] == li) { winner = false; break; }
-    if (winner) tv.lvl[0][li] = prio[i];
+    if (winner) {
+      if (kExponent) tv.lvl[0][li] = raise_priority(prio[i], alpha);
+      else tv.lvl[0][li] = prio[i];
+    }
   }
   __syncthreads();
   long long div = TREE_K;
@@ -178,6 +220,7 @@ struct Replay {
   long long sequence_counter = 0;
   long long rows_used = 0;
   long long evicted_total = 0;
+  float alpha = 1.0f;   // priority exponent: leaves hold p^alpha (1 = the raw priority, no pow on any path)
 };
 
 static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leaves, cudaStream_t stream) {
@@ -231,6 +274,26 @@ int replay_create(Replay** out, const r2d2_replay_config* cfg) {
   }
   r->tv.levels = levels;
   *out = r;
+  return R2D2_OK;
+}
+
+int replay_set_priority_exponent(Replay* r, float alpha) {
+  R2D2_REQUIRE(r, "null");
+  R2D2_REQUIRE(alpha >= 0.f && alpha <= 1.f, "priority exponent must lie in [0, 1]");
+  if (!r->episodes.empty()) {   // raw and exponentiated leaves in one tree would silently skew the draw
+    set_last_error("the priority exponent can only be set while the replay shard holds no episode");
+    return R2D2_ERR_STATE;
+  }
+  r->alpha = alpha;
+  return R2D2_OK;
+}
+
+// leaves [first, first + n) were just copied from the host as raw priorities: store p^alpha instead
+static int raise_fresh_leaves(Replay* r, long long first, long long n, cudaStream_t stream) {
+  if (r->alpha == 1.0f || n <= 0) return R2D2_OK;
+  raise_leaves_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(r->tv.lvl[0] + first, n, r->alpha);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;
 }
 
@@ -327,9 +390,11 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
   if (n_state_rows < n_rows)
     R2D2_CUDA_TRY(cudaMemsetAsync(r->state_rows + (start + n_state_rows) * 8 * H, 0,
                                   sizeof(float) * (size_t)(n_rows - n_state_rows) * 8 * H, stream));
-  if (n_starts > 0)
+  if (n_starts > 0) {
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + start, priority, sizeof(float) * (size_t)n_starts,
                                   cudaMemcpyHostToDevice, stream));
+    R2D2_TRY(raise_fresh_leaves(r, start, n_starts, stream));
+  }
   if (n_rows > n_starts)
     R2D2_CUDA_TRY(cudaMemsetAsync(r->tv.lvl[0] + start + n_starts, 0, sizeof(float) * (size_t)(n_rows - n_starts), stream));
   ranges.push_back({start, (long long)n_rows});
@@ -372,6 +437,7 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + run_start * 8 * H, states + src * 8 * H, sizeof(float) * n * 8 * H,
                                   cudaMemcpyHostToDevice, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + run_start, leaf_prio + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+    R2D2_TRY(raise_fresh_leaves(r, run_start, run_rows, stream));
     ranges.push_back({run_start, run_rows});
     src += run_rows;
     run_rows = 0;
@@ -418,7 +484,20 @@ int replay_sample(Replay* r, const float* u, int batch, long long* leaf_idx, flo
                   float* term, float* states, cudaStream_t stream) {
   R2D2_REQUIRE(r && u && leaf_idx && batch > 0, "args");
   R2D2_REQUIRE(!r->episodes.empty(), "replay is empty");
-  tree_sample_kernel<<<ceil_div(batch, 256), 256, 0, stream>>>(r->tv, u, batch, leaf_idx);
+  tree_sample_kernel<false><<<ceil_div(batch, 256), 256, 0, stream>>>(r->tv, u, batch, leaf_idx, nullptr);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return replay_gather(r, leaf_idx, batch, obs, act, rew, term, states, stream);
+}
+
+int replay_sample_weighted(Replay* r, const float* u, int batch, float beta, long long* leaf_idx, float* is_weight,
+                           float* obs, float* act, float* rew, float* term, float* states, cudaStream_t stream) {
+  R2D2_REQUIRE(r && u && leaf_idx && is_weight && batch > 0, "args");
+  R2D2_REQUIRE(beta >= 0.f && beta <= 1.f, "importance-sampling exponent must lie in [0, 1]");
+  R2D2_REQUIRE(!r->episodes.empty(), "replay is empty");
+  tree_sample_kernel<true><<<ceil_div(batch, 256), 256, 0, stream>>>(r->tv, u, batch, leaf_idx, is_weight);
+  count_launch();
+  is_weight_kernel<<<1, IS_WEIGHT_THREADS, 0, stream>>>(is_weight, batch, beta);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return replay_gather(r, leaf_idx, batch, obs, act, rew, term, states, stream);
@@ -427,7 +506,10 @@ int replay_sample(Replay* r, const float* u, int batch, long long* leaf_idx, flo
 int replay_update_priorities(Replay* r, const long long* leaf_idx, const float* prio, int batch, cudaStream_t stream) {
   R2D2_REQUIRE(r && leaf_idx && prio && batch > 0, "args");
   R2D2_REQUIRE(batch <= 5120, "priority batch larger than the shared-memory index table (40 KB)");
-  tree_update_kernel<<<1, 1024, sizeof(long long) * (size_t)batch, stream>>>(r->tv, leaf_idx, prio, batch);
+  if (r->alpha == 1.0f)
+    tree_update_kernel<false><<<1, 1024, sizeof(long long) * (size_t)batch, stream>>>(r->tv, leaf_idx, prio, batch, 1.0f);
+  else
+    tree_update_kernel<true><<<1, 1024, sizeof(long long) * (size_t)batch, stream>>>(r->tv, leaf_idx, prio, batch, r->alpha);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;

@@ -15,6 +15,7 @@ struct TreeView {
 struct Replay;
 int replay_create(Replay** out, const r2d2_replay_config* cfg);
 int replay_destroy(Replay* r);
+int replay_set_priority_exponent(Replay* r, float alpha);
 int replay_add_episode(Replay* r, const float* obs, const float* act, const float* rew, const float* term,
                        const float* states, int n_rows, int n_state_rows, const float* priority, int n_starts,
                        cudaStream_t stream);
@@ -24,6 +25,8 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
                         long long* sequence_counter_out, cudaStream_t stream);
 int replay_sample(Replay* r, const float* u, int batch, long long* leaf_idx, float* obs, float* act, float* rew,
                   float* term, float* states, cudaStream_t stream);
+int replay_sample_weighted(Replay* r, const float* u, int batch, float beta, long long* leaf_idx, float* is_weight,
+                           float* obs, float* act, float* rew, float* term, float* states, cudaStream_t stream);
 int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, float* act, float* rew, float* term,
                   float* states, cudaStream_t stream);
 int replay_update_priorities(Replay* r, const long long* leaf_idx, const float* prio, int batch, cudaStream_t stream);

@@ -13,6 +13,10 @@ WORLD_SIZE in the environment).  `Learner.__init__` then binds cuda:LOCAL_RANK, 
 ingests only the actors i with i mod WORLD_SIZE == RANK into its own HBM replay shard, and the two flat
 gradient blocks are summed over the ranks by the library's peer-memory kernels inside the iteration (csrc/peer.cu);
 rank 0 alone writes model.pt.  Nothing else crosses GPUs.
+
+Prioritized replay (R2D2's, absent from the reference): R2D2_PRIORITY_EXPONENT (alpha, default 1) and R2D2_IS_EXPONENT
+(beta, default 0) in the environment.  The defaults are the reference's behaviour; published R2D2 uses 0.9 / 0.6.
+Under data parallelism each rank normalises the weights over its own batch.
 """
 import os
 from time import sleep, time
@@ -70,15 +74,18 @@ class Learner:
         self.memory_update_interval = 50
         self.target_update_inverval = 500
         self.gamma, self.actor_lr, self.critic_lr = 0.997, 1e-4, 1e-3
+        self.priority_exponent = float(os.environ.get("R2D2_PRIORITY_EXPONENT", 1.0))
+        self.is_exponent = float(os.environ.get("R2D2_IS_EXPONENT", 0.0))
         cfg = PathConfig(obs=self.obs_size, act=self.n_actions, hidden=self.hidden, batch=self.batch_size,
                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
                          gamma=self.gamma, actor_lr=self.actor_lr, critic_lr=self.critic_lr,
-                         target_interval=self.target_update_inverval)
+                         target_interval=self.target_update_inverval, priority_exponent=self.priority_exponent,
+                         is_exponent=self.is_exponent)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
                                           obs_size=self.obs_size, n_actions=self.n_actions, hidden=self.hidden,
-                                          device=self.engine.device)
+                                          device=self.engine.device, priority_exponent=self.priority_exponent)
         self.state_path = self.model_path + 'learner_state.pt'
         if os.environ.get("R2D2_RESUME", "0") == "1" and os.path.isfile(self.state_path):
             self.load_checkpoint()                         # every rank loads the same file: replicas stay identical

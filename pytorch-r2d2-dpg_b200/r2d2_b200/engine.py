@@ -25,7 +25,11 @@ PARAM_KEYS = ("l1.weight", "l1.bias", "l2.weight_ih", "l2.weight_hh", "l2.bias_i
 
 @dataclass
 class PathConfig:
-    """Hyper-parameters of the path; defaults are the reference's literals (learner.py:29-34,43-49)."""
+    """Hyper-parameters of the path; defaults are the reference's literals (learner.py:29-34,43-49).
+
+    Prioritized replay (not in the reference, whose defaults these are): `priority_exponent` alpha - the replay shard
+    samples a start with probability p^alpha / sum p^alpha (published R2D2: 0.9) - and `is_exponent` beta - the critic
+    loss weights sequence b by (min_b' P_b' / P_b)^beta, normalised over the batch (R2D2: 0.6).  Both lie in [0, 1]."""
     obs: int
     act: int
     hidden: int = 128
@@ -38,6 +42,14 @@ class PathConfig:
     critic_lr: float = 1e-3
     eta: float = 0.9
     target_interval: int = 500
+    priority_exponent: float = 1.0
+    is_exponent: float = 0.0
+
+    def __post_init__(self):
+        for name in ("priority_exponent", "is_exponent"):
+            v = getattr(self, name)
+            if not 0.0 <= v <= 1.0:
+                raise ValueError("%s must lie in [0, 1], got %r" % (name, v))
 
     @property
     def rows(self) -> int:
@@ -125,9 +137,16 @@ class LearnerEngine:
                                 "states": nv.view_f32(b.states, (4, 2, B, H), dev),
                                 "leaf_idx": nv.view_i64(b.leaf_idx, (B,), dev),
                                 "uniforms": nv.view_f32(b.uniforms, (B,), dev)})
+            w = c_void_p()
+            nv.check(self.lib.r2d2_learner_is_weights(self._h, slot, byref(w)))
+            self._slots[-1]["is_weight"] = nv.view_f32(w.value, (B,), dev)
         self._lib_slot = 0
         self._targets_ahead = False      # the fill slot's target chains already ran: its batch must not change any more
         self._bind_slot(0)
+        # prioritized replay: the critic loss weights each sequence by the importance weight the draw wrote next to
+        # its leaf index (DeviceReplay.sample_into); off, the library runs the unweighted TD kernels
+        self.importance_weighting = cfg.is_exponent > 0
+        nv.check(self.lib.r2d2_learner_set_importance_weighting(self._h, int(self.importance_weighting)))
         self.q_value = nv.view_f32(b.q_value, (L * B, A), dev)
         self.target_q_value = nv.view_f32(b.target_q_value, (L * B, A), dev)
         self.td_sq = nv.view_f32(b.td_sq, (L * B,), dev)
@@ -287,7 +306,8 @@ class LearnerEngine:
 
     # ---- batch ------------------------------------------------------------------------------
     def set_batch(self, batch: dict):
-        """Copy an already sampled time-major batch (replay_memory.py:123-136 layout) into the engine."""
+        """Copy an already sampled time-major batch (replay_memory.py:123-136 layout) into the engine.  An optional
+        batch["is_weight"] [B] holds the importance weights; without it every weight is 1."""
         cv = lambda x: torch.as_tensor(np.asarray(x) if not isinstance(x, torch.Tensor) else x,  # noqa: E731
                                        dtype=torch.float32).to(self.device, non_blocking=True)
         self._guard_fill()
@@ -297,6 +317,10 @@ class LearnerEngine:
         self.term.copy_(cv(batch["term"]).reshape(self.term.shape))
         for i, k in enumerate(("a_state", "ta_state", "c_state", "tc_state")):
             self.states[i].copy_(cv(batch[k]))
+        if "is_weight" in batch:
+            self.is_weight.copy_(cv(batch["is_weight"]).reshape(self.is_weight.shape))
+        elif self.importance_weighting:
+            self.is_weight.fill_(1.0)
 
     # ---- one learner iteration (learner.py:86-132) on the batch currently in the engine ------------
     def step(self, prefetch=None):
@@ -365,7 +389,8 @@ class LearnerEngine:
 
     def _run_prefetch(self, prefetch):
         from types import SimpleNamespace
-        used = SimpleNamespace(leaf_idx=self.leaf_idx, priority=self.priority, losses=self.losses)
+        used = SimpleNamespace(leaf_idx=self.leaf_idx, priority=self.priority, losses=self.losses,
+                               is_weight=self.is_weight)
         self._bind_slot(1 - self._fill_slot)     # the phases still in flight keep reading the other slot
         prefetch(self, used)
 
@@ -426,6 +451,8 @@ class DeviceReplay:
                              int(capacity_rows), int(max_sequences))
         self._h = c_void_p()
         nv.check(self.lib.r2d2_replay_create(byref(self._h), byref(rc)))
+        if cfg.priority_exponent != 1.0:   # leaves hold p^alpha; actors and write-backs keep passing raw priorities
+            nv.check(self.lib.r2d2_replay_set_priority_exponent(self._h, float(cfg.priority_exponent)))
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h:
@@ -489,8 +516,11 @@ class DeviceReplay:
                                              None, None, None, nv.current_stream()))
         return leaf
 
-    def sample_into(self, eng: LearnerEngine, generator: torch.Generator | None = None, u: torch.Tensor | None = None):
-        """Draw eng.cfg.batch starts and gather the time-major batch straight into the engine's buffers."""
+    def sample_into(self, eng: LearnerEngine, generator: torch.Generator | None = None, u: torch.Tensor | None = None,
+                    beta: float | None = None):
+        """Draw eng.cfg.batch starts and gather the time-major batch straight into the engine's buffers.  With the
+        engine's importance weighting on, the draw also writes eng.is_weight with exponent `beta` (default
+        eng.cfg.is_exponent; pass it per draw to anneal it)."""
         ec, rc = eng.cfg, self.cfg
         eng._guard_fill()
         if (ec.obs, ec.act, ec.hidden, ec.rows) != (rc.obs, rc.act, rc.hidden, rc.rows):
@@ -500,12 +530,22 @@ class DeviceReplay:
             eng.uniforms.copy_(torch.rand(eng.cfg.batch, device=self.device, generator=generator))
         else:
             eng.uniforms.copy_(u)
+        if eng.importance_weighting:
+            b = ec.is_exponent if beta is None else float(beta)
+            if not 0.0 <= b <= 1.0:
+                raise ValueError("beta must lie in [0, 1], got %r" % (b,))
+            nv.check(self.lib.r2d2_replay_sample_weighted(self._h, nv.dptr(eng.uniforms), eng.cfg.batch, b,
+                                                          nv.dptr(eng.leaf_idx, torch.int64), nv.dptr(eng.is_weight),
+                                                          nv.dptr(eng.obs), nv.dptr(eng.act), nv.dptr(eng.rew),
+                                                          nv.dptr(eng.term), nv.dptr(eng.states), nv.current_stream()))
+            return
         nv.check(self.lib.r2d2_replay_sample(self._h, nv.dptr(eng.uniforms), eng.cfg.batch,
                                              nv.dptr(eng.leaf_idx, torch.int64), nv.dptr(eng.obs), nv.dptr(eng.act),
                                              nv.dptr(eng.rew), nv.dptr(eng.term), nv.dptr(eng.states),
                                              nv.current_stream()))
 
     def update_priorities(self, leaf_idx: torch.Tensor, prio: torch.Tensor):
+        """Write raw priorities back; the leaves store prio^alpha (PathConfig.priority_exponent)."""
         nv.check(self.lib.r2d2_replay_update_priorities(self._h, nv.dptr(leaf_idx, torch.int64), nv.dptr(prio),
                                                         leaf_idx.numel(), nv.current_stream()))
 

@@ -87,6 +87,9 @@ SIGNATURES = {
     "r2d2_scan_status": (c_int, [POINTER(c_int), c_void_p]),
     "r2d2_td_priority": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float,
                                  c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "r2d2_td_priority_weighted": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                          c_int, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p]),
     "r2d2_nstep_rewards": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "r2d2_actor_priorities": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                       c_float, c_float, c_int, c_void_p, c_void_p]),
@@ -97,12 +100,15 @@ SIGNATURES = {
                                c_float, c_float, c_void_p]),
     "r2d2_replay_create": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig)]),
     "r2d2_replay_destroy": (c_int, [c_void_p]),
+    "r2d2_replay_set_priority_exponent": (c_int, [c_void_p, c_float]),
     "r2d2_replay_add_episodes": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "r2d2_replay_add_episode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                         c_void_p, c_int, c_void_p]),
     "r2d2_replay_sample": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_void_p, c_void_p]),
+    "r2d2_replay_sample_weighted": (c_int, [c_void_p, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p]),
     "r2d2_replay_gather": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "r2d2_replay_update_priorities": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "r2d2_replay_stats": (c_int, [c_void_p, POINTER(ReplayStats), c_void_p]),
@@ -120,6 +126,8 @@ SIGNATURES = {
     "r2d2_learner_set_overlap_actor_inputs": (c_int, [c_void_p, c_int]),
     "r2d2_learner_buffers_get_slot": (c_int, [c_void_p, c_int, POINTER(LearnerBuffers)]),
     "r2d2_learner_select_batch": (c_int, [c_void_p, c_int]),
+    "r2d2_learner_is_weights": (c_int, [c_void_p, c_int, POINTER(c_void_p)]),
+    "r2d2_learner_set_importance_weighting": (c_int, [c_void_p, c_int]),
     "r2d2_learner_target_phase": (c_int, [c_void_p, c_int, c_void_p]),
     "r2d2_learner_discard_prefetch": (c_int, [c_void_p, c_void_p]),
     "r2d2_peer_layout_for": (c_int, [c_longlong, c_longlong, c_int, POINTER(PeerLayout)]),

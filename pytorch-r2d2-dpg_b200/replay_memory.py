@@ -6,7 +6,9 @@
                         replay_memory.py:67-175, but the storage is a replay shard in HBM with a sum tree
                         (r2d2_b200.engine.DeviceReplay -> csrc/replay.cu).  P(episode, sequence) is
                         proportional to priority[episode][sequence], the law of the reference's two-level
-                        WeightedRandomSampler draw (replay_memory.py:95-114).
+                        WeightedRandomSampler draw (replay_memory.py:95-114).  With a priority exponent alpha
+                        (R2D2_PRIORITY_EXPONENT, default 1 = the reference) the shard stores p^alpha instead:
+                        `priority[e][s]` reads the stored p^alpha, and a write of p through it stores p^alpha too.
 
 File format (actor.py:163-176, replay_memory.py:55-59): torch.save of
   {'replay_memory': deque[list[(obs f32[O], act f32[A], [reward], [terminal])]],
@@ -72,7 +74,8 @@ def pack_episode(rows, states, hidden=None):
 
 
 class _EpisodePriorities:
-    """`memory.priority[e]`: indexable / assignable view of one episode's leaf priorities in HBM."""
+    """`memory.priority[e]`: indexable / assignable view of one episode's leaf priorities in HBM.  Reads give the stored
+    leaf, p^alpha under a priority exponent; an assigned raw p goes through update_priorities and is raised as well."""
 
     def __init__(self, owner, e):
         self._o, self._e = owner, e
@@ -131,7 +134,7 @@ class _TotalPriority:
 
 class LearnerReplayMemory:
     def __init__(self, memory_sequence_size=500000, batch_size=32, obs_size=None, n_actions=None, hidden=128,
-                 capacity_rows=None, device=None):
+                 capacity_rows=None, device=None, priority_exponent=None):
         self.path = './memory_data/'
         self.memory_sequence_size = memory_sequence_size
         self.sequence_counter = 0
@@ -140,6 +143,10 @@ class LearnerReplayMemory:
         self.sequence_length = self.burn_in_length + self.learning_length
         self._hidden, self._obs, self._act = hidden, obs_size, n_actions
         self._capacity_rows, self._device = capacity_rows, device
+        if priority_exponent is None:
+            priority_exponent = float(os.environ.get("R2D2_PRIORITY_EXPONENT", 1.0))
+        self.priority_exponent = float(priority_exponent)
+        self._cfg()                                         # rejects an exponent outside [0, 1] before any ingest
         self._dev = None          # DeviceReplay, created when the row width is known
         self._episodes = deque()  # (row_start, n_rows, n_starts) in FIFO order, mirrors the native ring
         self.priority = _PriorityTable(self)
@@ -167,7 +174,8 @@ class LearnerReplayMemory:
     def _cfg(self):
         from r2d2_b200.engine import PathConfig
         return PathConfig(obs=self._obs, act=self._act, hidden=self._hidden, batch=self.batch_size,
-                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step)
+                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
+                          priority_exponent=self.priority_exponent)
 
     def _ensure_device(self, obs_size, n_actions, hidden):
         """Create the HBM shard on first use.  Sizes given to the constructor are binding: an actor file of another
