@@ -328,12 +328,7 @@ static int gemm_f32_dispatch(const GemmParams& p, GemmLayout layout, cudaStream_
   R2D2_REQUIRE(!p.bias2 || gemm_supports_bias2(p.M, p.N, p.K + p.K2), "bias2 needs the wgmma path (gemm_supports_bias2)");
   R2D2_REQUIRE((!p.C_img_k && !p.C_img_mn) || (layout == GEMM_NT && gemm_emits_operand_image(p.M, p.N, p.K + p.K2)),
                "C_img_* is produced by the small-K streaming kernel and the wgmma epilogue only (see gemm_emits_operand_image)");
-  if (gemm_get_impl() == 1 && !(skinny && gemm_get_impl_skinny_mma())) {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = getenv("R2D2_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
-    if (dbg) { GemmParams q = p; q.debug_flags = dbg; return gemm_f32_tc(q, layout, stream); }
-    return gemm_f32_tc(p, layout, stream);
-  }
+  if (gemm_get_impl() == 1 && !(skinny && gemm_get_impl_skinny_mma())) return gemm_f32_tc(p, layout, stream);
   switch (layout) {
     case GEMM_NT: return launch_gemm<GEMM_NT>(p, stream);
     case GEMM_NN: return launch_gemm<GEMM_NN>(p, stream);

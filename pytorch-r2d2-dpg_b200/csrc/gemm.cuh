@@ -45,7 +45,6 @@ struct GemmParams {
   float* colsum_b = nullptr;             // the bias gradient that goes with a weight gradient reads the same rows
   int reuse_packed_a = 0;    // wgmma path: A (pointer, shape, layout) is the operand the previous gemm_f32 call packed
                              // and its contents have not changed since -> skip the pack pass (dW_hh then dW_ih of a chain)
-  int debug_flags = 0;       // dev only (env R2D2_GEMM_DEBUG): 1 = producers skip fetch+convert, 2 = skip MMAs, 4 = skip epilogue stores
 };
 
 int gemm_f32(const GemmParams& p, GemmLayout layout, cudaStream_t stream);

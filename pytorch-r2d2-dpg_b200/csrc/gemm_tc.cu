@@ -94,7 +94,6 @@ struct PackedGemmParams {
   const float* Z; long long ldz;
   int epilogue, split_k;
   long long c_split_stride;  // split_k > 1: CTA z writes its partial product to C + z * c_split_stride
-  int debug_flags;
   unsigned char* c_img_k;    // optional: C also leaves as packed operand images (N % 32 == 0, split_k == 1), see epilogue
   unsigned char* c_img_mn;
 };
@@ -156,23 +155,21 @@ __global__ void __launch_bounds__(PACKED_GEMM_THREADS, CTAS_PER_SM) gemm_packed_
     const int s = i % STAGES;
     mbar_wait_spin(&full[s], (i / STAGES) & 1);
     const uint32_t sa = smem_base + s * STAGE_BYTES + a_half, sb = smem_base + s * STAGE_BYTES + TILE_BYTES;
-    if (!(p.debug_flags & 2)) {
-      sm90::fence_regs(acc);
-      sm90::wgmma_fence();
+    sm90::fence_regs(acc);
+    sm90::wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < TBK / 16; ++ks) {
-        const uint64_t a_hi = sm90::make_smem_desc(sa + ks * a_ks, a_lbo, a_sbo);
-        const uint64_t a_lo = sm90::make_smem_desc(sa + ks * a_ks + PLANE_BYTES, a_lbo, a_sbo);
-        const uint64_t b_hi = sm90::make_smem_desc(sb + ks * b_ks, b_lbo, b_sbo);
-        const uint64_t b_lo = sm90::make_smem_desc(sb + ks * b_ks + PLANE_BYTES, b_lbo, b_sbo);
-        sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_lo, b_hi);
-        sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_lo);
-        sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_hi);
-      }
-      sm90::wgmma_commit();
-      sm90::wgmma_wait<1>();   // k tile i - 1 is done, k tile i stays in flight
-      sm90::fence_regs(acc);
+    for (int ks = 0; ks < TBK / 16; ++ks) {
+      const uint64_t a_hi = sm90::make_smem_desc(sa + ks * a_ks, a_lbo, a_sbo);
+      const uint64_t a_lo = sm90::make_smem_desc(sa + ks * a_ks + PLANE_BYTES, a_lbo, a_sbo);
+      const uint64_t b_hi = sm90::make_smem_desc(sb + ks * b_ks, b_lbo, b_sbo);
+      const uint64_t b_lo = sm90::make_smem_desc(sb + ks * b_ks + PLANE_BYTES, b_lbo, b_sbo);
+      sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_lo, b_hi);
+      sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_lo);
+      sm90::wgmma_m64n128k16_bf16<A_MN, B_MN>(acc, a_hi, b_hi);
     }
+    sm90::wgmma_commit();
+    sm90::wgmma_wait<1>();   // k tile i - 1 is done, k tile i stays in flight
+    sm90::fence_regs(acc);
     __syncwarp();
     if (i > 0 && t == 0) sm90::mbar_arrive(&empty[(i - 1) % STAGES]);
   }
@@ -188,7 +185,6 @@ __global__ void __launch_bounds__(PACKED_GEMM_THREADS, CTAS_PER_SM) gemm_packed_
   float* const C = p.C + (long long)blockIdx.z * p.c_split_stride;
   const bool vec_c = ((reinterpret_cast<uintptr_t>(C) & 7) == 0) && (p.ldc % 2 == 0);
   const bool img = p.c_img_k != nullptr || p.c_img_mn != nullptr;   // kernel-uniform
-  if (p.debug_flags & 4) return;
 #pragma unroll
   for (int j = 0; j < TBN / 8; ++j) {
     const int col = n0 + 8 * j + c_off;
@@ -351,7 +347,6 @@ int gemm_f32_tc(const GemmParams& p, GemmLayout layout, cudaStream_t stream) {
   PackedGemmParams q;
   q.pa = p.A_img ? p.A_img : g_pack_a.ptr; q.pb = p.B_img ? p.B_img : g_pack_b.ptr; q.k_tiles = k_tiles; q.C = p.C; q.ldc = p.ldc; q.M = p.M; q.N = p.N;
   q.bias = p.bias; q.bias2 = p.bias ? p.bias2 : nullptr; q.Z = p.Z; q.ldz = p.ldz; q.epilogue = p.epilogue; q.split_k = p.split_k;
-  q.debug_flags = p.debug_flags;
   q.c_img_k = p.C_img_k; q.c_img_mn = p.C_img_mn;
   q.c_split_stride = 0;
   int slices = 1;

@@ -9,8 +9,6 @@
 //   thin_tn     : C[M,N] += A[K,M]^T B[K,N],                      M <= 32 or N <= 32, reduction over K rows
 #include "elementwise.cuh"
 #include "gemm.cuh"
-
-#include <stdlib.h>
 #include "sm90.cuh"
 
 namespace r2d2 {
@@ -262,59 +260,13 @@ __global__ void __launch_bounds__(SN_THREADS) thin_smalln_kernel(GemmParams p, i
 // ------------------------------------------------------------------------------------------------
 // Small-N products whose K is 128 / 256 / 512 (the heads at H = 128..512: N = 1..32 outputs per row).  The kernel
 // above keeps 32 accumulators per lane and re-reads the whole [NP][K] weight tile from shared memory for every ROW
-// (64 KB of shared-memory traffic per row at K = 512: it runs at the shared-memory roof).  Here a warp owns FOUR rows: lane = 8 * row + j, lane j of a row loads the 16-byte pieces
-// j, j + 8, j + 16, ... of that row (the 8 lanes of a row read 128 contiguous bytes per instruction, 4 full lines per
-// warp instruction) and keeps them in registers; for every output column the 8 lanes of a row multiply their pieces
-// with the matching weight pieces (shared memory: 8 distinct 16-byte addresses per instruction, broadcast over the
-// rows) and a 3-step shuffle tree adds the 8 partial sums.
+// (64 KB of shared-memory traffic per row at K = 512: it runs at the shared-memory roof).  This kernel also keeps the
+// [N][K] tile in shared memory, but a warp owns FOUR rows and all 32 lanes share one k-slice layout: lane j holds the
+// 16-byte pieces j, j + 32, ... of each of the four rows in registers.  One weight load then feeds four rows, so the
+// tile crosses the shared-memory pipe (one quarter warp per clock for 128-bit loads) once per four rows instead of once
+// per row.  The 4 x 32 partial sums are reduced with a transposing butterfly: 2 + 1 exchanges halve the rows per lane,
+// 3 more add the 8 lanes of a row (6 shuffles per column).
 // ------------------------------------------------------------------------------------------------
-template <bool NN, int KI>   // KI = K / 32: float4 pieces per lane
-__global__ void __launch_bounds__(256) thin_rowdot_kernel(GemmParams p) {
-  extern __shared__ __align__(16) float Wt[];   // [N][K]
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int K = KI * 32;
-  for (int idx = tid; idx < p.N * K; idx += 256) {
-    int n, k;
-    if (NN) { k = idx / p.N; n = idx % p.N; } else { n = idx / K; k = idx % K; }
-    Wt[n * K + k] = NN ? __ldg(p.B + (long long)k * p.ldb + n) : __ldg(p.B + (long long)n * p.ldb + k);
-  }
-  __syncthreads();
-  const int j = lane & 7, r = lane >> 3;
-  const bool needs_z = p.epilogue == EPI_MUL_DTANH || p.epilogue == EPI_ADD_Z;
-  const int groups = (p.M + 3) >> 2;
-  for (int g = blockIdx.x * 8 + warp; g < groups; g += gridDim.x * 8) {
-    const int row = g * 4 + r;
-    const bool on = row < p.M;
-    float4 a[KI];
-    const float4* arow = reinterpret_cast<const float4*>(p.A + (long long)(on ? row : 0) * p.lda);
-#pragma unroll
-    for (int i = 0; i < KI; ++i) a[i] = on ? __ldg(arow + i * 8 + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int n = 0; n < p.N; ++n) {
-      const float4* wrow = reinterpret_cast<const float4*>(Wt + n * K);
-      float acc = 0.f;
-#pragma unroll
-      for (int i = 0; i < KI; ++i) {
-        const float4 w = wrow[i * 8 + j];
-        acc = fmaf(a[i].w, w.w, fmaf(a[i].z, w.z, fmaf(a[i].y, w.y, fmaf(a[i].x, w.x, acc))));
-      }
-      acc += __shfl_xor_sync(0xffffffffu, acc, 4);
-      acc += __shfl_xor_sync(0xffffffffu, acc, 2);
-      acc += __shfl_xor_sync(0xffffffffu, acc, 1);
-      if (on && (n & 7) == j) {   // the 8 lanes of a row share the stores
-        const float b = p.bias ? __ldg(p.bias + n) : 0.f;
-        const float z = needs_z ? p.Z[(long long)row * p.ldz + n] : 0.f;
-        p.C[(long long)row * p.ldc + n] = apply_epilogue(acc + b, p.epilogue, z);
-      }
-    }
-  }
-}
-
-// Second version: the kernel above is bound by the shared-memory pipe - a 128-bit shared load is served one quarter
-// warp per clock and every quarter (= one row) re-reads the same 8 weight pieces, so the [N][K] tile crosses the pipe once
-// per ROW (69 groups x 17 columns x 16 loads x 4 clocks = 75 k clocks per SM at cfg-3).  Here all 32
-// lanes share one k-slice layout (lane j holds the 16-byte pieces j, j + 32, ... of each of the warp's FOUR rows), so a
-// weight load feeds four rows: the tile crosses the pipe once per four rows.  The 4 x 32 partial sums are reduced with a
-// transposing butterfly: 2 + 1 exchanges halve the rows per lane, 3 more add the 8 lanes of a row (6 shuffles per column).
 template <bool NN, int KI>   // KI = K / 32; K / 128 pieces per lane and row
 __global__ void __launch_bounds__(256, 2) thin_rowdot4_kernel(GemmParams p) {
   extern __shared__ __align__(16) float Wt[];   // [N][K]
@@ -388,17 +340,13 @@ __global__ void __launch_bounds__(256, 2) thin_rowdot4_kernel(GemmParams p) {
 template <bool NN, int KI>
 int launch_thin_rowdot(const GemmParams& p, cudaStream_t stream) {
   const size_t smem = (size_t)p.N * KI * 32 * sizeof(float);
-  static const bool v1 = [] { const char* e = getenv("R2D2_ROWDOT_V1"); return e && e[0] == '1'; }();   // dev A/B
   static PerDeviceOnce once;
-  if (smem > 48 * 1024 && once.need()) {
-    R2D2_CUDA_TRY(cudaFuncSetAttribute(thin_rowdot_kernel<NN, KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+  if (smem > 48 * 1024 && once.need())
     R2D2_CUDA_TRY(cudaFuncSetAttribute(thin_rowdot4_kernel<NN, KI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-  }
   const int groups = ceil_div(p.M, 4);
   int grid = ceil_div(groups, 8);
   if (grid > num_sms() * 4) grid = num_sms() * 4;
-  if (v1) thin_rowdot_kernel<NN, KI><<<grid, 256, smem, stream>>>(p);
-  else thin_rowdot4_kernel<NN, KI><<<grid, 256, smem, stream>>>(p);
+  thin_rowdot4_kernel<NN, KI><<<grid, 256, smem, stream>>>(p);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;

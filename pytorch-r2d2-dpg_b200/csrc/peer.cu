@@ -1,8 +1,6 @@
 // Gradient exchange over NVLink peer memory - see peer.cuh.
 #include "peer.cuh"
 
-#include <stdlib.h>
-
 namespace r2d2 {
 
 namespace {
@@ -107,12 +105,6 @@ peer_reduce_kernel(PeerPtrs p, int world, int rank, size_t off_flags, int block,
 
 }  // namespace
 
-// R2D2_PEER_DRY=1 (timing A/B only): buffers attached, no exchange kernels - the optimiser reads zeros
-static bool peer_dry() {
-  const char* e = getenv("R2D2_PEER_DRY");
-  return e && e[0] == '1';
-}
-
 PeerLayout peer_layout(long long n_critic, long long n_actor, int world) {
   PeerLayout l;
   const long long q = 4ll * world;
@@ -130,7 +122,6 @@ int peer_signal(PeerExchange& x, int block, cudaStream_t stream) {
   R2D2_REQUIRE(block == 0 || block == 1, "peer block");
   R2D2_REQUIRE(!x.reduce_pending[block] && !x.wait_pending[block], "peer_signal: the previous exchange of this block is not complete");
   x.epoch[block] += 1;
-  if (peer_dry()) return R2D2_OK;
   peer_signal_kernel<<<1, 32, 0, stream>>>(x.ptrs, x.world, x.rank,
                                            x.lay.off_flags + sizeof(unsigned) * (kFlagIn + block * kPeerMaxWorld), x.epoch[block]);
   count_launch();

@@ -100,9 +100,17 @@ class LearnerEngine:
     def __init__(self, cfg: PathConfig, device=None, seed: int = 1):
         if not torch.cuda.is_available():
             raise nv.NativeError("LearnerEngine needs a CUDA device (H100); there is no CPU fallback")
+        import os
+        # data-parallel gradient exchange: "peer" (default: the library's own kernels over NVLink peer memory, in the
+        # learner's stream) or "defer" (NCCL all-reduces on a side stream, the actor's waited for one critic phase later;
+        # also the fallback when no peer-mapped buffer can be set up)
+        self._dp_mode = os.environ.get("R2D2_DP_MODE", "peer")
+        if self._dp_mode not in ("peer", "defer"):
+            raise nv.NativeError("R2D2_DP_MODE=%r: the gradient exchange mode is 'peer' (default) or 'defer'"
+                                 % self._dp_mode)
         self.lib = nv.lib()
         self.cfg = cfg
-        self._pending_finish = False          # a deferred phase 3 (data-parallel "defer" mode), see step() / flush()
+        self._pending_finish = False          # a deferred phase 3 (data parallel), see step() / flush()
         self._h = None
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
         torch.cuda.set_device(self.device)
@@ -155,15 +163,8 @@ class LearnerEngine:
         self.world = 1
         self._dist = None
         self._sync = None
-        import os
-        # data-parallel gradient exchange: "peer" (default: the library's own kernels over NVLink peer memory, in the
-        # learner's stream), "defer" (NCCL all-reduces on a side stream, the actor's waited for one critic phase later;
-        # also the fallback when no peer-mapped buffer can be set up), A/B timing only: "overlap" (NCCL, both waited for
-        # where needed), "serial" (NCCL on the compute stream), "none" (no exchange at all: replicas diverge)
-        self._dp_mode = os.environ.get("R2D2_DP_MODE", "peer")
         self._peer_buf = None
         self._peer_hdl = None
-        self._pending_finish = False
         self._sync_actor = None
 
     def _guard_fill(self):
@@ -239,8 +240,8 @@ class LearnerEngine:
             self._sync_actor = GradSync(dist, self.world)
             if self._dp_mode == "peer":
                 self._attach_peers(dist)
-            if self._dp_mode in ("peer", "defer"):   # the actor's weights are final only after the deferred phase 3
-                nv.check(self.lib.r2d2_learner_set_overlap_actor_inputs(self._h, 0))
+            # both modes defer phase 3: the actor's weights are final only after it ran
+            nv.check(self.lib.r2d2_learner_set_overlap_actor_inputs(self._h, 0))
             for net in ("actor", "critic", "target_actor", "target_critic"):
                 dist.broadcast(self.flat[net], src=0)
             for d in (self.exp_avg, self.exp_avg_sq):
@@ -341,7 +342,6 @@ class LearnerEngine:
         after the next critic phase; the hook then runs at the end of the step."""
         s = nv.current_stream()
         scale = 1.0 / self.world
-        mode = self._dp_mode if self._dist is not None else "single"
         if self._fill_slot != self._lib_slot:
             nv.check(self.lib.r2d2_learner_select_batch(self._h, self._fill_slot))
             self._lib_slot = self._fill_slot
@@ -349,42 +349,30 @@ class LearnerEngine:
         if self._pending_finish and self._finish_updates_targets():
             self.flush()                                                  # the target chains below read the target nets
         nv.check(self.lib.r2d2_learner_critic_phase(self._h, s))
-        if mode in ("peer", "single", "none"):
-            if mode == "peer":
-                self.flush()                                              # phase 3 of the previous iteration
-            ahead = prefetch is not None and not self._finish_updates_targets()
-            if ahead:
-                self._run_prefetch(prefetch)
-                nv.check(self.lib.r2d2_learner_target_phase(self._h, self._fill_slot, s))
-                self._targets_ahead = True
-            nv.check(self.lib.r2d2_learner_actor_forward(self._h, s))
-            nv.check(self.lib.r2d2_learner_actor_phase(self._h, scale, s))
-            if mode == "peer":   # signal / slice-sum / wait kernels are issued by the phases themselves
-                self._pending_finish = True
-            else:
-                nv.check(self.lib.r2d2_learner_finish_phase(self._h, scale, s))
-            if prefetch is not None and not ahead:
-                self._run_prefetch(prefetch)
-            return
-        if mode in ("defer", "overlap"):
+        if self._dist is not None and self._dp_mode == "defer":
             self._sync.start(self.grads["critic"])                       # side stream
             self.flush()                                                  # phase 3 of the previous iteration (actor Adam)
             nv.check(self.lib.r2d2_learner_actor_forward(self._h, s))    # reads no critic weights: overlaps the all-reduce
             self._sync.wait(self.device)
-        elif mode == "serial":                                            # A/B: both all-reduces on the compute stream
-            self._dist.all_reduce(self.grads["critic"])
-        nv.check(self.lib.r2d2_learner_actor_phase(self._h, scale, s))
-        if mode == "defer":
+            nv.check(self.lib.r2d2_learner_actor_phase(self._h, scale, s))
             self._sync_actor.start(self.grads["actor"])
             self._pending_finish = True
+            if prefetch is not None:
+                self._run_prefetch(prefetch)
+            return
+        self.flush()                                                      # phase 3 of the previous iteration, if deferred
+        ahead = prefetch is not None and not self._finish_updates_targets()
+        if ahead:
+            self._run_prefetch(prefetch)
+            nv.check(self.lib.r2d2_learner_target_phase(self._h, self._fill_slot, s))
+            self._targets_ahead = True
+        nv.check(self.lib.r2d2_learner_actor_forward(self._h, s))
+        nv.check(self.lib.r2d2_learner_actor_phase(self._h, scale, s))
+        if self._dist is not None:   # "peer": signal / slice-sum / wait kernels are issued by the phases themselves
+            self._pending_finish = True
         else:
-            if mode == "overlap":
-                self._sync_actor.start(self.grads["actor"])
-                self._sync_actor.wait(self.device)
-            elif mode == "serial":
-                self._dist.all_reduce(self.grads["actor"])
             nv.check(self.lib.r2d2_learner_finish_phase(self._h, scale, s))
-        if prefetch is not None:
+        if prefetch is not None and not ahead:
             self._run_prefetch(prefetch)
 
     def _run_prefetch(self, prefetch):

@@ -1,6 +1,7 @@
 """Where a data-parallel iteration spends its time (dev tool): CUDA events at the phase boundaries of LearnerEngine.step,
 averaged per rank.  torchrun --nproc-per-node N tools/dp_phase_time.py [variant ...]
-variants: peer | none (no exchange: lock-step cost only), suffix _seq: next batch drawn at the end of the step (no target chains ahead)"""
+variants: peer | peer_seq (next batch drawn at the end of the step: no target chains ahead).  One process without
+torchrun times the single-GPU step."""
 import os
 import sys
 
@@ -22,18 +23,21 @@ NAMES = ["critic_phase", "flush(prev actor step)", "tree update + sample", "targ
 
 
 def run(variant):
-    os.environ["R2D2_DP_MODE"] = variant.split("_")[0]
-    os.environ["R2D2_PEER_DRY"] = "1" if variant.endswith("_dry") else "0"
+    if variant not in ("peer", "peer_seq"):
+        raise SystemExit(f"unknown variant {variant!r}: peer | peer_seq")
+    os.environ["R2D2_DP_MODE"] = "peer"
     arm = bench.Arm(engine, bench.CONFIGS["cfg3"], dev, env.rank, 96, data_parallel=dist is not None)
     eng, lib = arm.eng, arm.eng.lib
-    mode = eng._dp_mode if dist is not None else "none"
-    pipelined = not variant.endswith("_seq")
+    mode = eng._dp_mode if dist is not None else "single"
+    if mode == "defer":
+        raise SystemExit("no peer-mapped gradient buffer: the exchange fell back to NCCL, which this tool does not spell out")
+    pipelined = variant == "peer"
     arm.rp.sample_into(eng, generator=arm.gen)
     scale = 1.0 / eng.world
     evs = [[torch.cuda.Event(enable_timing=True) for _ in range(len(NAMES) + 1)] for _ in range(STEPS)]
 
     def one(ev):
-        """LearnerEngine.step(prefetch=...) for modes peer / none spelled out, with events between the calls"""
+        """LearnerEngine.step(prefetch=...) for mode peer / one GPU spelled out, with events between the calls"""
         s = nv.current_stream()
         rec = (lambda i: ev[i].record()) if ev is not None else (lambda i: None)
         rec(0)
@@ -44,8 +48,7 @@ def run(variant):
         if eng._pending_finish and eng._finish_updates_targets():
             eng.flush()
         nv.check(lib.r2d2_learner_critic_phase(eng._h, s)); rec(1)
-        if mode == "peer":
-            eng.flush()
+        eng.flush()
         rec(2)
         ahead = pipelined and not eng._finish_updates_targets()
         if ahead:
@@ -104,7 +107,7 @@ def run(variant):
         dist.barrier()
 
 
-for v in (sys.argv[1:] or ["peer", "none", "peer_seq"]):
+for v in (sys.argv[1:] or ["peer", "peer_seq"]):
     run(v)
 if dist is not None:
     dist.destroy_process_group()
