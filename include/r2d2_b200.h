@@ -267,8 +267,10 @@ int r2d2_learner_buffers_get(r2d2_learner_t* l, r2d2_learner_buffers* out);
 /* The batch has two slots.  r2d2_learner_buffers_get returns slot 0 (the only one a simple caller needs); a pipelined
  * caller fills slot 1-s with batch i+1 while the phases of iteration i still read slot s, runs that batch's target
  * chains early with r2d2_learner_target_phase (they read only the target nets: learner.py:87,94-95,106) and switches
- * with r2d2_learner_select_batch before the next r2d2_learner_critic_phase.  Not allowed between an iteration whose
- * finish phase copies the weights into the target nets and that finish phase (the targets would be stale). */
+ * with r2d2_learner_select_batch before the next r2d2_learner_critic_phase.  Not allowed on an iteration that updates
+ * the target nets (step count + 1 a multiple of target_update_interval) from its actor phase until its finish phase:
+ * with target_tau < 1 the actor phase already blends the critic's target, and the finish phase updates the actor's
+ * target (or copies both at target_tau = 1) - target chains run in between would read stale targets. */
 int r2d2_learner_buffers_get_slot(r2d2_learner_t* l, int slot, r2d2_learner_buffers* out);
 int r2d2_learner_select_batch(r2d2_learner_t* l, int slot);
 /* Importance weights of a batch slot: [B] floats next to leaf_idx / uniforms (fill them with
@@ -276,6 +278,19 @@ int r2d2_learner_select_batch(r2d2_learner_t* l, int slot);
  * while importance weighting is on; off (the default) it runs the unweighted TD kernels. */
 int r2d2_learner_is_weights(r2d2_learner_t* l, int slot, float** out);
 int r2d2_learner_set_importance_weighting(r2d2_learner_t* l, int on);
+/* Polyak target update (utils.py:4-6): on the iterations of the hard copy (step % target_update_interval == 0) each
+ * target becomes fl(fl(target * (float)(1 - (double)tau)) + fl(param' * tau)), param' the net's post-Adam weight, fused
+ * into that net's Adam launch (critic: actor phase, actor: finish phase).  tau in (0, 1]; 1 (the default) is the hard
+ * copy, unchanged.  Anything else, NaN included, is R2D2_ERR_ARG. */
+int r2d2_learner_set_target_tau(r2d2_learner_t* l, float tau);
+/* Global gradient-norm clipping per net (torch.nn.utils.clip_grad_norm_ over the whole flat block): with
+ * g = grads * grad_scale, N = ||g||_2 and c = min(1, max_norm / (N + 1e-6)), Adam consumes fl(g * c).  One norm kernel
+ * before each Adam, no host synchronisation, no floating-point atomics.  0 (the default) = off, no kernel; negative,
+ * NaN or inf is R2D2_ERR_ARG. */
+int r2d2_learner_set_grad_clip(r2d2_learner_t* l, float max_norm);
+/* DEVICE address of [critic N, actor N], the pre-clip norms of the last optimiser steps (written only while clipping
+ * is on; 0 after create) */
+int r2d2_learner_grad_norms(r2d2_learner_t* l, float** out);
 int r2d2_learner_target_phase(r2d2_learner_t* l, int slot, r2d2_stream_t stream);
 /* forget a target phase that ran ahead: the caller is about to overwrite that slot's batch */
 int r2d2_learner_discard_prefetch(r2d2_learner_t* l, r2d2_stream_t stream);
@@ -286,10 +301,12 @@ int r2d2_learner_critic_phase(r2d2_learner_t* l, r2d2_stream_t stream);
  * state, 2 cell steps per row).  It does not read the critic, so a data-parallel caller issues it while the
  * all-reduce of critic_grads is in flight; phase 2 then skips it.  Without this call phase 2 runs it itself. */
 int r2d2_learner_actor_forward(r2d2_learner_t* l, r2d2_stream_t stream);
-/* phase 2: critic Adam (grads * grad_scale), actor chain unless r2d2_learner_actor_forward already ran, critic on
- * actor actions, dgrad through critic, actor BPTT -> actor_grads */
+/* phase 2: critic Adam (grads * grad_scale; norm kernel first when clipping, Polyak update of the critic's target on
+ * update iterations when target_tau < 1), actor chain unless r2d2_learner_actor_forward already ran, critic on actor
+ * actions, dgrad through critic, actor BPTT -> actor_grads */
 int r2d2_learner_actor_phase(r2d2_learner_t* l, float grad_scale, r2d2_stream_t stream);
-/* phase 3: actor Adam, step counter, hard target update every target_update_interval steps */
+/* phase 3: actor Adam (same extras as the critic's), step counter, hard target update every target_update_interval
+ * steps at target_tau = 1 */
 int r2d2_learner_finish_phase(r2d2_learner_t* l, float grad_scale, r2d2_stream_t stream);
 int r2d2_learner_step_count(r2d2_learner_t* l);
 /* The critic phase pre-issues the input projection of the actor's DPG chain on a side stream (it reads the actor's

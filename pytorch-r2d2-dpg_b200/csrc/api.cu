@@ -1,5 +1,6 @@
 // extern "C" surface of libr2d2_b200 (declared in include/r2d2_b200.h).
 #include <atomic>
+#include <cmath>
 
 #include "common.cuh"
 #include "elementwise.cuh"
@@ -265,6 +266,23 @@ int r2d2_learner_is_weights(r2d2_learner_t* lh, int slot, float** out) {
 int r2d2_learner_set_importance_weighting(r2d2_learner_t* l, int on) {
   R2D2_REQUIRE(l, "null");
   reinterpret_cast<Learner*>(l)->importance_weighting = on != 0;
+  return R2D2_OK;
+}
+int r2d2_learner_set_target_tau(r2d2_learner_t* l, float tau) {
+  R2D2_REQUIRE(l, "null");
+  R2D2_REQUIRE(tau > 0.0f && tau <= 1.0f, "target_tau lies in (0, 1]");
+  reinterpret_cast<Learner*>(l)->target_tau = tau;
+  return R2D2_OK;
+}
+int r2d2_learner_set_grad_clip(r2d2_learner_t* l, float max_norm) {
+  R2D2_REQUIRE(l, "null");
+  R2D2_REQUIRE(max_norm >= 0.0f && std::isfinite(max_norm), "max_norm is finite and >= 0 (0 = off)");
+  reinterpret_cast<Learner*>(l)->grad_clip = max_norm;
+  return R2D2_OK;
+}
+int r2d2_learner_grad_norms(r2d2_learner_t* l, float** out) {
+  R2D2_REQUIRE(l && out, "null");
+  *out = reinterpret_cast<Learner*>(l)->optim;
   return R2D2_OK;
 }
 int r2d2_learner_select_batch(r2d2_learner_t* l, int slot) {

@@ -172,19 +172,84 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x
   }
 }
 
+// kClip: the gradient is multiplied by the clip coefficient grad_norm_kernel left at *clip_coef (one load per thread).
+// kPolyak: the target net is blended with the post-step weight while it is still in a register,
+// target = fl(fl(target * tau_keep) + fl(param' * tau)) - two rounded products and one rounded add, as utils.soft_update
+// computes it with torch.  <false, false> is the plain optimiser step; its extra arguments are never read.
+template <bool kClip, bool kPolyak>
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ param, const float* __restrict__ grad,
                                                    float* __restrict__ m, float* __restrict__ v, long long n,
                                                    float grad_scale, float beta1, float beta2, float step_size,
-                                                   float inv_bc2_sqrt, float eps) {
+                                                   float inv_bc2_sqrt, float eps, const float* __restrict__ clip_coef,
+                                                   float* __restrict__ target, float tau_keep, float tau) {
+  const float c = kClip ? *clip_coef : 1.0f;
   // torch.optim.Adam single-tensor math (learner.py:50,52 defaults): lerp m, addcmul v, sqrt/bc2 + eps, addcdiv
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float g = grad[i] * grad_scale;
+    float g = grad[i] * grad_scale;
+    if (kClip) g = __fmul_rn(g, c);   // c = 1: the unclipped bits
     const float mi = m[i] + (g - m[i]) * (1.0f - beta1);
-    const float vi = v[i] * beta2 + (1.0f - beta2) * g * g;
+    // the fused variants spell out the contraction the plain kernel compiles v's update to, fma(v, b2, ((1 - b2) g) g):
+    // left to itself the compiler contracts it as fma(g, (1 - b2) g, v b2) there, and c = 1 would change the bits
+    const float vi = (kClip || kPolyak) ? __fmaf_rn(v[i], beta2, __fmul_rn(__fmul_rn(1.0f - beta2, g), g))
+                                        : v[i] * beta2 + (1.0f - beta2) * g * g;
     m[i] = mi;
     v[i] = vi;
     const float denom = sqrtf(vi) * inv_bc2_sqrt + eps;
-    param[i] = param[i] - step_size * (mi / denom);
+    const float p = param[i] - step_size * (mi / denom);
+    param[i] = p;
+    if (kPolyak) target[i] = __fadd_rn(__fmul_rn(target[i], tau_keep), __fmul_rn(p, tau));
+  }
+}
+
+// Global L2 norm of grad * grad_scale (torch.nn.utils.clip_grad_norm_ over one net's flat block) and the clip
+// coefficient, without a host round trip and without floating-point atomics: a fixed grid of kGradNormBlocks CTAs writes
+// one partial sum of squares each; the CTA that draws the last ticket adds the partials in a fixed order, writes
+// norm = N, coef = min(1, max_norm / (N + 1e-6)) and resets the ticket for the next launch.  Same inputs, same bits.
+// Squares are summed in double: a float times a float is exact there, so N is well within 1e-6 of float64.
+constexpr int NORM_THREADS = 256;
+
+__device__ __forceinline__ double block_sum_f64(double x, double* s) {   // result valid in thread 0
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = x;
+  __syncthreads();
+  double t = 0.0;
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < NORM_THREADS / 32; ++k) t += s[k];
+  }
+  return t;
+}
+
+__global__ void __launch_bounds__(NORM_THREADS) grad_norm_kernel(const float* __restrict__ grad, long long n,
+                                                                 float grad_scale, float max_norm, double* part,
+                                                                 unsigned int* ticket, float* __restrict__ norm,
+                                                                 float* __restrict__ coef) {
+  __shared__ double s_part[NORM_THREADS / 32];
+  __shared__ double s_last[NORM_THREADS / 32];
+  __shared__ bool last;
+  double acc = 0.0;
+  for (long long i = blockIdx.x * (long long)NORM_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * NORM_THREADS) {
+    const float g = grad[i] * grad_scale;   // the gradient exactly as adam_kernel forms it
+    acc += (double)g * (double)g;
+  }
+  acc = block_sum_f64(acc, s_part);
+  if (threadIdx.x == 0) {
+    part[blockIdx.x] = acc;
+    __threadfence();                        // the partial is visible device-wide before the ticket is drawn
+    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double t = 0.0;
+  for (int k = threadIdx.x; k < (int)gridDim.x; k += NORM_THREADS) t += __ldcg(part + k);
+  t = block_sum_f64(t, s_last);
+  if (threadIdx.x == 0) {
+    const float nrm = (float)sqrt(t);
+    *norm = nrm;
+    *coef = fminf(1.0f, max_norm / (nrm + 1e-6f));
+    *ticket = 0u;
   }
 }
 
@@ -362,15 +427,31 @@ int colsum(const float* x, long long ld, int M, int N, float* out, float* out2, 
 }
 
 int adam_step(float* param, const float* grad, float* m, float* v, long long n, int step, float lr, float beta1,
-              float beta2, float eps, float grad_scale, cudaStream_t stream) {
+              float beta2, float eps, float grad_scale, cudaStream_t stream, const float* clip_coef, float* target,
+              float tau) {
   R2D2_REQUIRE(param && grad && m && v && n > 0 && step >= 1, "adam args");
+  R2D2_REQUIRE(!target || (tau > 0.0f && tau <= 1.0f), "Polyak weight");
   const double bc1 = 1.0 - pow((double)beta1, (double)step);
   const double bc2 = 1.0 - pow((double)beta2, (double)step);
   const float step_size = (float)((double)lr / bc1);
   const float inv_bc2_sqrt = (float)(1.0 / sqrt(bc2));
+  const float tau_keep = (float)(1.0 - (double)tau);   // how torch rounds the Python scalar (1.0 - tau)
   int blocks = (int)((n + 255) / 256);
   if (blocks > num_sms() * 8) blocks = num_sms() * 8;
-  adam_kernel<<<blocks, 256, 0, stream>>>(param, grad, m, v, n, grad_scale, beta1, beta2, step_size, inv_bc2_sqrt, eps);
+  auto kernel = clip_coef ? (target ? adam_kernel<true, true> : adam_kernel<true, false>)
+                          : (target ? adam_kernel<false, true> : adam_kernel<false, false>);
+  kernel<<<blocks, 256, 0, stream>>>(param, grad, m, v, n, grad_scale, beta1, beta2, step_size, inv_bc2_sqrt, eps,
+                                     clip_coef, target, tau_keep, tau);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return R2D2_OK;
+}
+
+int grad_norm(const float* grad, long long n, float grad_scale, float max_norm, double* partials, unsigned int* ticket,
+              float* norm, float* coef, cudaStream_t stream) {
+  R2D2_REQUIRE(grad && partials && ticket && norm && coef && n > 0 && max_norm >= 0.0f, "grad_norm args");
+  grad_norm_kernel<<<kGradNormBlocks, NORM_THREADS, 0, stream>>>(grad, n, grad_scale, max_norm, partials, ticket, norm,
+                                                                coef);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;

@@ -31,8 +31,16 @@ int actor_priorities(const float* q, const float* q_next, const float* rew, cons
 int colsum(const float* x, long long ld, int M, int N, float* out, float* out2, cudaStream_t stream);
 int add_vec(const float* a, const float* b, float* out, int n, cudaStream_t stream);
 int mul_dtanh(const float* d_out, const float* out, float* d_pre, long long n, cudaStream_t stream);
+// Adam on a flat buffer (grad * grad_scale).  clip_coef (device scalar from grad_norm, optional) multiplies the
+// gradient first; target (optional) receives the Polyak update target = target (1 - tau) + param' tau in the same pass.
 int adam_step(float* param, const float* grad, float* m, float* v, long long n, int step, float lr, float beta1,
-              float beta2, float eps, float grad_scale, cudaStream_t stream);
+              float beta2, float eps, float grad_scale, cudaStream_t stream, const float* clip_coef = nullptr,
+              float* target = nullptr, float tau = 1.0f);
+// *norm = ||grad * grad_scale||_2 and *coef = min(1, max_norm / (*norm + 1e-6)), one launch of kGradNormBlocks CTAs.
+// partials: kGradNormBlocks doubles; ticket: one zeroed word the kernel leaves zeroed.  One launch at a time per ticket.
+constexpr int kGradNormBlocks = 512;
+int grad_norm(const float* grad, long long n, float grad_scale, float max_norm, double* partials, unsigned int* ticket,
+              float* norm, float* coef, cudaStream_t stream);
 int fill_f32(float* x, long long n, float value, cudaStream_t stream);
 int scaled_sum(const float* x, long long n, float scale, float* out, cudaStream_t stream);
 

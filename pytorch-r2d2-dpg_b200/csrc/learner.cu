@@ -8,6 +8,10 @@
 //                                                                             (learner.py:114-127)
 //   phase 3  actor Adam; hard target update every `target_update_interval` steps (learner.py:128-132)
 //
+// Optional optimiser extras (off by default): global gradient-norm clipping per net (a norm kernel before each Adam) and
+// a Polyak target update (target_tau < 1) on the same iterations as the hard copy, fused into the Adam launches: the
+// critic's target in phase 2, the actor's in phase 3.
+//
 // The actor burn-in of learner.py:92 is skipped: its state is discarded at learner.py:117 before any use.
 #include "learner.cuh"
 
@@ -50,6 +54,7 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
   const size_t ws_c2 = ChainWs::floats(l->critic_sh, L, B, 1);
   total += ws_ta + ws_tc + ws_c1 + ws_a1 + ws_c2;
   total += 2 * align64(B);   // importance weights of the two slots, carved last: the buffers above keep their offsets
+  total += align64(8) + align64(4 * (size_t)kGradNormBlocks);   // optimiser scalars + tickets, norm partials (2 x double)
   R2D2_CUDA_TRY(cudaMalloc(&l->arena, total * sizeof(float)));
   R2D2_CUDA_TRY(cudaMemset(l->arena, 0, total * sizeof(float)));
   l->arena_floats = total;
@@ -76,6 +81,9 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
     b.is_weight = take(B);
     R2D2_TRY(fill_f32(b.is_weight, B, 1.0f, 0));
   }
+  l->optim = take(8);
+  l->norm_ticket = reinterpret_cast<unsigned int*>(l->optim + 4);   // zeroed with the arena
+  l->norm_part = reinterpret_cast<double*>(take(4 * (size_t)kGradNormBlocks));
   R2D2_CUDA_TRY(cudaStreamSynchronize(0));
   learner_select_batch(l, 0);
   {   // R2D2_OVERLAP_INPUTS=0 disables the side stream (A/B)
@@ -250,6 +258,29 @@ int learner_actor_forward(Learner* l, cudaStream_t st) {
   return R2D2_OK;
 }
 
+// The iteration in flight (l->step + 1 once its finish phase ran) updates the target nets (learner.py:131).
+static bool updates_targets(const Learner* l) {
+  const int k = l->cfg.target_update_interval;
+  return k > 0 && (l->step + 1) % k == 0;
+}
+
+// Adam of one net (learner.py:114,128) on the gradient block the optimiser reads - in data-parallel runs the rank sum
+// that peer_wait just completed - preceded by the norm kernel when clipping is on.  On an update iteration with
+// target_tau < 1 the net's target is blended in the same pass; target_tau = 1 keeps the finish phase's hard copy.
+static int optimiser_step(Learner* l, int block, float* params, float* exp_avg, float* exp_avg_sq, float* target,
+                          long long n, float lr, float grad_scale, cudaStream_t st) {
+  const float* grads = l->optimiser_grads(block);
+  const float* coef = nullptr;
+  if (l->grad_clip > 0.0f) {
+    R2D2_TRY(grad_norm(grads, n, grad_scale, l->grad_clip, l->norm_part + (size_t)block * kGradNormBlocks,
+                       l->norm_ticket + block, l->optim + block, l->optim + 2 + block, st));
+    coef = l->optim + 2 + block;
+  }
+  const bool polyak = l->target_tau < 1.0f && updates_targets(l);
+  return adam_step(params, grads, exp_avg, exp_avg_sq, n, l->step + 1, lr, 0.9f, 0.999f, 1e-8f, grad_scale, st, coef,
+                   polyak ? target : nullptr, l->target_tau);
+}
+
 int learner_actor_phase(Learner* l, float grad_scale, cudaStream_t st) {
   const r2d2_learner_config& c = l->cfg;
   const int B = c.batch, Bn = c.burn_in, L = c.learning, A = c.n_actions, O = c.obs_size;
@@ -266,9 +297,10 @@ int learner_actor_phase(Learner* l, float grad_scale, cudaStream_t st) {
   const long long launches1 = launch_count();
   (void)launches1;
   if (l->peer) R2D2_TRY(peer_wait(*l->peer, kPeerCritic, st));
-  R2D2_TRY(adam_step(c.critic_params, l->optimiser_grads(kPeerCritic), c.critic_exp_avg, c.critic_exp_avg_sq,
-                     (long long)l->critic_sh.param_count(), l->step + 1, c.critic_lr, 0.9f, 0.999f, 1e-8f,
-                     grad_scale, st));                                                     // learner.py:114
+  // on an update iteration the critic's target is blended here: nothing later in the iteration changes the critic's
+  // weights, and no target chain runs before the iteration ends
+  R2D2_TRY(optimiser_step(l, kPeerCritic, c.critic_params, c.critic_exp_avg, c.critic_exp_avg_sq, c.target_critic_params,
+                          (long long)l->critic_sh.param_count(), c.critic_lr, grad_scale, st));   // learner.py:114
   {
     // the other slot already holds the next batch (its target chains ran ahead): the input projection of ITS online
     // critic chain needs the weights Adam just wrote and nothing else - side stream, under the scans of this phase
@@ -303,11 +335,10 @@ int learner_finish_phase(Learner* l, float grad_scale, cudaStream_t st) {
   const r2d2_learner_config& c = l->cfg;
   const long long launches0 = launch_count();
   if (l->peer) R2D2_TRY(peer_wait(*l->peer, kPeerActor, st));   // runs the slice reduction first if no critic phase did
-  R2D2_TRY(adam_step(c.actor_params, l->optimiser_grads(kPeerActor), c.actor_exp_avg, c.actor_exp_avg_sq,
-                     (long long)l->actor_sh.param_count(), l->step + 1, c.actor_lr, 0.9f, 0.999f, 1e-8f, grad_scale,
-                     st));                                                                 // learner.py:128
+  R2D2_TRY(optimiser_step(l, kPeerActor, c.actor_params, c.actor_exp_avg, c.actor_exp_avg_sq, c.target_actor_params,
+                          (long long)l->actor_sh.param_count(), c.actor_lr, grad_scale, st));     // learner.py:128
   l->step += 1;
-  if (c.target_update_interval > 0 && l->step % c.target_update_interval == 0) {           // learner.py:131-132
+  if (l->target_tau == 1.0f && c.target_update_interval > 0 && l->step % c.target_update_interval == 0) {  // :131-132
     R2D2_CUDA_TRY(cudaMemcpyAsync(c.target_actor_params, c.actor_params, sizeof(float) * l->actor_sh.param_count(),
                                   cudaMemcpyDeviceToDevice, st));
     R2D2_CUDA_TRY(cudaMemcpyAsync(c.target_critic_params, c.critic_params, sizeof(float) * l->critic_sh.param_count(),

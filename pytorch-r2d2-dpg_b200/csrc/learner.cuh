@@ -40,6 +40,14 @@ struct Learner {
   long long* leaf_idx = nullptr;
   float* is_weight = nullptr;
   bool importance_weighting = false;   // the TD kernels read is_weight (off: NULL, the unweighted loss)
+  // optimiser step: Polyak weight of the target update (1: the hard copy) and the per-net global gradient-norm bound
+  // (0: no clipping).  optim = [critic N, actor N, critic coef, actor coef] of the last step; norm_part / norm_ticket:
+  // grad_norm's partials and tickets, one set per net
+  float target_tau = 1.0f;
+  float grad_clip = 0.0f;
+  float* optim = nullptr;
+  unsigned int* norm_ticket = nullptr;
+  double* norm_part = nullptr;
   // intermediates / results
   float *act_tc = nullptr, *q = nullptr, *q_next = nullptr, *target = nullptr, *dq = nullptr, *mu = nullptr,
         *q_pi = nullptr, *dq_pi = nullptr, *dpre_actor = nullptr, *td_sq = nullptr, *priority = nullptr,

@@ -17,6 +17,10 @@ rank 0 alone writes model.pt.  Nothing else crosses GPUs.
 Prioritized replay (R2D2's, absent from the reference): R2D2_PRIORITY_EXPONENT (alpha, default 1) and R2D2_IS_EXPONENT
 (beta, default 0) in the environment.  The defaults are the reference's behaviour; published R2D2 uses 0.9 / 0.6.
 Under data parallelism each rank normalises the weights over its own batch.
+
+Optimiser step: R2D2_TARGET_TAU (Polyak weight tau of the target update, default 1 = the reference's hard copy),
+R2D2_TARGET_INTERVAL (iterations between target updates, default 500 = the reference's target_update_inverval; DDPG-style
+soft updates use tau 0.005 at interval 1) and R2D2_GRAD_CLIP (global gradient-norm bound per net, default 0 = off).
 """
 import os
 from time import sleep, time
@@ -72,15 +76,19 @@ class Learner:
         self.memory_path = './memory_data/'
         self.model_save_interval = 50
         self.memory_update_interval = 50
-        self.target_update_inverval = 500
+        self.target_update_inverval = int(os.environ.get("R2D2_TARGET_INTERVAL", 500))
+        if self.target_update_inverval < 1:
+            raise ValueError("R2D2_TARGET_INTERVAL must be >= 1, got {}".format(self.target_update_inverval))
         self.gamma, self.actor_lr, self.critic_lr = 0.997, 1e-4, 1e-3
         self.priority_exponent = float(os.environ.get("R2D2_PRIORITY_EXPONENT", 1.0))
         self.is_exponent = float(os.environ.get("R2D2_IS_EXPONENT", 0.0))
+        self.target_tau = float(os.environ.get("R2D2_TARGET_TAU", 1.0))
+        self.grad_clip_norm = float(os.environ.get("R2D2_GRAD_CLIP", 0.0))
         cfg = PathConfig(obs=self.obs_size, act=self.n_actions, hidden=self.hidden, batch=self.batch_size,
                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
                          gamma=self.gamma, actor_lr=self.actor_lr, critic_lr=self.critic_lr,
                          target_interval=self.target_update_inverval, priority_exponent=self.priority_exponent,
-                         is_exponent=self.is_exponent)
+                         is_exponent=self.is_exponent, target_tau=self.target_tau, grad_clip_norm=self.grad_clip_norm)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,

@@ -10,6 +10,7 @@ replay_memory.py:67-136) with the sum tree in HBM.
 """
 from __future__ import annotations
 
+import math
 from collections import OrderedDict
 from ctypes import byref, c_int, c_longlong, c_void_p
 from dataclasses import dataclass
@@ -29,7 +30,13 @@ class PathConfig:
 
     Prioritized replay (not in the reference, whose defaults these are): `priority_exponent` alpha - the replay shard
     samples a start with probability p^alpha / sum p^alpha (published R2D2: 0.9) - and `is_exponent` beta - the critic
-    loss weights sequence b by (min_b' P_b' / P_b)^beta, normalised over the batch (R2D2: 0.6).  Both lie in [0, 1]."""
+    loss weights sequence b by (min_b' P_b' / P_b)^beta, normalised over the batch (R2D2: 0.6).  Both lie in [0, 1].
+
+    Optimiser step (not in the reference either): `target_tau` tau in (0, 1] - on the iterations of the target update
+    (every `target_interval` steps) each target net becomes target (1 - tau) + tau * the net's post-Adam weights, like
+    the reference's unused utils.soft_update; 1 is the hard copy (DDPG: 0.005 at interval 1).  The library holds tau in
+    float32.  `grad_clip_norm` M >= 0 - each net's gradient is scaled by min(1, M / (N + 1e-6)), N its global L2 norm,
+    like torch.nn.utils.clip_grad_norm_; 0 is off."""
     obs: int
     act: int
     hidden: int = 128
@@ -44,12 +51,18 @@ class PathConfig:
     target_interval: int = 500
     priority_exponent: float = 1.0
     is_exponent: float = 0.0
+    target_tau: float = 1.0
+    grad_clip_norm: float = 0.0
 
     def __post_init__(self):
         for name in ("priority_exponent", "is_exponent"):
             v = getattr(self, name)
             if not 0.0 <= v <= 1.0:
                 raise ValueError("%s must lie in [0, 1], got %r" % (name, v))
+        if not 0.0 < self.target_tau <= 1.0:
+            raise ValueError("target_tau must lie in (0, 1], got %r" % (self.target_tau,))
+        if not (0.0 <= self.grad_clip_norm and math.isfinite(self.grad_clip_norm)):
+            raise ValueError("grad_clip_norm must be finite and >= 0 (0 = off), got %r" % (self.grad_clip_norm,))
 
     @property
     def rows(self) -> int:
@@ -155,6 +168,12 @@ class LearnerEngine:
         # its leaf index (DeviceReplay.sample_into); off, the library runs the unweighted TD kernels
         self.importance_weighting = cfg.is_exponent > 0
         nv.check(self.lib.r2d2_learner_set_importance_weighting(self._h, int(self.importance_weighting)))
+        # optimiser step: Polyak target update fused into the Adam launches, per-net gradient-norm clipping before them
+        nv.check(self.lib.r2d2_learner_set_target_tau(self._h, float(cfg.target_tau)))
+        nv.check(self.lib.r2d2_learner_set_grad_clip(self._h, float(cfg.grad_clip_norm)))
+        gn = c_void_p()
+        nv.check(self.lib.r2d2_learner_grad_norms(self._h, byref(gn)))
+        self.grad_norms = nv.view_f32(gn.value, (2,), dev)   # [critic, actor] pre-clip norms of the last step
         self.q_value = nv.view_f32(b.q_value, (L * B, A), dev)
         self.target_q_value = nv.view_f32(b.target_q_value, (L * B, A), dev)
         self.td_sq = nv.view_f32(b.td_sq, (L * B,), dev)
@@ -333,8 +352,10 @@ class LearnerEngine:
         allows - right after the critic phase, when the priorities exist - and the next batch's target chains run
         straight away, in the middle of this iteration: they read only the target nets, so they are the independent
         work that lets the data-parallel ranks drift by a millisecond or two without waiting for each other (and on
-        one GPU the input projections hide under their scans as before).  On iterations whose finish phase copies
-        into the target nets it is called at the end of the step instead.
+        one GPU the input projections hide under their scans as before).  On iterations that update the target nets
+        (hard copy, or the Polyak blend of `target_tau` < 1, which starts at the critic's optimiser step) it is called at
+        the end of the step instead, and a deferred data-parallel phase 3 is completed before the next critic phase.
+        At `target_interval` 1 that is every iteration: the next batch's target chains never run ahead.
 
         Data parallel, mode "peer" (default): the gradient blocks are summed by the library's own kernels over NVLink
         peer memory inside the phases (csrc/peer.cuh); the actor's optimiser step of iteration i runs after the critic

@@ -128,6 +128,9 @@ SIGNATURES = {
     "r2d2_learner_select_batch": (c_int, [c_void_p, c_int]),
     "r2d2_learner_is_weights": (c_int, [c_void_p, c_int, POINTER(c_void_p)]),
     "r2d2_learner_set_importance_weighting": (c_int, [c_void_p, c_int]),
+    "r2d2_learner_set_target_tau": (c_int, [c_void_p, c_float]),
+    "r2d2_learner_set_grad_clip": (c_int, [c_void_p, c_float]),
+    "r2d2_learner_grad_norms": (c_int, [c_void_p, POINTER(c_void_p)]),
     "r2d2_learner_target_phase": (c_int, [c_void_p, c_int, c_void_p]),
     "r2d2_learner_discard_prefetch": (c_int, [c_void_p, c_void_p]),
     "r2d2_peer_layout_for": (c_int, [c_longlong, c_longlong, c_int, POINTER(PeerLayout)]),

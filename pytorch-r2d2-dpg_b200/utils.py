@@ -8,10 +8,11 @@ import torch
 
 
 def soft_update(target_model, model, tau):
-    """Polyak update theta' <- (1-tau) theta' + tau theta (utils.py:4-6; unused by the reference's loops)."""
+    """Polyak update theta' <- (1-tau) theta' + tau theta (utils.py:4-6).  Two rounded products and one rounded add, as
+    the reference computes it and as the learner's fused update (PathConfig.target_tau) rounds it."""
     with torch.no_grad():
         for tp, p in zip(target_model.parameters(), model.parameters()):
-            tp.mul_(1.0 - tau).add_(p, alpha=tau)
+            tp.copy_(tp * (1.0 - tau) + p * tau)
 
 
 def get_obs(observation):
