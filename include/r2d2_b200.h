@@ -119,6 +119,34 @@ int r2d2_td_priority_weighted(const float* q, const float* q_next, const float* 
                               float* target, float* dq, float* td_sq, float* priority, float* critic_loss,
                               r2d2_stream_t stream);
 
+/* n-step target and priority options (published R2D2; neither is in the reference):
+ *   rescaling  R2D2_RESCALE_REFERENCE (default): y = h0(R + gamma^n (1-d) Q'), h0(x) = sign(x)(sqrt(|x|+1) - 1) - no eps x
+ *              term and no inverse on the bootstrap (utils.py:20-21, learner.py:107-108);
+ *              R2D2_RESCALE_INVERTIBLE: y = h_eps(R + gamma^n (1-d) h_eps^-1(Q')), h_eps(x) = h0(x) + eps x, in forms that
+ *              keep fp32 accurate near 0: h_eps(x) = sign(x) |x| / (sqrt(|x|+1) + 1) + eps x and
+ *              h_eps^-1(x) = sign(x) v (v+2), v = 2|x| / ((1+2eps) + sqrt((1+2eps)^2 + 4 eps |x|)).
+ *              The loss stays the MSE against y; target, dq and td_sq keep their meaning.
+ *   eps        h_eps's eps in [0, 1] (R2D2: 1e-3); ignored by the reference rescaling.
+ *   priority_metric  R2D2_PRIORITY_SQUARED (default): eta max + (1-eta) mean of td_sq (utils.py:17-18);
+ *              R2D2_PRIORITY_ABS: of m = sqrt(td_sq), the RMS over the A actions = |delta| at A = 1.  td_sq and the loss
+ *              do not change.
+ * NULL options = the defaults, the kernels and bits of the entries without _ex.  An unknown mode or metric, or (invertible)
+ * an eps that is NaN, inf, negative or > 1, is R2D2_ERR_ARG. */
+#define R2D2_RESCALE_REFERENCE 0
+#define R2D2_RESCALE_INVERTIBLE 1
+#define R2D2_PRIORITY_SQUARED 0
+#define R2D2_PRIORITY_ABS 1
+typedef struct {
+  int rescaling;
+  float eps;
+  int priority_metric;
+} r2d2_td_options;
+/* r2d2_td_priority_weighted (is_weight may be NULL) with options */
+int r2d2_td_priority_ex(const float* q, const float* q_next, const float* rew, const float* term, const float* is_weight,
+                        int L, int B, int A, int burn_in, int n_step, float gamma, float eta, float* target, float* dq,
+                        float* td_sq, float* priority, float* critic_loss, const r2d2_td_options* options,
+                        r2d2_stream_t stream);
+
 /* Actor-side rows of the path (SURVEY 8f N2), batched over finished episodes (one episode per batch column, time-major,
  * zero padded): n-step discounted reward pre-sum (actor.py:74-76; rows i < n_rows[b] - n_step, later rows copied) and
  * the initial sequence priorities (actor.py:78-107): priority k = eta*max + (1-eta)*mean over j = k+burn_in+1 ..
@@ -130,6 +158,12 @@ int r2d2_nstep_rewards(const float* raw, const int* n_rows, int T, int B, int n_
 int r2d2_actor_priorities(const float* q, const float* q_next, const float* rew, const float* term, const int* n_rows,
                           int B, int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max,
                           float* prio, r2d2_stream_t stream);
+/* r2d2_actor_priorities with options (r2d2_td_options): the invertible target, and under R2D2_PRIORITY_ABS |td| in place
+ * of td^2 - td still the MEAN difference over actions, where the learner's abs metric takes the RMS; the actor and the
+ * learner differ here as they do in the squared metric. */
+int r2d2_actor_priorities_ex(const float* q, const float* q_next, const float* rew, const float* term, const int* n_rows,
+                             int B, int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max,
+                             float* prio, const r2d2_td_options* options, r2d2_stream_t stream);
 
 /* Actor side, per env step: the four nets of N actor lanes stepped once (Actor.run, actor.py:149-154).
  * shape: O, A, H (is_critic ignored).  params: flat blocks of actor, target_actor, critic, target_critic (the critics'
@@ -288,6 +322,11 @@ int r2d2_learner_set_target_tau(r2d2_learner_t* l, float tau);
  * before each Adam, no host synchronisation, no floating-point atomics.  0 (the default) = off, no kernel; negative,
  * NaN or inf is R2D2_ERR_ARG. */
 int r2d2_learner_set_grad_clip(r2d2_learner_t* l, float max_norm);
+/* The learner's n-step target and priority options (r2d2_td_options; the defaults after create).  Either may change between
+ * any two iterations: q_next is the target critic's raw output in every mode, h_eps^-1 is applied inside the TD kernel.
+ * Same kernel count per iteration in every combination.  Bad values are R2D2_ERR_ARG and leave the setting as it was. */
+int r2d2_learner_set_value_rescaling(r2d2_learner_t* l, int mode, float eps);
+int r2d2_learner_set_priority_metric(r2d2_learner_t* l, int metric);
 /* DEVICE address of [critic N, actor N], the pre-clip norms of the last optimiser steps (written only while clipping
  * is on; 0 after create) */
 int r2d2_learner_grad_norms(r2d2_learner_t* l, float** out);

@@ -15,8 +15,9 @@ import numpy as np
 import torch
 
 from models import ActorNet, CriticNet
+from r2d2_b200 import td_options
 from replay_memory import ReplayMemory
-from utils import calc_priority, get_obs, invertical_vf
+from utils import calc_priority, get_obs, inverse_value_rescale, invertical_vf, value_rescale
 
 
 class _SyntheticEnv:
@@ -82,6 +83,7 @@ class Actor:
         self.actor_parameter_update_interval = 500
         self.model_path = './model_data/'
         self.hidden = int(os.environ.get("R2D2_HIDDEN", 128))
+        self.td_options = td_options.from_environ()     # the learner's n-step target / priority options
         self.device = torch.device(os.environ.get("R2D2_ACTOR_DEVICE", "cpu"))  # actors are CPU workers here
         self.actor = ActorNet(self.obs_size, self.action_size, 0, hidden=self.hidden).to(self.device).eval()
         self.target_actor = deepcopy(self.actor)
@@ -114,7 +116,11 @@ class Actor:
 
     @torch.no_grad()
     def calc_priorities(self):
-        """Initial sequence priorities by replaying the episode through the four nets (actor.py:78-107)."""
+        """Initial sequence priorities by replaying the episode through the four nets (actor.py:78-107).  Under R2D2's
+        options (r2d2_b200.td_options) the target is h_eps(R + gamma^n (1-d) h_eps^-1(Q')) and the priority is taken over
+        |mean difference| instead of its square."""
+        opt = self.td_options
+        invertible, eps = opt.value_rescaling == "invertible", opt.rescaling_eps
         for _, net in self._nets():
             net.reset_state()
         self.td_loss = deque(maxlen=self.learning_length)
@@ -129,11 +135,14 @@ class Actor:
             q_next = self.target_critic(nxt, self.target_actor(nxt)).cpu().numpy()
             if i >= self.burn_in_length:
                 terminal = self.sequence[i + self.n_step - 1][3][0]
+                if invertible:
+                    q_next = inverse_value_rescale(torch.tensor(q_next), eps).numpy()
                 y = self.sequence[i][2][0] + (self.gamma ** self.n_step) * (1.0 - terminal) * q_next
-                y = invertical_vf(torch.tensor(y)).numpy()
+                y = (value_rescale(torch.tensor(y), eps) if invertible else invertical_vf(torch.tensor(y))).numpy()
                 self.td_loss.append((q - y).mean())
             if i >= self.sequence_length:
-                self.priority.append(calc_priority(np.array(list(self.td_loss), dtype=np.float32) ** 2.0))
+                td = np.array(list(self.td_loss), dtype=np.float32)
+                self.priority.append(calc_priority(np.abs(td) if opt.priority_metric == "abs" else td ** 2.0))
 
     def run(self, max_episodes=None):
         episode = step = 0

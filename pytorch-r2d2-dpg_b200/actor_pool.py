@@ -7,7 +7,7 @@ lane steps its own environment on the host.  Lane by lane it does what `Actor.ru
     critic, target_critic (actor.py:149,166);
   * episodes shorter than burn_in + learning = 60 steps are dropped; kept ones get n_step pad rows, n-step rewards and
     initial priorities (r2d2_b200.actor_priority.episode_priorities, batched over every lane that finished on the same
-    step);
+    step), with the target / priority options of the environment (r2d2_b200.td_options, as the learner reads them);
   * each lane has its own ReplayMemory, saved to memory{actor_id}.pt once it holds more than 3 episodes (same file
     format and atomic rename);
   * model.pt is reloaded every 500 pool steps; lane 0 prints its episode reward.
@@ -99,6 +99,8 @@ class ActorPool:
                                     max_episode_steps=max_episode_steps)
         self.stepper = stepper
         self.device = stepper.device
+        from r2d2_b200 import td_options
+        self.td_options = td_options.from_environ()
         self.priority_fn = priority_fn or self._gpu_priorities
         self.model_dict = initial_model_dict(self.obs_size, self.action_size, self.hidden)
         self.stepper.load(self.model_dict)
@@ -117,7 +119,8 @@ class ActorPool:
         return actor_priority.episode_priorities(
             model_dict["critic"], model_dict["target_actor"], model_dict["target_critic"], episodes,
             hidden=self.hidden, burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
-            gamma=self.gamma, rewards_are_raw=True, device=self.device)
+            gamma=self.gamma, rewards_are_raw=True, device=self.device, rescaling=self.td_options.value_rescaling,
+            eps=self.td_options.rescaling_eps, priority_metric=self.td_options.priority_metric)
 
     def load_model(self):
         """Follow the learner's model.pt (actor.py:50-72); retried while the file is being replaced."""

@@ -159,6 +159,27 @@ int r2d2_td_priority_weighted(const float* q, const float* q_next, const float* 
   return td_priority(p, S(stream));
 }
 
+static int td_options_of(const r2d2_td_options* o, TdOptions* out) {
+  *out = TdOptions();
+  if (o) { out->rescaling = o->rescaling; out->eps = o->eps; out->priority_metric = o->priority_metric; }
+  return check_td_options(*out);
+}
+
+int r2d2_td_priority_ex(const float* q, const float* q_next, const float* rew, const float* term, const float* is_weight,
+                        int L, int B, int A, int burn_in, int n_step, float gamma, float eta, float* target, float* dq,
+                        float* td_sq, float* priority, float* critic_loss, const r2d2_td_options* options,
+                        r2d2_stream_t stream) {
+  TdOptions opt;
+  R2D2_TRY(td_options_of(options, &opt));
+  TdPriorityParams p;
+  p.q = q; p.q_next = q_next; p.rew = rew; p.term = term; p.target = target; p.dq = dq; p.td_sq = td_sq;
+  p.priority = priority; p.loss_sum = critic_loss; p.L = L; p.B = B; p.A = A; p.burn_in = burn_in; p.n_step = n_step;
+  p.gamma_n = (float)pow((double)gamma, (double)n_step);
+  p.eta = eta;
+  p.is_weight = is_weight;
+  return td_priority(p, S(stream), opt);
+}
+
 int r2d2_nstep_rewards(const float* raw, const int* n_rows, int T, int B, int n_step, float gamma, float* out,
                        r2d2_stream_t stream) {
   return nstep_rewards(raw, n_rows, T, B, n_step, gamma, out, S(stream));
@@ -167,6 +188,14 @@ int r2d2_actor_priorities(const float* q, const float* q_next, const float* rew,
                           int B, int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max,
                           float* prio, r2d2_stream_t stream) {
   return actor_priorities(q, q_next, rew, term, n_rows, B, A, burn_in, learning, n_step, gamma, eta, p_max, prio, S(stream));
+}
+int r2d2_actor_priorities_ex(const float* q, const float* q_next, const float* rew, const float* term, const int* n_rows,
+                             int B, int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max,
+                             float* prio, const r2d2_td_options* options, r2d2_stream_t stream) {
+  TdOptions opt;
+  R2D2_TRY(td_options_of(options, &opt));
+  return actor_priorities(q, q_next, rew, term, n_rows, B, A, burn_in, learning, n_step, gamma, eta, p_max, prio,
+                          S(stream), opt);
 }
 
 size_t r2d2_policy_workspace_floats(const r2d2_net_shape* shape, int N) {
@@ -278,6 +307,22 @@ int r2d2_learner_set_grad_clip(r2d2_learner_t* l, float max_norm) {
   R2D2_REQUIRE(l, "null");
   R2D2_REQUIRE(max_norm >= 0.0f && std::isfinite(max_norm), "max_norm is finite and >= 0 (0 = off)");
   reinterpret_cast<Learner*>(l)->grad_clip = max_norm;
+  return R2D2_OK;
+}
+int r2d2_learner_set_value_rescaling(r2d2_learner_t* l, int mode, float eps) {
+  R2D2_REQUIRE(l, "null");
+  Learner* e = reinterpret_cast<Learner*>(l);
+  TdOptions opt{mode, eps, e->priority_metric};
+  R2D2_TRY(check_td_options(opt));
+  e->rescaling = mode;
+  e->rescaling_eps = mode == kRescaleReference ? 0.0f : eps;
+  return R2D2_OK;
+}
+int r2d2_learner_set_priority_metric(r2d2_learner_t* l, int metric) {
+  R2D2_REQUIRE(l, "null");
+  Learner* e = reinterpret_cast<Learner*>(l);
+  R2D2_TRY(check_td_options(TdOptions{kRescaleReference, 0.0f, metric}));
+  e->priority_metric = metric;
   return R2D2_OK;
 }
 int r2d2_learner_grad_norms(r2d2_learner_t* l, float** out) {

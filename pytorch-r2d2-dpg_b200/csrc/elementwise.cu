@@ -17,9 +17,38 @@ __device__ __forceinline__ float value_rescale(float x) {
   return x > 0.f ? m : (x < 0.f ? -m : 0.f);
 }
 
+// ---- R2D2's invertible value rescaling (TdPriorityParams::rescaling = R2D2_RESCALE_INVERTIBLE), in forms that stay
+// accurate in fp32 near zero, where critic outputs start (l3 ~ U(+-3e-3)); the textbook closed forms cancel there.
+// h_eps(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x, with sqrt(a + 1) - 1 written as a / (sqrt(a + 1) + 1).
+__device__ __forceinline__ float value_rescale_eps(float x, float eps) {
+  const float a = fabsf(x);
+  return copysignf(a / (sqrtf(a + 1.0f) + 1.0f), x) + eps * x;
+}
+// h_eps^-1(x) = sign(x) v (v + 2), v = sqrt(s + 1) - 1 the positive root of eps v^2 + (1 + 2 eps) v - |x| = 0, taken as
+// 2 |x| / ((1 + 2 eps) + sqrt((1 + 2 eps)^2 + 4 eps |x|)): no step cancels, and eps = 0 gives v = |x|.
+__device__ __forceinline__ float inverse_value_rescale(float x, float eps) {
+  const float a = fabsf(x);
+  const float c = 1.0f + 2.0f * eps;
+  const float v = (2.0f * a) / (c + sqrtf(c * c + 4.0f * eps * a));
+  return copysignf(v * (v + 2.0f), x);
+}
+
+// the n-step target of one element: reference h0(r + cont q'), or invertible h_eps(r + cont h_eps^-1(q'))
+template <bool kInvertible>
+__device__ __forceinline__ float td_target(float r, float cont, float qn, float eps) {
+  if (kInvertible) return value_rescale_eps(r + cont * inverse_value_rescale(qn, eps), eps);
+  return value_rescale(r + cont * qn);
+}
+
+// what a time step contributes to its sequence's priority: the squared TD (reference) or its root, the RMS over actions
+template <bool kAbs>
+__device__ __forceinline__ float priority_term(float td_sq) { return kAbs ? sqrtf(td_sq) : td_sq; }
+
 // fallback (no td_sq buffer to reduce through): grid ceil(B/32) CTAs, 1024 threads = 32 warps; lane -> batch column, warp -> time rows i = w, w+32, ...
 // (the kernel moves ~1 MB: it is bound by the length of the per-thread dependent load chain, hence the wide block)
+// <false, false> is the reference's target and squared-error priority; see td_target / priority_term for the others.
 constexpr int TD_WARPS = 32;
+template <bool kInvertible, bool kAbs>
 __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPriorityParams p, float* loss_part) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int b = blockIdx.x * 32 + lane;
@@ -39,7 +68,7 @@ __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPri
       float sq = 0.f;
       for (int a = 0; a < A; ++a) {
         const float q = __ldg(p.q + base + a);
-        const float y = value_rescale(r + cont * __ldg(p.q_next + base + a));
+        const float y = td_target<kInvertible>(r, cont, __ldg(p.q_next + base + a), p.eps);
         const float diff = q - y;
         if (p.target) p.target[base + a] = y;
         if (p.dq) p.dq[base + a] = gs * diff;
@@ -49,7 +78,11 @@ __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPri
       const float td = sq * inv_a;
       if (p.td_sq) p.td_sq[(size_t)i * B + b] = td;
       // learner.py:137 `average_td_loss[b:-1:B]` drops flat index L*B-1, i.e. (i=L-1, b=B-1)
-      if (!(i == L - 1 && b == B - 1)) { run_max = fmaxf(run_max, td); run_sum += td; }
+      if (!(i == L - 1 && b == B - 1)) {
+        const float m = priority_term<kAbs>(td);
+        run_max = fmaxf(run_max, m);
+        run_sum += m;
+      }
     }
   }
   __shared__ float s_max[TD_WARPS][32], s_sum[TD_WARPS][32], s_sq[TD_WARPS];
@@ -82,6 +115,7 @@ __global__ void __launch_bounds__(TD_WARPS * 32) td_priority_column_kernel(TdPri
 // target and the loss gradient back into the same shared slots and the warp stores them with unit-stride writes.
 // Pass 2 reduces td_sq[L,B] per batch element (max / mean with the [b:-1:B] quirk) and sums the loss: lanes along b.
 constexpr int TD1_WARPS = 8;
+template <bool kInvertible>
 __global__ void __launch_bounds__(TD1_WARPS * 32) td_elem_kernel(TdPriorityParams p) {
   extern __shared__ float td_smem[];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -107,7 +141,7 @@ __global__ void __launch_bounds__(TD1_WARPS * 32) td_elem_kernel(TdPriorityParam
     const float gs = grad_scale * (p.is_weight ? __ldg(p.is_weight + b) : 1.0f);   // w = 1: exactly grad_scale
     float sq = 0.f;
     for (int a = 0; a < A; ++a) {
-      const float y = value_rescale(r + cont * sn_[lane * A + a]);
+      const float y = td_target<kInvertible>(r, cont, sn_[lane * A + a], p.eps);
       const float diff = sq_[lane * A + a] - y;
       sn_[lane * A + a] = y;
       sq_[lane * A + a] = gs * diff;
@@ -121,6 +155,7 @@ __global__ void __launch_bounds__(TD1_WARPS * 32) td_elem_kernel(TdPriorityParam
 }
 
 constexpr int TD2_WARPS = 8;
+template <bool kAbs>
 __global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityParams p, float* loss_part) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int b = blockIdx.x * 32 + lane;
@@ -132,7 +167,11 @@ __global__ void __launch_bounds__(TD2_WARPS * 32) td_reduce_kernel(TdPriorityPar
       const float td = p.td_sq[(size_t)i * B + b];
       tot += wb * td;
       // learner.py:137 `average_td_loss[b:-1:B]` drops flat index L*B-1, i.e. (i=L-1, b=B-1)
-      if (!(i == L - 1 && b == B - 1)) { run_max = fmaxf(run_max, td); run_sum += td; }
+      if (!(i == L - 1 && b == B - 1)) {
+        const float m = priority_term<kAbs>(td);
+        run_max = fmaxf(run_max, m);
+        run_sum += m;
+      }
     }
   }
   __shared__ float s_max[TD2_WARPS][32], s_sum[TD2_WARPS][32], s_tot[TD2_WARPS][32];
@@ -317,33 +356,46 @@ __global__ void __launch_bounds__(256) nstep_reward_kernel(const float* __restri
 // priority k of episode b: 0.9 max + 0.1 mean over j = k+Bn+1 .. k+Bn+L of td_j^2,
 // td_j = mean_A(q[j,b,:] - h(R[j,b] + gamma^n (1 - term[j+n-1,b]) q_next[j+n,b,:]))  -  the reference's deque of
 // `learning` entries is one step ahead of the window the learner trains on (actor.py:102-107), reproduced here.
+// kInvertible: the target of td_target<true>.  kAbs: |td_j| in place of td_j^2 - still the MEAN difference over actions,
+// where the learner's abs metric takes the RMS; the two sides differ here as they do in the squared metric.
+template <bool kInvertible, bool kAbs>
 __global__ void __launch_bounds__(128) actor_priority_kernel(const float* __restrict__ q, const float* __restrict__ q_next,
                                                              const float* __restrict__ rew, const float* __restrict__ term,
                                                              const int* __restrict__ n_rows, int B, int A, int burn_in,
                                                              int learning, int n_step, float gamma_n, float eta,
-                                                             int p_max, float* __restrict__ prio) {
+                                                             int p_max, float* __restrict__ prio, float eps) {
   const int b = blockIdx.y;
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= p_max) return;
   const int E = n_rows[b] - n_step;
   float out = 0.f;
+  int k_out = k;
   if (k < E - (burn_in + learning)) {
     float mx = -INFINITY, sum = 0.f;
-    for (int j = k + burn_in + 1; j <= k + burn_in + learning; ++j) {
+    int j = k + burn_in + 1;
+    for (; j <= k + burn_in + learning; ++j) {
       const float r = rew[(size_t)j * B + b];
       const float cont = gamma_n * (1.0f - term[(size_t)(j + n_step - 1) * B + b]);
       const float* qj = q + ((size_t)j * B + b) * A;
       const float* qn = q_next + ((size_t)(j + n_step) * B + b) * A;
       float acc = 0.f;
-      for (int a = 0; a < A; ++a) acc += qj[a] - value_rescale(r + cont * qn[a]);
+      if (kInvertible) {   // one element at a time: unrolled, its two divisions' slow paths would keep more live
+#pragma unroll 1
+        for (int a = 0; a < A; ++a) acc += qj[a] - td_target<true>(r, cont, qn[a], eps);
+      } else {
+        for (int a = 0; a < A; ++a) acc += qj[a] - td_target<false>(r, cont, qn[a], eps);
+      }
       const float td = acc / (float)A;
-      const float sq = td * td;
+      const float sq = kAbs ? fabsf(td) : td * td;
       mx = fmaxf(mx, sq);
       sum += sq;
     }
     out = eta * mx + (1.0f - eta) * (sum / (float)learning);
+    // the new variants take k back from the loop counter: k itself, kept across the division slow-path calls of the
+    // loop, costs the default variant 8 bytes of stack (its code stays as it was)
+    if (kInvertible || kAbs) k_out = j - (burn_in + learning + 1);
   }
-  prio[(size_t)b * p_max + k] = out;
+  prio[(size_t)b * p_max + k_out] = out;
 }
 
 }  // namespace
@@ -358,11 +410,15 @@ int nstep_rewards(const float* raw, const int* n_rows, int T, int B, int n_step,
 
 int actor_priorities(const float* q, const float* q_next, const float* rew, const float* term, const int* n_rows, int B,
                      int A, int burn_in, int learning, int n_step, float gamma, float eta, int p_max, float* prio,
-                     cudaStream_t stream) {
+                     cudaStream_t stream, const TdOptions& opt) {
   R2D2_REQUIRE(q && q_next && rew && term && n_rows && prio && B > 0 && A > 0 && p_max > 0, "actor_priorities args");
+  R2D2_TRY(check_td_options(opt));
   const float gamma_n = (float)std::pow((double)gamma, (double)n_step);
-  actor_priority_kernel<<<dim3(ceil_div(p_max, 128), B), 128, 0, stream>>>(q, q_next, rew, term, n_rows, B, A, burn_in, learning,
-                                                                           n_step, gamma_n, eta, p_max, prio);
+  const bool inv = opt.rescaling == kRescaleInvertible, abs_ = opt.priority_metric == kPriorityAbs;
+  auto kernel = inv ? (abs_ ? actor_priority_kernel<true, true> : actor_priority_kernel<true, false>)
+                    : (abs_ ? actor_priority_kernel<false, true> : actor_priority_kernel<false, false>);
+  kernel<<<dim3(ceil_div(p_max, 128), B), 128, 0, stream>>>(q, q_next, rew, term, n_rows, B, A, burn_in, learning, n_step,
+                                                           gamma_n, eta, p_max, prio, opt.eps);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;
@@ -384,9 +440,23 @@ int mul_dtanh(const float* d_out, const float* out, float* d_pre, long long n, c
   return R2D2_OK;
 }
 
-int td_priority(const TdPriorityParams& p, cudaStream_t stream) {
-  R2D2_REQUIRE(p.q && p.q_next && p.rew && p.term, "null input");
-  R2D2_REQUIRE(p.L > 0 && p.B > 0 && p.A > 0, "shape");
+int check_td_options(const TdOptions& opt) {
+  R2D2_REQUIRE(opt.rescaling == kRescaleReference || opt.rescaling == kRescaleInvertible,
+               "value rescaling is R2D2_RESCALE_REFERENCE (0) or R2D2_RESCALE_INVERTIBLE (1)");
+  R2D2_REQUIRE(opt.priority_metric == kPrioritySquared || opt.priority_metric == kPriorityAbs,
+               "priority metric is R2D2_PRIORITY_SQUARED (0) or R2D2_PRIORITY_ABS (1)");
+  R2D2_REQUIRE(opt.rescaling == kRescaleReference || (opt.eps >= 0.0f && opt.eps <= 1.0f),
+               "rescaling eps lies in [0, 1]");   // NaN fails both comparisons
+  return R2D2_OK;
+}
+
+int td_priority(const TdPriorityParams& params, cudaStream_t stream, const TdOptions& opt) {
+  R2D2_REQUIRE(params.q && params.q_next && params.rew && params.term, "null input");
+  R2D2_REQUIRE(params.L > 0 && params.B > 0 && params.A > 0, "shape");
+  R2D2_TRY(check_td_options(opt));
+  const bool inv = opt.rescaling == kRescaleInvertible, abs_ = opt.priority_metric == kPriorityAbs;
+  TdPriorityParams p = params;
+  p.eps = opt.eps;
   const int col_blocks = ceil_div(p.B, 32);
   float* loss_part = nullptr;     // one partial loss per column block, summed in block order
   if (p.loss_sum) {
@@ -395,14 +465,18 @@ int td_priority(const TdPriorityParams& p, cudaStream_t stream) {
   }
   const size_t smem = (size_t)TD1_WARPS * 2 * 32 * p.A * sizeof(float);
   if (p.td_sq && smem <= 48 * 1024) {   // the path's configuration: two line-coalesced passes over L x B x A and L x B
-    td_elem_kernel<<<dim3(col_blocks, ceil_div(p.L, TD1_WARPS)), TD1_WARPS * 32, smem, stream>>>(p);
+    auto elem = inv ? td_elem_kernel<true> : td_elem_kernel<false>;
+    elem<<<dim3(col_blocks, ceil_div(p.L, TD1_WARPS)), TD1_WARPS * 32, smem, stream>>>(p);
     count_launch();
     if (p.priority || p.loss_sum) {
-      td_reduce_kernel<<<col_blocks, TD2_WARPS * 32, 0, stream>>>(p, loss_part);
+      auto reduce = abs_ ? td_reduce_kernel<true> : td_reduce_kernel<false>;
+      reduce<<<col_blocks, TD2_WARPS * 32, 0, stream>>>(p, loss_part);
       count_launch();
     }
   } else {
-    td_priority_column_kernel<<<col_blocks, TD_WARPS * 32, 0, stream>>>(p, loss_part);
+    auto column = inv ? (abs_ ? td_priority_column_kernel<true, true> : td_priority_column_kernel<true, false>)
+                      : (abs_ ? td_priority_column_kernel<false, true> : td_priority_column_kernel<false, false>);
+    column<<<col_blocks, TD_WARPS * 32, 0, stream>>>(p, loss_part);
     count_launch();
   }
   R2D2_CUDA_TRY(cudaGetLastError());

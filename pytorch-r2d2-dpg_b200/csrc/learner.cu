@@ -223,7 +223,7 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
   tp.gamma_n = (float)std::pow((double)c.gamma, (double)n);
   tp.eta = c.eta;
   tp.is_weight = l->importance_weighting ? l->is_weight : nullptr;
-  R2D2_TRY(td_priority(tp, st));
+  R2D2_TRY(td_priority(tp, st, TdOptions{l->rescaling, l->rescaling_eps, l->priority_metric}));
 
   R2D2_CUDA_TRY(cudaMemsetAsync(c.critic_grads, 0, sizeof(float) * l->critic_sh.param_count(), st));
   R2D2_TRY(net_backward(l->critic_sh, Pc, &Gc, l->ws_c1, l->obs, l->act, l->dq, Bn, Tc, B, 1, nullptr, nullptr, st));

@@ -1,5 +1,6 @@
 #pragma once
 #include "common.cuh"
+#include "elementwise.cuh"
 #include "net.cuh"
 #include "peer.cuh"
 
@@ -48,6 +49,12 @@ struct Learner {
   float* optim = nullptr;
   unsigned int* norm_ticket = nullptr;
   double* norm_part = nullptr;
+  // n-step target and priority options of the TD kernels (elementwise.cuh TdOptions): the reference's by default.  q_next
+  // is the target critic's raw output in every mode (h_eps^-1 runs inside the TD kernel), so they may change between
+  // any two iterations
+  int rescaling = kRescaleReference;
+  float rescaling_eps = 0.0f;
+  int priority_metric = kPrioritySquared;
   // intermediates / results
   float *act_tc = nullptr, *q = nullptr, *q_next = nullptr, *target = nullptr, *dq = nullptr, *mu = nullptr,
         *q_pi = nullptr, *dq_pi = nullptr, *dpre_actor = nullptr, *td_sq = nullptr, *priority = nullptr,

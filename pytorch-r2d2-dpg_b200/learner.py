@@ -21,6 +21,13 @@ Under data parallelism each rank normalises the weights over its own batch.
 Optimiser step: R2D2_TARGET_TAU (Polyak weight tau of the target update, default 1 = the reference's hard copy),
 R2D2_TARGET_INTERVAL (iterations between target updates, default 500 = the reference's target_update_inverval; DDPG-style
 soft updates use tau 0.005 at interval 1) and R2D2_GRAD_CLIP (global gradient-norm bound per net, default 0 = off).
+
+n-step target and priorities (r2d2_b200.td_options, read the same way by the drop-in Actor and ActorPool):
+R2D2_VALUE_RESCALING=reference|invertible (default reference: the reference's y = h(R + gamma^n (1-d) Q') with
+h(x) = sign(x)(sqrt(|x|+1) - 1), no eps x and no inverse on the bootstrap; invertible: published R2D2's
+y = h_eps(R + gamma^n (1-d) h_eps^-1(Q')), h_eps = h + eps x), R2D2_RESCALING_EPS (eps, default 1e-3) and
+R2D2_PRIORITY_METRIC=squared|abs (default squared: the reference's eta max + (1-eta) mean of squared TD errors; abs: of
+absolute ones, R2D2's).  Any other value raises.  The checkpoint records them and a resume under other settings is refused.
 """
 import os
 from time import sleep, time
@@ -84,11 +91,15 @@ class Learner:
         self.is_exponent = float(os.environ.get("R2D2_IS_EXPONENT", 0.0))
         self.target_tau = float(os.environ.get("R2D2_TARGET_TAU", 1.0))
         self.grad_clip_norm = float(os.environ.get("R2D2_GRAD_CLIP", 0.0))
+        from r2d2_b200 import td_options
+        self.td_options = td_options.from_environ()
         cfg = PathConfig(obs=self.obs_size, act=self.n_actions, hidden=self.hidden, batch=self.batch_size,
                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
                          gamma=self.gamma, actor_lr=self.actor_lr, critic_lr=self.critic_lr,
                          target_interval=self.target_update_inverval, priority_exponent=self.priority_exponent,
-                         is_exponent=self.is_exponent, target_tau=self.target_tau, grad_clip_norm=self.grad_clip_norm)
+                         is_exponent=self.is_exponent, target_tau=self.target_tau, grad_clip_norm=self.grad_clip_norm,
+                         value_rescaling=self.td_options.value_rescaling, rescaling_eps=self.td_options.rescaling_eps,
+                         priority_metric=self.td_options.priority_metric)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,

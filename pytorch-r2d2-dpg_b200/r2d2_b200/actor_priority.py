@@ -8,6 +8,8 @@ priorities that every reference actor computes per finished episode at batch 1 o
 
 The reference's quirks are kept (see include/r2d2_b200.h): every net sees rows 0, 1, 2, ... once; the deque of
 `learning` TD values is one step ahead of the learner's window; the TD is the mean difference over actions, squared.
+With R2D2's options (r2d2_b200.td_options) the target is h_eps(R + gamma^n (1-d) h_eps^-1(Q')) and/or the priority is
+taken over |td| (still the mean difference over actions) instead of td^2.
 """
 from __future__ import annotations
 
@@ -15,6 +17,7 @@ import numpy as np
 import torch
 
 from . import native as nv
+from . import td_options
 
 PARAM_KEYS = ("l1.weight", "l1.bias", "l2.weight_ih", "l2.weight_hh", "l2.bias_ih", "l2.bias_hh", "l3.weight", "l3.bias")
 
@@ -34,10 +37,13 @@ def nstep_rewards(raw_tb: torch.Tensor, n_rows: torch.Tensor, n_step: int, gamma
 
 
 def episode_priorities(critic, target_actor, target_critic, episodes, *, hidden, burn_in=20, learning=40, n_step=5,
-                       gamma=0.997, eta=0.9, rewards_are_raw=False, device=None):
+                       gamma=0.997, eta=0.9, rewards_are_raw=False, device=None, rescaling="reference",
+                       eps=td_options.DEFAULT_EPS, priority_metric="squared"):
     """episodes: list of (obs [N,O], act [N,A], rew [N], term [N]) host arrays, N = real rows + n_step pad rows
-    (actor.py:173).  Weights: state_dicts (or dicts of arrays) with the reference's keys.  Returns
+    (actor.py:173).  Weights: state_dicts (or dicts of arrays) with the reference's keys.  rescaling / eps /
+    priority_metric: r2d2_b200.td_options (the defaults are the reference's).  Returns
     (list of float32 arrays [N - n_step - burn_in - learning], list of n-step reward arrays [N])."""
+    opts = td_options.TdOptions(rescaling, eps, priority_metric)
     if not torch.cuda.is_available():
         raise nv.NativeError("episode_priorities needs a CUDA device; there is no CPU fallback")
     lib = nv.lib()
@@ -77,8 +83,14 @@ def episode_priorities(critic, target_actor, target_critic, episodes, *, hidden,
                                        nv.dptr(q_t), nv.dptr(ws), st))
     p_max = max(1, Te - (burn_in + learning))
     prio = torch.empty((B, p_max), device=dev)
-    nv.check(lib.r2d2_actor_priorities(nv.dptr(q), nv.dptr(q_t), nv.dptr(rew), nv.dptr(term), nv.dptr(n_rows, torch.int32),
-                                       B, A, burn_in, learning, n_step, gamma, eta, p_max, nv.dptr(prio), st))
+    if opts.is_default:
+        nv.check(lib.r2d2_actor_priorities(nv.dptr(q), nv.dptr(q_t), nv.dptr(rew), nv.dptr(term),
+                                           nv.dptr(n_rows, torch.int32), B, A, burn_in, learning, n_step, gamma, eta, p_max,
+                                           nv.dptr(prio), st))
+    else:
+        nv.check(lib.r2d2_actor_priorities_ex(nv.dptr(q), nv.dptr(q_t), nv.dptr(rew), nv.dptr(term),
+                                              nv.dptr(n_rows, torch.int32), B, A, burn_in, learning, n_step, gamma, eta,
+                                              p_max, nv.dptr(prio), nv.byref(nv.TdOptions(*opts.native())), st))
     prio_h, rew_h = prio.cpu().numpy(), rew.cpu().numpy()
     out = [prio_h[b, :max(0, lens[b] - n_step - burn_in - learning)].copy() for b in range(B)]
     return out, [rew_h[:lens[b], b].copy() for b in range(B)]

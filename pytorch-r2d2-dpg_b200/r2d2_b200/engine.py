@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from . import native as nv
+from . import td_options
 
 PARAM_KEYS = ("l1.weight", "l1.bias", "l2.weight_ih", "l2.weight_hh", "l2.bias_ih", "l2.bias_hh",
               "l3.weight", "l3.bias")
@@ -36,7 +37,11 @@ class PathConfig:
     (every `target_interval` steps) each target net becomes target (1 - tau) + tau * the net's post-Adam weights, like
     the reference's unused utils.soft_update; 1 is the hard copy (DDPG: 0.005 at interval 1).  The library holds tau in
     float32.  `grad_clip_norm` M >= 0 - each net's gradient is scaled by min(1, M / (N + 1e-6)), N its global L2 norm,
-    like torch.nn.utils.clip_grad_norm_; 0 is off."""
+    like torch.nn.utils.clip_grad_norm_; 0 is off.
+
+    n-step target and priorities (r2d2_b200.td_options): `value_rescaling` "reference" (the reference's h0 without an
+    inverse on the bootstrap) or "invertible" (R2D2's h_eps(R + gamma^n (1-d) h_eps^-1(Q')) with eps = `rescaling_eps`,
+    in [0, 1]); `priority_metric` "squared" (the reference's) or "abs" (R2D2's absolute TD errors)."""
     obs: int
     act: int
     hidden: int = 128
@@ -53,8 +58,12 @@ class PathConfig:
     is_exponent: float = 0.0
     target_tau: float = 1.0
     grad_clip_norm: float = 0.0
+    value_rescaling: str = "reference"
+    rescaling_eps: float = td_options.DEFAULT_EPS
+    priority_metric: str = "squared"
 
     def __post_init__(self):
+        td_options.validate(self.value_rescaling, self.rescaling_eps, self.priority_metric)
         for name in ("priority_exponent", "is_exponent"):
             v = getattr(self, name)
             if not 0.0 <= v <= 1.0:
@@ -171,6 +180,9 @@ class LearnerEngine:
         # optimiser step: Polyak target update fused into the Adam launches, per-net gradient-norm clipping before them
         nv.check(self.lib.r2d2_learner_set_target_tau(self._h, float(cfg.target_tau)))
         nv.check(self.lib.r2d2_learner_set_grad_clip(self._h, float(cfg.grad_clip_norm)))
+        # n-step target and priorities: the library starts at the reference's; set only when asked for
+        if not self.td_options.is_default:
+            self.set_td_options(cfg.value_rescaling, cfg.rescaling_eps, cfg.priority_metric)
         gn = c_void_p()
         nv.check(self.lib.r2d2_learner_grad_norms(self._h, byref(gn)))
         self.grad_norms = nv.view_f32(gn.value, (2,), dev)   # [critic, actor] pre-clip norms of the last step
@@ -185,6 +197,20 @@ class LearnerEngine:
         self._peer_buf = None
         self._peer_hdl = None
         self._sync_actor = None
+
+    @property
+    def td_options(self) -> td_options.TdOptions:
+        c = self.cfg
+        return td_options.TdOptions(c.value_rescaling, c.rescaling_eps, c.priority_metric)
+
+    def set_td_options(self, value_rescaling: str, rescaling_eps: float, priority_metric: str):
+        """Change the n-step target / priority options; allowed between any two steps (the TD kernel applies
+        h_eps^-1 to the target critic's raw output, so nothing computed earlier depends on them)."""
+        rescaling, eps, metric = td_options.TdOptions(value_rescaling, rescaling_eps, priority_metric).native()
+        nv.check(self.lib.r2d2_learner_set_value_rescaling(self._h, rescaling, eps))
+        nv.check(self.lib.r2d2_learner_set_priority_metric(self._h, metric))
+        self.cfg.value_rescaling, self.cfg.rescaling_eps, self.cfg.priority_metric = value_rescaling, rescaling_eps, \
+            priority_metric
 
     def _guard_fill(self):
         if self._targets_ahead:
@@ -422,16 +448,32 @@ class LearnerEngine:
 
     # ---- full training state (SURVEY 8f N3: the reference checkpoints weights only and cannot resume) ---------------
     def training_state(self) -> dict:
-        """Everything a restart needs: the four nets (reference keys), both Adam moment sets, the step counter."""
+        """Everything a restart needs: the four nets (reference keys), both Adam moment sets, the step counter, and the
+        n-step target / priority options the critic was trained under."""
         torch.cuda.synchronize(self.device)
         out = {net: self.state_dict(net) for net in ("actor", "target_actor", "critic", "target_critic")}
         for net in ("actor", "critic"):
             out[net + "_optimizer"] = {"exp_avg": OrderedDict((k, v.detach().clone()) for k, v in self.views(net, "exp_avg").items()),
                                        "exp_avg_sq": OrderedDict((k, v.detach().clone()) for k, v in self.views(net, "exp_avg_sq").items())}
         out["step"] = self.step_count
+        o = self.td_options
+        out.update(value_rescaling=o.value_rescaling, rescaling_eps=float(o.rescaling_eps), priority_metric=o.priority_metric)
         return out
 
     def load_training_state(self, st: dict):
+        """Refuses a state saved under other target / priority options: a critic trained in one value space means nothing
+        in the other.  A state without them was saved by a build that had only the reference's (reference, squared)."""
+        def key(o):
+            return (o.value_rescaling, float(np.float32(o.rescaling_eps)) if o.value_rescaling == "invertible" else None,
+                    o.priority_metric)
+        saved = td_options.TdOptions(st.get("value_rescaling", "reference"),
+                                     st.get("rescaling_eps", td_options.DEFAULT_EPS), st.get("priority_metric", "squared"))
+        mine = self.td_options
+        if key(saved) != key(mine):
+            raise ValueError("training state was saved with value_rescaling=%r rescaling_eps=%r priority_metric=%r; this "
+                             "engine runs value_rescaling=%r rescaling_eps=%r priority_metric=%r"
+                             % (saved.value_rescaling, saved.rescaling_eps, saved.priority_metric, mine.value_rescaling,
+                                mine.rescaling_eps, mine.priority_metric))
         self.load_state_dicts(st["actor"], st["critic"], st.get("target_actor"), st.get("target_critic"))
         for net in ("actor", "critic"):
             opt = st.get(net + "_optimizer")

@@ -51,6 +51,10 @@ class LearnerConfig(Structure):
                 ("critic_exp_avg_sq", c_void_p)]
 
 
+class TdOptions(Structure):
+    _fields_ = [("rescaling", c_int), ("eps", c_float), ("priority_metric", c_int)]
+
+
 class PeerLayout(Structure):
     _fields_ = [(k, c_size_t) for k in ("bytes", "off_critic_grads", "off_actor_grads", "off_critic_sums",
                                         "off_actor_sums")]
@@ -90,9 +94,14 @@ SIGNATURES = {
     "r2d2_td_priority_weighted": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                           c_int, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p]),
+    "r2d2_td_priority_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                    c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    POINTER(TdOptions), c_void_p]),
     "r2d2_nstep_rewards": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
     "r2d2_actor_priorities": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                       c_float, c_float, c_int, c_void_p, c_void_p]),
+    "r2d2_actor_priorities_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                         c_int, c_float, c_float, c_int, c_void_p, POINTER(TdOptions), c_void_p]),
     "r2d2_policy_workspace_floats": (c_size_t, [POINTER(NetShape), c_int]),
     "r2d2_policy_step": (c_int, [POINTER(NetShape), POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                  c_void_p, c_void_p]),
@@ -130,6 +139,8 @@ SIGNATURES = {
     "r2d2_learner_set_importance_weighting": (c_int, [c_void_p, c_int]),
     "r2d2_learner_set_target_tau": (c_int, [c_void_p, c_float]),
     "r2d2_learner_set_grad_clip": (c_int, [c_void_p, c_float]),
+    "r2d2_learner_set_value_rescaling": (c_int, [c_void_p, c_int, c_float]),
+    "r2d2_learner_set_priority_metric": (c_int, [c_void_p, c_int]),
     "r2d2_learner_grad_norms": (c_int, [c_void_p, POINTER(c_void_p)]),
     "r2d2_learner_target_phase": (c_int, [c_void_p, c_int, c_void_p]),
     "r2d2_learner_discard_prefetch": (c_int, [c_void_p, c_void_p]),
@@ -202,4 +213,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "LearnerConfig", "LearnerBuffers", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "LearnerConfig", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]

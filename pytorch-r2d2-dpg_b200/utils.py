@@ -27,6 +27,22 @@ def calc_priority(td_loss, eta=0.9):
     return eta * max(vals) + (1.0 - eta) * (sum(vals) / len(vals))
 
 
+def value_rescale(x, eps=1e-3):
+    """R2D2's h_eps(x) = sign(x) (sqrt(|x| + 1) - 1) + eps x, as sign(x) |x| / (sqrt(|x| + 1) + 1) + eps x: the same
+    function without the cancellation of sqrt(|x| + 1) - 1 near 0 (the form the learner's TD kernels use)."""
+    a = torch.abs(x)
+    return torch.sign(x) * (a / (torch.sqrt(a + 1) + 1)) + eps * x
+
+
+def inverse_value_rescale(x, eps=1e-3):
+    """h_eps^-1(x) = sign(x) v (v + 2), v = 2|x| / ((1 + 2 eps) + sqrt((1 + 2 eps)^2 + 4 eps |x|)), the positive root of
+    eps v^2 + (1 + 2 eps) v - |x| = 0; no step cancels, and eps = 0 gives (|x| + 1)^2 - 1."""
+    a = torch.abs(x)
+    c = 1.0 + 2.0 * eps
+    v = 2 * a / (c + torch.sqrt(c * c + 4 * eps * a))
+    return torch.sign(x) * (v * (v + 2))
+
+
 def invertical_vf(x):
     """Value rescaling h(x) = sign(x) (sqrt(|x| + 1) - 1) without the eps*x term (utils.py:20-21)."""
     return torch.sign(x) * (torch.sqrt(torch.abs(x) + 1) - 1)
