@@ -292,11 +292,52 @@ typedef struct {
   float* target_q_value; /* [L,B,A] */
   float* td_sq;          /* [L,B]   */
   float* priority;       /* [B]     */
-  float* losses;         /* [2] critic_loss, actor_loss */
+  float* losses;         /* [2] critic_loss, actor_loss; [3] with the twin critic: critic 2's loss in [2] */
 } r2d2_learner_buffers;
 
 int r2d2_learner_create(r2d2_learner_t** out, const r2d2_learner_config* cfg);
 int r2d2_learner_destroy(r2d2_learner_t* l);
+
+/* TD3's target (Fujimoto et al. 2018; delayed policy updates are not part of it here), off by default.
+ *
+ * twin_critic (create-time: it sizes the buffers and the arena).  With it on, EVERY critic_* pointer of the config -
+ * critic_params, target_critic_params, critic_grads, critic_exp_avg, critic_exp_avg_sq - is a block of 2 P' floats
+ * [critic 1 | pad | critic 2 | pad], P the critic's parameter count and P' = P rounded up to a multiple of 64 floats
+ * (critic 2 starts at float P', 256-byte aligned like critic 1: the GEMM kernels read weights with vector loads).  The
+ * padding is zero and stays zero (zero gradients, zero moments).  Then:
+ *   - y is today's target (rescaling, options and weights included) with q' = min(Q'_1(s, a'), Q'_2(s, a')) elementwise;
+ *     both rescalings are monotone, so the minimum of the raw outputs is the minimum after h_eps^-1;
+ *   - each critic's loss is today's MSE against y, each gets its own BPTT into its half of critic_grads;
+ *   - critic 1 is the existing critic: it alone starts from the stored recurrent state (states[2] / states[3]), it alone
+ *     feeds the DPG actor loss, the priorities, td_sq and target_q_value.  Critic 2 and its target start from the zero
+ *     state and rely on the burn-in rows: the replay's states[4,2,B,H] carry the four reference nets only;
+ *   - Adam over the 2 P block is two independent Adams with one lr and step; gradient-norm clipping is JOINT over both
+ *     critics (clip_grad_norm_ over the twin module), and the critic norm of r2d2_learner_grad_norms is that joint norm;
+ *     the hard copy, the Polyak blend and the data-parallel exchange cover the whole block.
+ * NULL options = r2d2_learner_create. */
+typedef struct {
+  int twin_critic;   /* 0 or 1 */
+} r2d2_learner_options;
+int r2d2_learner_create_ex(r2d2_learner_t** out, const r2d2_learner_config* cfg, const r2d2_learner_options* options);
+/* Target policy smoothing: a' = clip(mu'(s) + clip(sigma z, -clip, clip), -1, 1) on the target actor's actions of the
+ * rows the target critic bootstraps from (rows [Bn+n, Bn+n+L) of its input; the stored actions before them are
+ * untouched); every target critic sees the same a'.  z comes from r2d2_target_smoothing's generator with key (seed, rank)
+ * and iter = the index of the iteration that trains on the batch (critic phases run so far; r2d2_learner_set_step_count
+ * sets it too), so a pipelined, a sequential and a resumed run draw the same noise.  sigma = 0 (the default) is off: no
+ * launch.  sigma finite >= 0 and clip finite > 0, else R2D2_ERR_ARG; R2D2_ERR_STATE while a target phase has run
+ * ahead and not yet been consumed by a critic phase. */
+int r2d2_learner_set_target_smoothing(r2d2_learner_t* l, float sigma, float clip, unsigned int seed, unsigned int rank);
+/* DEVICE address of critic 2's q [L,B,A] (NULL without the twin), critic 2's offset P' in floats inside each critic
+ * block (0 without the twin) and the arena bytes the twin added (0 without it).  Critic 2's loss is losses[2] of
+ * r2d2_learner_buffers. */
+int r2d2_learner_twin_buffers(r2d2_learner_t* l, float** q2, long long* critic2_offset, size_t* twin_bytes);
+/* The smoothing kernel alone: out[e] = clip(mu[e] + clip(sigma z_e, -clip, clip), -1, 1), e < n (out may be mu).
+ * z_e: Philox4x32-10 with key = (seed, rank), counter = (e >> 2, (uint32) iter, iter >> 32, 0); the output words
+ * (x0, x1) serve e % 4 in {0, 1} and (x2, x3) serve {2, 3}; u = (2 (x >> 9) + 1) 2^-24; z = sqrt(-2 ln u_a) cos(2 pi u_b)
+ * for the even element of a pair and sin for the odd one, (u_a, u_b) the pair's two words, in fp32 with precise logf,
+ * sqrtf and sincospif.  One launch. */
+int r2d2_target_smoothing(const float* mu, float* out, long long n, float sigma, float clip, unsigned int seed,
+                          unsigned int rank, unsigned long long iter, r2d2_stream_t stream);
 int r2d2_learner_buffers_get(r2d2_learner_t* l, r2d2_learner_buffers* out);
 /* The batch has two slots.  r2d2_learner_buffers_get returns slot 0 (the only one a simple caller needs); a pipelined
  * caller fills slot 1-s with batch i+1 while the phases of iteration i still read slot s, runs that batch's target

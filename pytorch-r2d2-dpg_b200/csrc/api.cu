@@ -10,6 +10,7 @@
 #include "net.cuh"
 #include "policy.cuh"
 #include "replay.cuh"
+#include "td3.cuh"
 
 namespace r2d2 {
 static thread_local std::string g_last_error;
@@ -269,6 +270,35 @@ int r2d2_replay_tree_level(r2d2_replay_t* r, int level, const float** dev_ptr, l
 int r2d2_learner_create(r2d2_learner_t** out, const r2d2_learner_config* cfg) {
   return learner_create(reinterpret_cast<Learner**>(out), cfg);
 }
+int r2d2_learner_create_ex(r2d2_learner_t** out, const r2d2_learner_config* cfg, const r2d2_learner_options* options) {
+  if (options) R2D2_REQUIRE(options->twin_critic == 0 || options->twin_critic == 1, "twin_critic is 0 or 1");
+  return learner_create(reinterpret_cast<Learner**>(out), cfg, options && options->twin_critic == 1);
+}
+int r2d2_learner_set_target_smoothing(r2d2_learner_t* lh, float sigma, float clip, unsigned int seed, unsigned int rank) {
+  R2D2_REQUIRE(lh, "null");
+  R2D2_REQUIRE(sigma >= 0.0f && std::isfinite(sigma), "target noise sigma is finite and >= 0 (0 = off)");
+  R2D2_REQUIRE(clip > 0.0f && std::isfinite(clip), "target noise clip is finite and > 0");
+  Learner* l = reinterpret_cast<Learner*>(lh);
+  if (l->targets_slot >= 0) {
+    set_last_error("a target phase ran ahead with the old target noise and has not been consumed");
+    return R2D2_ERR_STATE;
+  }
+  l->target_noise = sigma; l->target_noise_clip = clip; l->noise_seed = seed; l->noise_rank = rank;
+  return R2D2_OK;
+}
+int r2d2_learner_twin_buffers(r2d2_learner_t* lh, float** q2, long long* critic2_offset, size_t* twin_bytes) {
+  R2D2_REQUIRE(lh && q2 && critic2_offset && twin_bytes, "null");
+  Learner* l = reinterpret_cast<Learner*>(lh);
+  *q2 = l->q2;
+  *critic2_offset = l->twin ? (long long)l->critic_stride() : 0;
+  *twin_bytes = l->twin_floats * sizeof(float);
+  return R2D2_OK;
+}
+int r2d2_target_smoothing(const float* mu, float* out, long long n, float sigma, float clip, unsigned int seed,
+                          unsigned int rank, unsigned long long iter, r2d2_stream_t stream) {
+  R2D2_REQUIRE(std::isfinite(sigma) && std::isfinite(clip), "sigma and clip are finite");
+  return target_smoothing(mu, out, n, sigma, clip, seed, rank, iter, S(stream));
+}
 int r2d2_learner_destroy(r2d2_learner_t* l) { return learner_destroy(reinterpret_cast<Learner*>(l)); }
 int r2d2_learner_buffers_get(r2d2_learner_t* lh, r2d2_learner_buffers* o) {
   R2D2_REQUIRE(lh && o, "null");
@@ -377,7 +407,7 @@ int r2d2_peer_layout_for(long long n_critic, long long n_actor, int world, r2d2_
 int r2d2_learner_peer_layout(r2d2_learner_t* lh, int world, r2d2_peer_layout* out) {
   R2D2_REQUIRE(lh && out && world >= 2 && world <= kPeerMaxWorld, "peer layout arguments");
   Learner* l = reinterpret_cast<Learner*>(lh);
-  const PeerLayout pl = peer_layout((long long)l->critic_sh.param_count(), (long long)l->actor_sh.param_count(), world);
+  const PeerLayout pl = peer_layout((long long)l->critic_block(), (long long)l->actor_sh.param_count(), world);
   out->bytes = pl.bytes;
   out->off_critic_grads = pl.off_grads[kPeerCritic];
   out->off_actor_grads = pl.off_grads[kPeerActor];
@@ -403,6 +433,7 @@ int r2d2_learner_peer_counters(r2d2_learner_t* lh, unsigned long long* out6, int
 int r2d2_learner_set_step_count(r2d2_learner_t* l, int step) {
   R2D2_REQUIRE(l && step >= 0, "step");
   reinterpret_cast<Learner*>(l)->step = step;
+  reinterpret_cast<Learner*>(l)->critic_iters = step;   // the target noise's iteration index resumes with it
   return R2D2_OK;
 }
 int r2d2_learner_launches_per_iteration(r2d2_learner_t* lh) {

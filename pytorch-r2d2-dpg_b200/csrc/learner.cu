@@ -12,6 +12,12 @@
 // a Polyak target update (target_tau < 1) on the same iterations as the hard copy, fused into the Adam launches: the
 // critic's target in phase 2, the actor's in phase 3.
 //
+// TD3's target (off by default, td3.cuh): with target noise the target actor's actions for the bootstrap rows are
+// smoothed in place right after its head; with the twin critic a second target critic (zero state) runs on the same
+// actions and q_next becomes the elementwise minimum, and in phase 1 a second online critic (zero state) runs its own
+// TD against the same y and its own BPTT into the second half of the critic gradient block.  Critic 1 keeps every other
+// role: the DPG loss of phase 2, the priorities, td_sq and the target written out.
+//
 // The actor burn-in of learner.py:92 is skipped: its state is discarded at learner.py:117 before any use.
 #include "learner.cuh"
 
@@ -21,12 +27,13 @@
 #include "elementwise.cuh"
 #include "gemm.cuh"
 #include "lstm_scan.cuh"
+#include "td3.cuh"
 
 namespace r2d2 {
 
 static size_t align64(size_t n) { return (n + 63) & ~(size_t)63; }
 
-int learner_create(Learner** out, const r2d2_learner_config* cfg) {
+int learner_create(Learner** out, const r2d2_learner_config* cfg, bool twin_critic) {
   R2D2_REQUIRE(out && cfg, "null");
   R2D2_REQUIRE(cfg->obs_size > 0 && cfg->n_actions > 0 && cfg->hidden > 0 && cfg->hidden % 4 == 0, "sizes");
   R2D2_REQUIRE(cfg->batch > 0 && cfg->burn_in >= 0 && cfg->learning > 0 && cfg->n_step > 0, "window");
@@ -55,6 +62,13 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
   total += ws_ta + ws_tc + ws_c1 + ws_a1 + ws_c2;
   total += 2 * align64(B);   // importance weights of the two slots, carved last: the buffers above keep their offsets
   total += align64(8) + align64(4 * (size_t)kGradNormBlocks);   // optimiser scalars + tickets, norm partials (2 x double)
+  // twin critic: carved last, only when on, so the default arena and every offset above are unchanged
+  l->twin = twin_critic;
+  if (twin_critic) {
+    // target / online critic 2 chains, q_next2 / q2 / dq2, td_sq2
+    l->twin_floats = align64(ws_tc) + align64(ws_c1) + 3 * n_lba + align64((size_t)L * B);
+    total += l->twin_floats;
+  }
   R2D2_CUDA_TRY(cudaMalloc(&l->arena, total * sizeof(float)));
   R2D2_CUDA_TRY(cudaMemset(l->arena, 0, total * sizeof(float)));
   l->arena_floats = total;
@@ -84,6 +98,13 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg) {
   l->optim = take(8);
   l->norm_ticket = reinterpret_cast<unsigned int*>(l->optim + 4);   // zeroed with the arena
   l->norm_part = reinterpret_cast<double*>(take(4 * (size_t)kGradNormBlocks));
+  if (twin_critic) {
+    l->ws_tc_2 = ChainWs::carve(take(ws_tc), l->critic_sh, Tt, B, 1);
+    l->ws_c1_2 = ChainWs::carve(take(ws_c1), l->critic_sh, Tc, B, 1);
+    l->ws_tc_2.inference_only = true;
+    l->q_next2 = take(n_lba); l->q2 = take(n_lba); l->dq2 = take(n_lba);
+    l->td_sq2 = take((size_t)L * B);
+  }
   R2D2_CUDA_TRY(cudaStreamSynchronize(0));
   learner_select_batch(l, 0);
   {   // R2D2_OVERLAP_INPUTS=0 disables the side stream (A/B)
@@ -186,10 +207,21 @@ int learner_target_phase(Learner* l, int slot, cudaStream_t st) {
     R2D2_TRY(peer_reduce(*l->peer, kPeerActor, st));
   }
   R2D2_CUDA_TRY(cudaMemcpyAsync(l->act_tc, b.act, sizeof(float) * (size_t)(Bn + n) * B * A, cudaMemcpyDeviceToDevice, st));
-  R2D2_TRY(net_head_forward(l->actor_sh, Pa_t, l->ws_ta, Bn + n, Tt, B, 1, l->act_tc + (size_t)(Bn + n) * B * A, A, st));
+  float* act_next = l->act_tc + (size_t)(Bn + n) * B * A;
+  R2D2_TRY(net_head_forward(l->actor_sh, Pa_t, l->ws_ta, Bn + n, Tt, B, 1, act_next, A, st));
+  // TD3 target policy smoothing, in place on the rows the target critics bootstrap from (stored actions stay as they are)
+  if (l->target_noise > 0.0f)
+    R2D2_TRY(target_smoothing(act_next, act_next, (long long)L * B * A, l->target_noise, l->target_noise_clip,
+                              l->noise_seed, l->noise_rank, (unsigned long long)l->critic_iters, st));
   // target critic: stored actions while burning in, target-actor actions afterwards (learner.py:95,106)
   R2D2_TRY(net_forward(l->critic_sh, Pc_t, l->ws_tc, b.obs, l->act_tc, st_tc, st_tc + BH, Tt, B, 1, st));
   R2D2_TRY(net_head_forward(l->critic_sh, Pc_t, l->ws_tc, Bn + n, Tt, B, 1, l->q_next, A, st));
+  if (l->twin) {   // target critic 2 from the zero state on the same actions, then q_next = min(q'_1, q'_2)
+    const NetParams Pc_t2 = NetParams::from_flat(c.target_critic_params + l->critic_stride(), l->critic_sh);
+    R2D2_TRY(net_forward(l->critic_sh, Pc_t2, l->ws_tc_2, b.obs, l->act_tc, nullptr, nullptr, Tt, B, 1, st));
+    R2D2_TRY(net_head_forward(l->critic_sh, Pc_t2, l->ws_tc_2, Bn + n, Tt, B, 1, l->q_next2, A, st));
+    R2D2_TRY(q_min(l->q_next, l->q_next2, (long long)L * B * A, st));
+  }
   l->targets_slot = slot;
   l->launches_target = (int)(launch_count() - launches0);
   return R2D2_OK;
@@ -225,8 +257,24 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
   tp.is_weight = l->importance_weighting ? l->is_weight : nullptr;
   R2D2_TRY(td_priority(tp, st, TdOptions{l->rescaling, l->rescaling_eps, l->priority_metric}));
 
-  R2D2_CUDA_TRY(cudaMemsetAsync(c.critic_grads, 0, sizeof(float) * l->critic_sh.param_count(), st));
+  R2D2_CUDA_TRY(cudaMemsetAsync(c.critic_grads, 0, sizeof(float) * l->critic_block(), st));
   R2D2_TRY(net_backward(l->critic_sh, Pc, &Gc, l->ws_c1, l->obs, l->act, l->dq, Bn, Tc, B, 1, nullptr, nullptr, st));
+  if (l->twin) {
+    // critic 2 from the zero state over the same rows with the stored actions, its TD against the same y (q_next is
+    // already the minimum; target / priority stay critic 1's), its loss into losses[2], its BPTT into the second half
+    const size_t off = l->critic_stride();
+    const NetParams Pc2 = NetParams::from_flat(c.critic_params + off, l->critic_sh);
+    const NetParams Gc2 = NetParams::from_flat(c.critic_grads + off, l->critic_sh);
+    R2D2_TRY(net_forward(l->critic_sh, Pc2, l->ws_c1_2, l->obs, l->act, nullptr, nullptr, Tc, B, 1, st));
+    R2D2_TRY(net_head_forward(l->critic_sh, Pc2, l->ws_c1_2, Bn, Tc, B, 1, l->q2, A, st));
+    TdPriorityParams tp2 = tp;
+    tp2.q = l->q2; tp2.target = nullptr; tp2.dq = l->dq2; tp2.td_sq = l->td_sq2; tp2.priority = nullptr;
+    tp2.loss_sum = l->losses + 2;
+    R2D2_TRY(td_priority(tp2, st, TdOptions{l->rescaling, l->rescaling_eps, l->priority_metric}));
+    R2D2_TRY(net_backward(l->critic_sh, Pc2, &Gc2, l->ws_c1_2, l->obs, l->act, l->dq2, Bn, Tc, B, 1, nullptr, nullptr,
+                          st));
+  }
+  l->critic_iters += 1;
   if (l->peer) R2D2_TRY(peer_signal(*l->peer, kPeerCritic, st));
   l->launches_phase[0] = (int)(launch_count() - launches0);
   return R2D2_OK;
@@ -300,7 +348,7 @@ int learner_actor_phase(Learner* l, float grad_scale, cudaStream_t st) {
   // on an update iteration the critic's target is blended here: nothing later in the iteration changes the critic's
   // weights, and no target chain runs before the iteration ends
   R2D2_TRY(optimiser_step(l, kPeerCritic, c.critic_params, c.critic_exp_avg, c.critic_exp_avg_sq, c.target_critic_params,
-                          (long long)l->critic_sh.param_count(), c.critic_lr, grad_scale, st));   // learner.py:114
+                          (long long)l->critic_block(), c.critic_lr, grad_scale, st));   // learner.py:114; twin: both
   {
     // the other slot already holds the next batch (its target chains ran ahead): the input projection of ITS online
     // critic chain needs the weights Adam just wrote and nothing else - side stream, under the scans of this phase
@@ -341,7 +389,7 @@ int learner_finish_phase(Learner* l, float grad_scale, cudaStream_t st) {
   if (l->target_tau == 1.0f && c.target_update_interval > 0 && l->step % c.target_update_interval == 0) {  // :131-132
     R2D2_CUDA_TRY(cudaMemcpyAsync(c.target_actor_params, c.actor_params, sizeof(float) * l->actor_sh.param_count(),
                                   cudaMemcpyDeviceToDevice, st));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(c.target_critic_params, c.critic_params, sizeof(float) * l->critic_sh.param_count(),
+    R2D2_CUDA_TRY(cudaMemcpyAsync(c.target_critic_params, c.critic_params, sizeof(float) * l->critic_block(),
                                   cudaMemcpyDeviceToDevice, st));
   }
   l->launches_phase[2] = (int)(launch_count() - launches0);
@@ -355,7 +403,7 @@ int learner_attach_peers(Learner* l, int rank, int world, void* const* peer_base
   PeerExchange* x = new PeerExchange();
   x->rank = rank;
   x->world = world;
-  x->lay = peer_layout((long long)l->critic_sh.param_count(), (long long)l->actor_sh.param_count(), world);
+  x->lay = peer_layout((long long)l->critic_block(), (long long)l->actor_sh.param_count(), world);
   for (int k = 0; k < world; ++k) {
     if (!peer_bases[k]) { delete x; R2D2_REQUIRE(false, "null peer buffer"); }
     x->ptrs.base[k] = static_cast<char*>(peer_bases[k]);

@@ -55,11 +55,29 @@ struct Learner {
   int rescaling = kRescaleReference;
   float rescaling_eps = 0.0f;
   int priority_metric = kPrioritySquared;
+  // TD3's target (td3.cuh), off by default.  twin: a create-time choice - every cfg.critic_* block holds 2 P' floats
+  // [critic 1 | pad | critic 2 | pad], P = critic_sh.param_count() and P' = P rounded up to 64 floats, so that critic 2's
+  // matrices sit at the same 256-byte alignment as critic 1's (the GEMM kernels load them with vector accesses); the
+  // padding stays zero.  Critic 1 is the reference's critic with its stored state, critic 2 and its target start from
+  // the zero state.  target_noise > 0: smoothing of the target actor's actions, keyed on (noise_seed, noise_rank) and
+  // critic_iters.
+  bool twin = false;
+  float target_noise = 0.0f, target_noise_clip = 0.5f;
+  unsigned int noise_seed = 0, noise_rank = 0;
+  // critic phases run so far: the index of the iteration that trains on the batch a target phase prepares (a target
+  // phase run ahead after critic phase i sees i + 1, one inside critic phase i sees i); r2d2_learner_set_step_count sets it
+  long long critic_iters = 0;
+  size_t twin_floats = 0;   // arena floats carved for the twin (0 without it)
+  size_t critic_stride() const { return twin ? (critic_sh.param_count() + 63) & ~(size_t)63 : critic_sh.param_count(); }
+  size_t critic_block() const { return critic_stride() * (twin ? 2 : 1); }
   // intermediates / results
   float *act_tc = nullptr, *q = nullptr, *q_next = nullptr, *target = nullptr, *dq = nullptr, *mu = nullptr,
         *q_pi = nullptr, *dq_pi = nullptr, *dpre_actor = nullptr, *td_sq = nullptr, *priority = nullptr,
         *losses = nullptr;
   ChainWs ws_ta, ws_tc, ws_c1, ws_a1, ws_c2;
+  // twin only: target critic 2 / online critic 2 chains, and critic 2's q_next, q, dq and td_sq (scratch)
+  ChainWs ws_tc_2, ws_c1_2;
+  float *q_next2 = nullptr, *q2 = nullptr, *dq2 = nullptr, *td_sq2 = nullptr;
   // data-parallel learner: gradient blocks live in a peer-mapped buffer and are summed by peer.cu's kernels in this
   // learner's own stream (null: single GPU, or the caller reduces cfg.*_grads itself between the phases)
   PeerExchange* peer = nullptr;
@@ -68,7 +86,7 @@ struct Learner {
   }
 };
 
-int learner_create(Learner** out, const r2d2_learner_config* cfg);
+int learner_create(Learner** out, const r2d2_learner_config* cfg, bool twin_critic = false);
 int learner_destroy(Learner* l);
 int learner_select_batch(Learner* l, int slot);
 // target chains of the batch in `slot` (learner.py:87,94-95,106): q_next for the next learner_critic_phase on that slot.

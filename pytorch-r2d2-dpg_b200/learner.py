@@ -28,6 +28,12 @@ h(x) = sign(x)(sqrt(|x|+1) - 1), no eps x and no inverse on the bootstrap; inver
 y = h_eps(R + gamma^n (1-d) h_eps^-1(Q')), h_eps = h + eps x), R2D2_RESCALING_EPS (eps, default 1e-3) and
 R2D2_PRIORITY_METRIC=squared|abs (default squared: the reference's eta max + (1-eta) mean of squared TD errors; abs: of
 absolute ones, R2D2's).  Any other value raises.  The checkpoint records them and a resume under other settings is refused.
+
+TD3's target (r2d2_b200.td3_options): R2D2_TWIN_CRITIC=0|1 (default 0; 1 adds a second critic and target critic and
+bootstraps from the minimum of the two), R2D2_TARGET_NOISE (target policy smoothing sigma, default 0 = off),
+R2D2_TARGET_NOISE_CLIP (default 0.5) and R2D2_TARGET_NOISE_SEED (default 0).  model.pt keeps its four reference keys
+(critic 1 is the reference's critic); the resumable checkpoint holds critic 2 as well, and a resume across a twin /
+single-critic change is refused.
 """
 import os
 from time import sleep, time
@@ -91,15 +97,16 @@ class Learner:
         self.is_exponent = float(os.environ.get("R2D2_IS_EXPONENT", 0.0))
         self.target_tau = float(os.environ.get("R2D2_TARGET_TAU", 1.0))
         self.grad_clip_norm = float(os.environ.get("R2D2_GRAD_CLIP", 0.0))
-        from r2d2_b200 import td_options
+        from r2d2_b200 import td3_options, td_options
         self.td_options = td_options.from_environ()
+        self.td3_options = td3_options.from_environ()
         cfg = PathConfig(obs=self.obs_size, act=self.n_actions, hidden=self.hidden, batch=self.batch_size,
                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
                          gamma=self.gamma, actor_lr=self.actor_lr, critic_lr=self.critic_lr,
                          target_interval=self.target_update_inverval, priority_exponent=self.priority_exponent,
                          is_exponent=self.is_exponent, target_tau=self.target_tau, grad_clip_norm=self.grad_clip_norm,
                          value_rescaling=self.td_options.value_rescaling, rescaling_eps=self.td_options.rescaling_eps,
-                         priority_metric=self.td_options.priority_metric)
+                         priority_metric=self.td_options.priority_metric, **self.td3_options)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
@@ -140,7 +147,7 @@ class Learner:
         self.engine.flush()
         self.engine.discard_prefetched()      # target chains that already ran for the next batch used the old target nets
         self.engine.flat['target_actor'].copy_(self.engine.flat['actor'])
-        self.engine.flat['target_critic'].copy_(self.engine.flat['critic'])
+        self.engine.flat['target_critic'].copy_(self.engine.flat['critic'])   # twin critic: the whole [1 | 2] block
 
     def _ingest(self):
         for i in self.dist_env.owned_actors(self.n_actors):   # all of them in a single-process run (learner.py:70-73)

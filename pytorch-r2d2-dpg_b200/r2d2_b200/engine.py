@@ -11,6 +11,7 @@ replay_memory.py:67-136) with the sum tree in HBM.
 from __future__ import annotations
 
 import math
+import numbers
 from collections import OrderedDict
 from ctypes import byref, c_int, c_longlong, c_void_p
 from dataclasses import dataclass
@@ -41,7 +42,12 @@ class PathConfig:
 
     n-step target and priorities (r2d2_b200.td_options): `value_rescaling` "reference" (the reference's h0 without an
     inverse on the bootstrap) or "invertible" (R2D2's h_eps(R + gamma^n (1-d) h_eps^-1(Q')) with eps = `rescaling_eps`,
-    in [0, 1]); `priority_metric` "squared" (the reference's) or "abs" (R2D2's absolute TD errors)."""
+    in [0, 1]); `priority_metric` "squared" (the reference's) or "abs" (R2D2's absolute TD errors).
+
+    TD3's target (include/r2d2_b200.h, r2d2_learner_options): `twin_critic` adds a second critic and target critic and
+    bootstraps from the minimum of the two target critics; `target_noise` sigma >= 0 (0 = off) smooths the target actor's
+    actions with clip(sigma z, -c, c), c = `target_noise_clip` > 0, z keyed on (`target_noise_seed`, rank) and the
+    iteration index.  TD3's usual setting: twin, sigma 0.2, c 0.5, target_tau 0.005 at target_interval 1."""
     obs: int
     act: int
     hidden: int = 128
@@ -61,9 +67,23 @@ class PathConfig:
     value_rescaling: str = "reference"
     rescaling_eps: float = td_options.DEFAULT_EPS
     priority_metric: str = "squared"
+    twin_critic: bool = False
+    target_noise: float = 0.0
+    target_noise_clip: float = 0.5
+    target_noise_seed: int = 0
 
     def __post_init__(self):
         td_options.validate(self.value_rescaling, self.rescaling_eps, self.priority_metric)
+        if not isinstance(self.twin_critic, bool):
+            raise ValueError("twin_critic must be True or False, got %r" % (self.twin_critic,))
+        for name, lo_ok in (("target_noise", lambda v: v >= 0.0), ("target_noise_clip", lambda v: v > 0.0)):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, numbers.Real) or not (math.isfinite(v) and lo_ok(v)):
+                raise ValueError("%s must be finite and %s, got %r" % (name, ">= 0 (0 = off)" if name == "target_noise"
+                                                                        else "> 0", v))
+        s = self.target_noise_seed
+        if isinstance(s, bool) or not isinstance(s, (int, np.integer)) or not 0 <= s < 2 ** 32:
+            raise ValueError("target_noise_seed must be an integer in [0, 2**32), got %r" % (s,))
         for name in ("priority_exponent", "is_exponent"):
             v = getattr(self, name)
             if not 0.0 <= v <= 1.0:
@@ -139,12 +159,20 @@ class LearnerEngine:
         na = sum(int(np.prod(s)) for s in param_shapes(cfg, False).values())
         nc = sum(int(np.prod(s)) for s in param_shapes(cfg, True).values())
         z = lambda n: torch.zeros(n, dtype=torch.float32, device=self.device)  # noqa: E731
-        self.flat = {"actor": z(na), "critic": z(nc), "target_actor": z(na), "target_critic": z(nc)}
-        self.grads = {"actor": z(na), "critic": z(nc)}
-        self.exp_avg = {"actor": z(na), "critic": z(nc)}
-        self.exp_avg_sq = {"actor": z(na), "critic": z(nc)}
+        # twin critic: every critic block is [critic 1 | pad | critic 2 | pad], critic 2 at P' = P rounded up to 64 floats
+        # (include/r2d2_b200.h); views("critic") stays critic 1
+        self._n_critic = nc
+        self._critic2_off = -(-nc // 64) * 64 if cfg.twin_critic else 0
+        ncb = 2 * self._critic2_off if cfg.twin_critic else nc
+        self.flat = {"actor": z(na), "critic": z(ncb), "target_actor": z(na), "target_critic": z(ncb)}
+        self.grads = {"actor": z(na), "critic": z(ncb)}
+        self.exp_avg = {"actor": z(na), "critic": z(ncb)}
+        self.exp_avg_sq = {"actor": z(na), "critic": z(ncb)}
         g = torch.Generator().manual_seed(seed)
         self.load_state_dicts(init_reference_params(cfg, False, g), init_reference_params(cfg, True, g))
+        if cfg.twin_critic:                      # drawn after the four reference nets: their values do not move
+            c2 = init_reference_params(cfg, True, g)
+            self.load_state_dicts(None, None, critic2=c2, target_critic2=c2)
         c = nv.LearnerConfig(cfg.obs, cfg.act, cfg.hidden, cfg.batch, cfg.burn_in, cfg.learning, cfg.n_step,
                              cfg.gamma, cfg.actor_lr, cfg.critic_lr, cfg.eta, cfg.target_interval,
                              self.flat["actor"].data_ptr(), self.flat["critic"].data_ptr(),
@@ -153,7 +181,11 @@ class LearnerEngine:
                              self.exp_avg["actor"].data_ptr(), self.exp_avg_sq["actor"].data_ptr(),
                              self.exp_avg["critic"].data_ptr(), self.exp_avg_sq["critic"].data_ptr())
         self._h = c_void_p()
-        nv.check(self.lib.r2d2_learner_create(byref(self._h), byref(c)))
+        if cfg.twin_critic:
+            nv.check(self.lib.r2d2_learner_create_ex(byref(self._h), byref(c), byref(nv.LearnerOptions(1))))
+        else:
+            nv.check(self.lib.r2d2_learner_create(byref(self._h), byref(c)))
+        self._rank = 0
         T, B, O, A, H, L = cfg.rows, cfg.batch, cfg.obs, cfg.act, cfg.hidden, cfg.learning
         dev = self.device
         # the batch has two slots (include/r2d2_b200.h): the attributes obs .. uniforms are views of the slot the NEXT
@@ -190,7 +222,17 @@ class LearnerEngine:
         self.target_q_value = nv.view_f32(b.target_q_value, (L * B, A), dev)
         self.td_sq = nv.view_f32(b.td_sq, (L * B,), dev)
         self.priority = nv.view_f32(b.priority, (B,), dev)
-        self.losses = nv.view_f32(b.losses, (2,), dev)
+        self.losses = nv.view_f32(b.losses, (3 if cfg.twin_critic else 2,), dev)
+        # TD3: critic 2's q (losses[2] is its loss) and the arena bytes the twin added; target noise only when asked for
+        q2, off2, tb = c_void_p(), c_longlong(), nv.c_size_t()
+        nv.check(self.lib.r2d2_learner_twin_buffers(self._h, byref(q2), byref(off2), byref(tb)))
+        if int(off2.value) != self._critic2_off:
+            raise nv.NativeError("critic 2 sits at float %d of the library's critic block, not %d"
+                                 % (off2.value, self._critic2_off))
+        self.q_value2 = nv.view_f32(q2.value, (L * B, A), dev) if cfg.twin_critic else None
+        self.twin_added_bytes = int(tb.value)
+        if cfg.target_noise > 0:
+            self.set_target_smoothing()
         self.world = 1
         self._dist = None
         self._sync = None
@@ -211,6 +253,21 @@ class LearnerEngine:
         nv.check(self.lib.r2d2_learner_set_priority_metric(self._h, metric))
         self.cfg.value_rescaling, self.cfg.rescaling_eps, self.cfg.priority_metric = value_rescaling, rescaling_eps, \
             priority_metric
+
+    def set_target_smoothing(self, sigma: float | None = None, clip: float | None = None, seed: int | None = None,
+                             rank: int | None = None):
+        """TD3 target policy smoothing (sigma 0 = off); arguments left out keep the engine's setting.  The noise is a
+        function of (seed, rank, iteration index, element): data-parallel ranks draw different noise, a resumed run the
+        same as an uninterrupted one.  Refused while a prefetched batch's target chains have already run."""
+        c = self.cfg
+        sigma = c.target_noise if sigma is None else float(sigma)
+        clip = c.target_noise_clip if clip is None else float(clip)
+        seed = c.target_noise_seed if seed is None else int(seed)
+        rank = self._rank if rank is None else int(rank)
+        if not (0 <= seed < 2 ** 32 and 0 <= rank < 2 ** 32):
+            raise ValueError("seed and rank are integers in [0, 2**32), got %r, %r" % (seed, rank))
+        nv.check(self.lib.r2d2_learner_set_target_smoothing(self._h, sigma, clip, seed, rank))
+        c.target_noise, c.target_noise_clip, c.target_noise_seed, self._rank = sigma, clip, seed, rank
 
     def _guard_fill(self):
         if self._targets_ahead:
@@ -253,20 +310,46 @@ class LearnerEngine:
     def views(self, net: str, what: str = "params"):
         self.flush()
         src = {"params": self.flat, "grads": self.grads, "exp_avg": self.exp_avg, "exp_avg_sq": self.exp_avg_sq}[what]
-        return flat_views(src[net], self.cfg, "critic" in net)
+        return flat_views(self._block(src, net), self.cfg, "critic" in net)
+
+    @property
+    def nets(self) -> tuple:
+        """The engine's nets: the reference's four, and critic 2 / target critic 2 with the twin critic."""
+        return ("actor", "target_actor", "critic", "target_critic") + (
+            ("critic2", "target_critic2") if self.cfg.twin_critic else ())
+
+    def _block(self, src: dict, net: str) -> torch.Tensor:
+        """A net's flat block in one of the buffer dicts: with the twin, "critic" / "target_critic" (and their moments
+        and gradients) are the first half of the 2 P block, "critic2" / "target_critic2" the second."""
+        if net.endswith("2"):
+            if not self.cfg.twin_critic or net not in ("critic2", "target_critic2"):
+                raise KeyError("%r: this engine has %s" % (net, ", ".join(self.nets)))
+            return src[net[:-1]][self._critic2_off:self._critic2_off + self._n_critic]
+        t = src[net]
+        return t[:self._n_critic] if "critic" in net and self.cfg.twin_critic else t
 
     def state_dict(self, net: str):
         return OrderedDict((k, v.detach().clone()) for k, v in self.views(net).items())
 
-    def load_state_dicts(self, actor, critic, target_actor=None, target_critic=None):
+    def load_state_dicts(self, actor, critic, target_actor=None, target_critic=None, critic2=None, target_critic2=None):
+        """The reference's four nets (a target defaults to its net), and with the twin critic 2 and its target
+        (target_critic2 defaults to critic2; left out, critic 2 keeps its weights).  actor / critic None: unchanged."""
         def put(net, sd):
             for k, v in self.views(net).items():
                 v.copy_(torch.as_tensor(np.asarray(sd[k]) if not isinstance(sd[k], torch.Tensor) else sd[k],
                                         dtype=torch.float32).to(self.device))
-        put("actor", actor)
-        put("critic", critic)
-        put("target_actor", target_actor if target_actor is not None else actor)
-        put("target_critic", target_critic if target_critic is not None else critic)
+        if actor is not None:
+            put("actor", actor)
+            put("target_actor", target_actor if target_actor is not None else actor)
+        if critic is not None:
+            put("critic", critic)
+            put("target_critic", target_critic if target_critic is not None else critic)
+        if critic2 is not None or target_critic2 is not None:
+            if not self.cfg.twin_critic:
+                raise ValueError("critic 2 weights given to an engine without the twin critic")
+            if critic2 is not None:
+                put("critic2", critic2)
+            put("target_critic2", target_critic2 if target_critic2 is not None else critic2)
 
     def enable_data_parallel(self, require: bool | None = None):
         """Gradients are averaged over ranks at the two optimiser steps: by the library's own kernels over NVLink peer
@@ -283,6 +366,9 @@ class LearnerEngine:
             self.world = dist.get_world_size()
             self._sync = GradSync(dist, self.world)
             self._sync_actor = GradSync(dist, self.world)
+            self._rank = dist.get_rank()             # the target noise is keyed on (seed, rank): ranks draw their own
+            if self.cfg.target_noise > 0:
+                self.set_target_smoothing()
             if self._dp_mode == "peer":
                 self._attach_peers(dist)
             # both modes defer phase 3: the actor's weights are final only after it ran
@@ -451,18 +537,27 @@ class LearnerEngine:
         """Everything a restart needs: the four nets (reference keys), both Adam moment sets, the step counter, and the
         n-step target / priority options the critic was trained under."""
         torch.cuda.synchronize(self.device)
-        out = {net: self.state_dict(net) for net in ("actor", "target_actor", "critic", "target_critic")}
-        for net in ("actor", "critic"):
+        out = {net: self.state_dict(net) for net in self.nets}
+        for net in [n for n in self.nets if not n.startswith("target")]:
             out[net + "_optimizer"] = {"exp_avg": OrderedDict((k, v.detach().clone()) for k, v in self.views(net, "exp_avg").items()),
                                        "exp_avg_sq": OrderedDict((k, v.detach().clone()) for k, v in self.views(net, "exp_avg_sq").items())}
         out["step"] = self.step_count
         o = self.td_options
         out.update(value_rescaling=o.value_rescaling, rescaling_eps=float(o.rescaling_eps), priority_metric=o.priority_metric)
+        c = self.cfg
+        out.update(twin_critic=bool(c.twin_critic), target_noise=float(c.target_noise),
+                   target_noise_clip=float(c.target_noise_clip), target_noise_seed=int(c.target_noise_seed))
         return out
 
     def load_training_state(self, st: dict):
         """Refuses a state saved under other target / priority options: a critic trained in one value space means nothing
-        in the other.  A state without them was saved by a build that had only the reference's (reference, squared)."""
+        in the other.  A state without them was saved by a build that had only the reference's (reference, squared).
+        Likewise a twin-critic state and a single-critic engine, or the other way round (a state without the key is
+        single-critic).  The target-noise settings of the state are informational: the engine keeps its own."""
+        saved_twin = bool(st.get("twin_critic", False))
+        if saved_twin != bool(self.cfg.twin_critic):
+            raise ValueError("training state was saved with twin_critic=%r; this engine runs twin_critic=%r"
+                             % (saved_twin, bool(self.cfg.twin_critic)))
         def key(o):
             return (o.value_rescaling, float(np.float32(o.rescaling_eps)) if o.value_rescaling == "invertible" else None,
                     o.priority_metric)
@@ -474,8 +569,9 @@ class LearnerEngine:
                              "engine runs value_rescaling=%r rescaling_eps=%r priority_metric=%r"
                              % (saved.value_rescaling, saved.rescaling_eps, saved.priority_metric, mine.value_rescaling,
                                 mine.rescaling_eps, mine.priority_metric))
-        self.load_state_dicts(st["actor"], st["critic"], st.get("target_actor"), st.get("target_critic"))
-        for net in ("actor", "critic"):
+        self.load_state_dicts(st["actor"], st["critic"], st.get("target_actor"), st.get("target_critic"),
+                              st.get("critic2"), st.get("target_critic2"))
+        for net in [n for n in self.nets if not n.startswith("target")]:
             opt = st.get(net + "_optimizer")
             if opt is not None:
                 for what in ("exp_avg", "exp_avg_sq"):

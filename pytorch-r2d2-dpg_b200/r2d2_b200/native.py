@@ -8,7 +8,8 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, Structure, byref, c_char_p, c_double, c_float, c_int, c_longlong, c_size_t, c_void_p
+from ctypes import (POINTER, Structure, byref, c_char_p, c_double, c_float, c_int, c_longlong, c_size_t, c_uint,
+                    c_ulonglong, c_void_p)
 
 import numpy as np
 import torch
@@ -53,6 +54,10 @@ class LearnerConfig(Structure):
 
 class TdOptions(Structure):
     _fields_ = [("rescaling", c_int), ("eps", c_float), ("priority_metric", c_int)]
+
+
+class LearnerOptions(Structure):
+    _fields_ = [("twin_critic", c_int)]
 
 
 class PeerLayout(Structure):
@@ -124,6 +129,11 @@ SIGNATURES = {
     "r2d2_replay_decode": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "r2d2_replay_tree_level": (c_int, [c_void_p, c_int, POINTER(c_void_p), POINTER(c_longlong)]),
     "r2d2_learner_create": (c_int, [POINTER(c_void_p), POINTER(LearnerConfig)]),
+    "r2d2_learner_create_ex": (c_int, [POINTER(c_void_p), POINTER(LearnerConfig), POINTER(LearnerOptions)]),
+    "r2d2_learner_set_target_smoothing": (c_int, [c_void_p, c_float, c_float, c_uint, c_uint]),
+    "r2d2_learner_twin_buffers": (c_int, [c_void_p, POINTER(c_void_p), POINTER(c_longlong), POINTER(c_size_t)]),
+    "r2d2_target_smoothing": (c_int, [c_void_p, c_void_p, c_longlong, c_float, c_float, c_uint, c_uint, c_ulonglong,
+                                      c_void_p]),
     "r2d2_learner_destroy": (c_int, [c_void_p]),
     "r2d2_learner_buffers_get": (c_int, [c_void_p, POINTER(LearnerBuffers)]),
     "r2d2_learner_critic_phase": (c_int, [c_void_p, c_void_p]),
@@ -213,4 +223,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "LearnerConfig", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "LearnerConfig", "LearnerOptions", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
