@@ -28,8 +28,9 @@ def nstep_rewards(raw, n_step, gamma):
 
 
 def episode_priorities(critic, target_actor, target_critic, obs, act, rew, term, *, burn_in, learning, n_step,
-                       gamma, eta=0.9):
-    """obs [N,O], act [N,A], rew [N] (already n-step sums), term [N]; N = E + n_step.  Returns priorities [E - burn_in - learning]."""
+                       gamma, eta=0.9, rescaling="reference", eps=1e-3, metric="squared"):
+    """obs [N,O], act [N,A], rew [N] (already n-step sums), term [N]; N = E + n_step.  Returns priorities [E - burn_in - learning].
+    rescaling / eps / metric: the TD options of learner_oracle.td_targets_and_priorities."""
     f = lambda a: np.asarray(a, np.float32).astype(np.float64)  # noqa: E731
     N = obs.shape[0]
     E = N - n_step
@@ -41,12 +42,22 @@ def episode_priorities(critic, target_actor, target_critic, obs, act, rew, term,
     a_t = lo.net_forward(P(target_actor), f(obs)[:, None, :], z, z, critic=False)["out"]    # [N, 1, A]
     x_t = np.concatenate((f(obs)[:, None, :], a_t), 2)
     q_t = lo.net_forward(P(target_critic), x_t, z, z, critic=True)["out"][:, 0]             # [N, A]
+    return window_priorities(q, q_t, rew, term, burn_in=burn_in, learning=learning, n_step=n_step, gamma=gamma, eta=eta,
+                             rescaling=rescaling, eps=eps, metric=metric)
+
+
+def window_priorities(q, q_t, rew, term, *, burn_in, learning, n_step, gamma, eta=0.9, rescaling="reference", eps=1e-3,
+                      metric="squared"):
+    """The windowed part on given critic outputs: q [E,A] online, q_t [N,A] target; rew, term [N].  "abs" takes |td| in
+    place of td^2."""
+    E = q.shape[0]
     td = np.zeros(E)
     for i in range(burn_in, E):
-        y = lo.value_rescale(rew[i] + gamma ** n_step * (1.0 - term[i + n_step - 1]) * q_t[i + n_step])
+        y = lo.n_step_target(rew[i], gamma ** n_step * (1.0 - term[i + n_step - 1]), q_t[i + n_step], rescaling, eps)
         td[i] = (q[i] - y).mean()
     out = []
     for i in range(burn_in + learning, E):
-        w = td[i - learning + 1:i + 1] ** 2
+        w = td[i - learning + 1:i + 1]
+        w = np.abs(w) if metric == "abs" else w ** 2
         out.append(eta * w.max() + (1 - eta) * w.mean())
     return np.asarray(out, np.float64)

@@ -8,16 +8,9 @@ import pytest
 import torch
 
 from conftest import rel_l2
+from learner_harness import col_err
 from oracle import learner_oracle as lo
 from oracle import ref_port
-
-
-def col_err(x, ref, A):
-    """max over action columns j of ||x_j - ref_j|| / (||ref|| / sqrt(A)); both reshaped to [-1, A]."""
-    x = np.asarray(x, np.float64).reshape(-1, A)
-    ref = np.asarray(ref, np.float64).reshape(-1, A)
-    rms_col = np.linalg.norm(ref) / np.sqrt(A)
-    return float(np.linalg.norm(x - ref, axis=0).max() / max(rms_col, 1e-30))
 
 
 def action_views(block, O, A):

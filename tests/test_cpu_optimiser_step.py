@@ -1,26 +1,20 @@
-"""Optimiser-step extras on the host side: the float64 oracle (tests/optim_oracle.py) against torch's own
+"""Optimiser-step extras on the host side: the float64 oracle's target_tau and grad_clip against torch's own
 clip_grad_norm_ + Adam + soft_update on float64 modules, PathConfig and drop-in validation, and the compiler's report
 on the new kernels (no spills, no local memory)."""
-import os
-import re
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
+from learner_harness import fake_engine_learner
 from oracle import learner_oracle as lo
 from oracle import ref_port
-from optim_oracle import ClipHook, PolyakOracle
-from test_cpu_prioritized_replay import _dropin_learner
-from test_cpu_sass_gemm import CSRC, ROOT, _functions, _ops
+from sass_report import functions, library_sass, ops, ptxas_report
 
 
 @pytest.mark.parametrize("tau,interval,clip", [(0.05, 1, 0.1), (0.3, 3, 0.0), (1.0, 2, 1e9), (0.5, 2, 1e-4)])
 def test_oracle_matches_torch_clip_adam_soft_update(tau, interval, clip):
     """Six iterations of the float64 torch port of the reference learner with clip_grad_norm_ before each Adam step and
-    utils.soft_update on the update iterations, against PolyakOracle + ClipHook."""
+    utils.soft_update on the update iterations, against the oracle with target_tau and grad_clip."""
     import utils
     kw = dict(obs=4, act=2, hidden=8, batch=3, burn_in=2, learning=3, n_step=2)
     prev = torch.get_default_dtype()
@@ -28,9 +22,8 @@ def test_oracle_matches_torch_clip_adam_soft_update(tau, interval, clip):
     try:
         port = ref_port.PortLearner(ref_port.PathConfig(**kw, target_interval=1 << 30), seed=4)
         sd = lambda m: {k: v.detach().numpy().copy() for k, v in m.state_dict().items()}  # noqa: E731
-        ol = PolyakOracle(sd(port.actor), sd(port.critic), burn_in=2, learning=3, n_step=2, target_interval=interval,
-                          target_tau=tau)
-        hook = ClipHook(clip)
+        ol = lo.OracleLearner(sd(port.actor), sd(port.critic), burn_in=2, learning=3, n_step=2,
+                              target_interval=interval, target_tau=tau, grad_clip=clip)
         torch_norms, clipped = {}, False
         for net, opt in (("critic", port.critic_opt), ("actor", port.actor_opt)):
             params = list(getattr(port, net).parameters())
@@ -45,10 +38,10 @@ def test_oracle_matches_torch_clip_adam_soft_update(tau, interval, clip):
             if (it + 1) % interval == 0:
                 utils.soft_update(port.target_actor, port.actor, tau)
                 utils.soft_update(port.target_critic, port.critic, tau)
-            ol.iteration(batch, grad_hook=hook)
+            ol.iteration(batch)
             for net in ("critic", "actor"):
-                assert abs(hook.norms[net] / torch_norms[net] - 1) < 1e-12, (it, net)
-                clipped |= 0 < clip < hook.norms[net]
+                assert abs(ol.norms[net] / torch_norms[net] - 1) < 1e-12, (it, net)
+                clipped |= 0 < clip < ol.norms[net]
         rel = lambda a, b: np.linalg.norm(a - b) / np.linalg.norm(b)  # noqa: E731
         for net in ("actor", "critic", "target_actor", "target_critic"):
             got, want = getattr(ol, net), sd(getattr(port, net))
@@ -76,17 +69,17 @@ def test_path_config_optimiser_values_are_validated():
 
 
 def test_dropin_optimiser_environment_variables(monkeypatch, tmp_path):
-    lr = _dropin_learner(monkeypatch, tmp_path, R2D2_TARGET_TAU="0.005", R2D2_TARGET_INTERVAL="1", R2D2_GRAD_CLIP="40")
+    lr = fake_engine_learner(monkeypatch, tmp_path, R2D2_TARGET_TAU="0.005", R2D2_TARGET_INTERVAL="1", R2D2_GRAD_CLIP="40")
     c = lr.engine.cfg
     assert (c.target_tau, c.target_interval, c.grad_clip_norm) == (0.005, 1, 40.0)
     for k in ("R2D2_TARGET_TAU", "R2D2_TARGET_INTERVAL", "R2D2_GRAD_CLIP"):
         monkeypatch.delenv(k)
-    c = _dropin_learner(monkeypatch, tmp_path).engine.cfg
+    c = fake_engine_learner(monkeypatch, tmp_path).engine.cfg
     assert (c.target_tau, c.target_interval, c.grad_clip_norm) == (1.0, 500, 0.0)
     for bad in (dict(R2D2_TARGET_TAU="0"), dict(R2D2_TARGET_TAU="2"), dict(R2D2_GRAD_CLIP="-1"),
                 dict(R2D2_TARGET_INTERVAL="0")):
         with pytest.raises(ValueError):
-            _dropin_learner(monkeypatch, tmp_path, **bad)
+            fake_engine_learner(monkeypatch, tmp_path, **bad)
         monkeypatch.delenv(next(iter(bad)))
 
 
@@ -94,36 +87,26 @@ NEW_KERNELS = ("adam_kernel", "grad_norm_kernel")
 
 
 def test_optimiser_kernels_do_not_spill():
-    nvcc = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.isfile("/usr/local/cuda/bin/nvcc") else None)
-    if not nvcc:
-        pytest.skip("nvcc unavailable")
-    res = subprocess.run([nvcc, "-O3", "-std=c++17", "-I", os.path.join(ROOT, "include"), "-gencode",
-                          "arch=compute_90a,code=sm_90a", "-Xptxas", "-v", "-c", os.path.join(CSRC, "elementwise.cu"),
-                          "-o", os.devnull], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-2000:]
+    report, stderr = ptxas_report("elementwise.cu")
     found = {k: 0 for k in NEW_KERNELS}
-    for m in re.finditer(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
-                         r"(\d+) bytes spill loads", res.stderr):
+    for m in report:
         for k in NEW_KERNELS:
             if k in m.group(1):
                 found[k] += 1
                 assert m.group(2) == m.group(3) == m.group(4) == "0", m.group(0)
-    assert found == {"adam_kernel": 4, "grad_norm_kernel": 1}, res.stderr[-2000:]
+    assert found == {"adam_kernel": 4, "grad_norm_kernel": 1}, stderr[-2000:]
 
 
 def test_optimiser_sass_has_no_local_memory():
-    from r2d2_b200 import native
-    sass = subprocess.run(["cuobjdump", "-sass", native.LIB_PATH], capture_output=True, text=True).stdout
-    if not sass:
-        pytest.skip("cuobjdump unavailable")
+    sass = library_sass()
     for k, want in (("adam_kernel", 4), ("grad_norm_kernel", 1)):
-        funcs = _functions(sass, k)
+        funcs = functions(sass, k)
         assert len(funcs) == want, sorted(funcs)
         for name, body in funcs.items():
-            ops = [op for op, _ in _ops(body)]
-            assert not [op for op in ops if op.startswith(("LDL", "STL"))], f"local-memory traffic in {name}"
+            body_ops = [op for op, _ in ops(body)]
+            assert not [op for op in body_ops if op.startswith(("LDL", "STL"))], f"local-memory traffic in {name}"
     # the fused Polyak update rounds like torch: FMUL, FMUL, FADD - the blend is never contracted into an FFMA
-    for name, body in _functions(sass, "adam_kernel").items():
+    for name, body in functions(sass, "adam_kernel").items():
         if "ILb0ELb1E" in name or "ILb1ELb1E" in name:
-            ops = [op for op, _ in _ops(body)]
-            assert ops.count("FADD") >= 1 and ops.count("FMUL") >= 2, name
+            body_ops = [op for op, _ in ops(body)]
+            assert body_ops.count("FADD") >= 1 and body_ops.count("FMUL") >= 2, name

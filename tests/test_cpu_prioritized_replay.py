@@ -1,14 +1,13 @@
 """Prioritized replay on the host side: PathConfig validation, the drop-in modules' environment switches, and the float64
-restatement of the importance-weighted TD gradient (tests/per_oracle.py) against a finite difference of its loss."""
-import os
+oracle's importance-weighted TD gradient against a finite difference of its loss."""
 import sys
 
 import numpy as np
 import pytest
 
+from learner_harness import fake_engine_learner
 from oracle import learner_oracle as lo
 from oracle import ref_port
-from per_oracle import weighted_iteration, weighted_td
 
 
 def test_path_config_exponents_are_validated():
@@ -22,49 +21,19 @@ def test_path_config_exponents_are_validated():
             engine.PathConfig(obs=3, act=1, **bad)
 
 
-class _FakeEngine:
-    def __init__(self, cfg, device=None):
-        self.cfg, self.device = cfg, device
-
-    def enable_data_parallel(self):
-        pass
-
-    def views(self, net):
-        return {}
-
-
-def _dropin_learner(monkeypatch, tmp_path, **env):
-    monkeypatch.setenv("R2D2_OBS_SIZE", "5")
-    monkeypatch.setenv("R2D2_N_ACTIONS", "2")
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    from r2d2_b200 import engine
-    monkeypatch.setattr(engine, "LearnerEngine", _FakeEngine)
-    monkeypatch.chdir(tmp_path)
-    os.makedirs("model_data", exist_ok=True)
-    for m in ("learner", "replay_memory"):
-        sys.modules.pop(m, None)
-    import learner as dropin_learner
-    try:
-        return dropin_learner.Learner(n_actors=1)
-    finally:
-        for m in ("learner", "replay_memory"):
-            sys.modules.pop(m, None)
-
-
 def test_dropin_environment_switches(monkeypatch, tmp_path):
-    lr = _dropin_learner(monkeypatch, tmp_path, R2D2_PRIORITY_EXPONENT="0.9", R2D2_IS_EXPONENT="0.6")
+    lr = fake_engine_learner(monkeypatch, tmp_path, R2D2_PRIORITY_EXPONENT="0.9", R2D2_IS_EXPONENT="0.6")
     assert lr.engine.cfg.priority_exponent == 0.9 and lr.engine.cfg.is_exponent == 0.6
     assert lr.memory.priority_exponent == 0.9 and lr.memory._cfg().priority_exponent == 0.9
     monkeypatch.delenv("R2D2_PRIORITY_EXPONENT")
     monkeypatch.delenv("R2D2_IS_EXPONENT")
-    lr = _dropin_learner(monkeypatch, tmp_path)
+    lr = fake_engine_learner(monkeypatch, tmp_path)
     assert (lr.engine.cfg.priority_exponent, lr.engine.cfg.is_exponent) == (1.0, 0.0)
     assert lr.memory._cfg().priority_exponent == 1.0
     with pytest.raises(ValueError):
-        _dropin_learner(monkeypatch, tmp_path, R2D2_PRIORITY_EXPONENT="2")
+        fake_engine_learner(monkeypatch, tmp_path, R2D2_PRIORITY_EXPONENT="2")
     with pytest.raises(ValueError):
-        _dropin_learner(monkeypatch, tmp_path, R2D2_IS_EXPONENT="-0.5")
+        fake_engine_learner(monkeypatch, tmp_path, R2D2_IS_EXPONENT="-0.5")
 
 
 def test_replay_memory_exponent_argument_and_environment(monkeypatch):
@@ -87,9 +56,9 @@ def test_weighted_td_gradient_matches_finite_difference():
     q, q_next = rng.standard_normal((L, B, A)), rng.standard_normal((L, B, A))
     rew, term = rng.standard_normal((T, B)), (rng.uniform(size=(T, B)) < 0.2).astype(np.float64)
     w = rng.uniform(0.1, 1.0, B)
-    td = weighted_td(w)
     kw = dict(burn_in=Bn, learning=L, n_step=n, gamma=0.997)
-    _, loss, dq, td_sq, prio = td(q, q_next, rew, term, **kw)
+    td = lambda *a: lo.td_targets_and_priorities(*a, **kw, is_weight=w)  # noqa: E731
+    _, loss, dq, td_sq, prio = td(q, q_next, rew, term)
     _, loss0, dq0, td_sq0, prio0 = lo.td_targets_and_priorities(q, q_next, rew, term, **kw)
     assert np.array_equal(td_sq, td_sq0) and np.array_equal(prio, prio0)      # unweighted by definition
     assert abs(loss - np.sum(w[None, :] * td_sq0) / (L * B)) < 1e-12
@@ -99,10 +68,10 @@ def test_weighted_td_gradient_matches_finite_difference():
         qp, qm = q.copy(), q.copy()
         qp[idx] += eps
         qm[idx] -= eps
-        fd[idx] = (td(qp, q_next, rew, term, **kw)[1] - td(qm, q_next, rew, term, **kw)[1]) / (2 * eps)
+        fd[idx] = (td(qp, q_next, rew, term)[1] - td(qm, q_next, rew, term)[1]) / (2 * eps)
     assert np.abs(fd - dq).max() < 1e-8 * max(1.0, np.abs(dq).max())
     # unit weights are the unweighted loss
-    _, loss1, dq1, _, _ = weighted_td(np.ones(B))(q, q_next, rew, term, **kw)
+    _, loss1, dq1, _, _ = lo.td_targets_and_priorities(q, q_next, rew, term, **kw, is_weight=np.ones(B))
     assert abs(loss1 - loss0) < 1e-14 and np.allclose(dq1, dq0, rtol=1e-14, atol=0)
 
 
@@ -113,8 +82,7 @@ def test_weighted_iteration_restores_the_unweighted_oracle():
     batch = ref_port.synthetic_batch(pc, seed=2)
     a = lo.OracleLearner(sd(port.actor), sd(port.critic), burn_in=2, learning=3, n_step=2)
     b = lo.OracleLearner(sd(port.actor), sd(port.critic), burn_in=2, learning=3, n_step=2)
-    ow = weighted_iteration(a, batch, np.full(3, 0.5))
-    assert lo.td_targets_and_priorities is not None and lo.td_targets_and_priorities.__name__ == "td_targets_and_priorities"
+    ow = a.iteration(dict(batch, is_weight=np.full(3, 0.5)))
     o1 = b.iteration(batch)
     assert abs(ow["critic_loss"] - 0.5 * o1["critic_loss"]) < 1e-12
     for k in lo.PARAM_KEYS:

@@ -3,26 +3,15 @@ step ahead, not through loads that the pointwise phase waits on.  In the SASS of
 cfg-3 instantiation), from the step loop's first mbarrier wait on, the only global loads are LDGSTS (the stage copies)
 and the LDG.E.STRONG.SYS status read of the bounded wait's slow path."""
 import re
-import subprocess
 
-import pytest
+from sass_report import functions, library_sass
 
 KERNEL = "lstm_scan_bwd_kernelILi512ELi16E"
 
 
-def _function_sass(sass, key):
-    for block in re.split(r"\n\s*Function : ", sass)[1:]:
-        if key in block.split("\n", 1)[0]:
-            return block
-    return None
-
-
 def test_bwd_scan_step_loop_has_no_blocking_global_loads():
     from r2d2_b200 import native
-    sass = subprocess.run(["cuobjdump", "-sass", native.LIB_PATH], capture_output=True, text=True).stdout
-    if not sass:
-        pytest.skip("cuobjdump unavailable")
-    body = _function_sass(sass, KERNEL)
+    body = next(iter(functions(library_sass(), KERNEL).values()), None)
     assert body is not None, f"{KERNEL} not found in {native.LIB_PATH}"
     ops = [m.group(1) for m in re.finditer(r"/\*[0-9a-f]{4,}\*/\s*(?:@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)", body)]
     first_wait = next((i for i, op in enumerate(ops) if op.startswith("SYNCS.PHASECHK")), None)

@@ -1,23 +1,19 @@
-"""TD3's target on the host side: the oracle's Philox against Random123's known answers, the TD3 oracle against the plain
-learner oracle (twin off, no noise) and against a torch-autograd float64 restatement on oracle/ref_port.py's nets (twin,
-smoothing, Polyak targets, joint clipping), validation of PathConfig / the environment variables / checkpoints, and the
-compiler's report on the new kernels (present, no spills, no local memory)."""
+"""TD3's target on the host side: the oracle's Philox against Random123's known answers, the float64 oracle with the
+twin against a torch-autograd float64 restatement on oracle/ref_port.py's nets (twin, smoothing, Polyak targets, joint
+clipping), validation of PathConfig / the environment variables / checkpoints, and the compiler's report on the new
+kernels (present, no spills, no local memory)."""
 import copy
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-import td3_oracle as t3
 from conftest import rel_l2
+from learner_harness import fake_engine_learner
 from oracle import learner_oracle as lo
 from oracle import ref_port
-from test_cpu_prioritized_replay import _dropin_learner
-from test_cpu_sass_gemm import CSRC, ROOT, _functions, _ops
+from oracle import target_noise as tn
+from sass_report import functions, library_sass, ops, ptxas_report
 
 SMALL = dict(obs=5, act=2, hidden=16, batch=4, burn_in=3, learning=5, n_step=2)
 
@@ -31,52 +27,33 @@ KAT = [((0, 0, 0, 0), (0, 0), (0x6627e8d5, 0xe169c58d, 0xbc57ac4c, 0x9b00dbd8)),
 
 @pytest.mark.parametrize("ctr,key,want", KAT)
 def test_philox_known_answers(ctr, key, want):
-    assert tuple(int(x) for x in t3.philox4x32_10(ctr, key)) == want
+    assert tuple(int(x) for x in tn.philox4x32_10(ctr, key)) == want
 
 
 def test_noise_layout_and_range():
     """Four elements share one Philox block; u is an odd multiple of 2^-24 inside (0, 1); (seed, rank, iter) all key."""
-    z = t3.normal(4096, 7, 0, 3)
-    x = t3.philox4x32_10((np.uint64(1), np.uint64(3), np.uint64(0), np.uint64(0)), (np.uint64(7), np.uint64(0)))
-    u = t3.unit_open(np.asarray(x))
+    z = tn.normal(4096, 7, 0, 3)
+    x = tn.philox4x32_10((np.uint64(1), np.uint64(3), np.uint64(0), np.uint64(0)), (np.uint64(7), np.uint64(0)))
+    u = tn.unit_open(np.asarray(x))
     r01, r23 = np.sqrt(-2 * np.log(u[0])), np.sqrt(-2 * np.log(u[2]))
     assert np.allclose(z[4:8], [r01 * np.cos(2 * np.pi * u[1]), r01 * np.sin(2 * np.pi * u[1]),
                                 r23 * np.cos(2 * np.pi * u[3]), r23 * np.sin(2 * np.pi * u[3])], rtol=0, atol=0)
-    assert t3.unit_open(np.uint32(0)) == 2.0 ** -24 and t3.unit_open(np.uint32(0xffffffff)) == 1 - 2.0 ** -24
-    for other in (t3.normal(4096, 8, 0, 3), t3.normal(4096, 7, 1, 3), t3.normal(4096, 7, 0, 4),
-                  t3.normal(4096, 7, 0, 3 + 2 ** 32)):
+    assert tn.unit_open(np.uint32(0)) == 2.0 ** -24 and tn.unit_open(np.uint32(0xffffffff)) == 1 - 2.0 ** -24
+    for other in (tn.normal(4096, 8, 0, 3), tn.normal(4096, 7, 1, 3), tn.normal(4096, 7, 0, 4),
+                  tn.normal(4096, 7, 0, 3 + 2 ** 32)):
         assert not np.any(other == z)
-    a = t3.smooth(np.full(4096, 0.9), 1.0, 0.3, 7, 0, 3)
+    a = tn.smooth(np.full(4096, 0.9), 1.0, 0.3, 7, 0, 3)
     low = 0.9 - 0.3                                    # the c clip binds below, the [-1, 1] clamp above
     assert a.max() == 1.0 and a.min() == low and np.any(a == low) and np.any((a > low) & (a < 1.0))
 
 
-# ------------------------------------------------------------------------------------------------ 2. oracle vs base
+# ------------------------------------------------------------------------------------------------ 2. nets
 def _port_params(seed=1, cfg=None):
     pc = ref_port.PathConfig(**(cfg or SMALL))
     port = ref_port.PortLearner(pc, seed=seed)
     sd = lambda m: {k: v.detach().numpy().astype(np.float64) for k, v in m.state_dict().items()}  # noqa: E731
     c2 = ref_port.PortCriticNet(pc.obs, pc.act, 0, pc.hidden)
     return pc, sd(port.actor), sd(port.critic), sd(c2)
-
-
-def test_twin_off_without_noise_is_the_plain_oracle():
-    pc, a, c, _ = _port_params()
-    kw = dict(burn_in=pc.burn_in, learning=pc.learning, n_step=pc.n_step, target_interval=2)
-    base, mine = lo.OracleLearner(a, c, **kw), t3.TD3Oracle(a, c, **kw)
-    for it in range(3):
-        batch = ref_port.synthetic_batch(pc, seed=it)
-        x, y = base.iteration(batch), mine.iteration(batch)
-        for k in ("critic_loss", "actor_loss"):
-            assert x[k] == y[k], k
-        for k in ("priority", "average_td_loss", "q_value", "target_q_value", "act_next", "q_next"):
-            assert np.array_equal(x[k], y[k]), k
-        for net in ("critic_grad", "actor_grad"):
-            for k in lo.PARAM_KEYS:
-                assert np.array_equal(x[net][k], y[net][k]), (net, k)
-    for net in ("actor", "critic", "target_actor", "target_critic"):
-        for k in lo.PARAM_KEYS:
-            assert np.array_equal(getattr(base, net)[k], getattr(mine, net)[k]), (net, k)
 
 
 # ------------------------------------------------------------------------------------------------ 3. vs autograd
@@ -102,7 +79,7 @@ def _autograd_run(pc, actor, critic, critic2, batches, *, sigma, clip_c, seed, t
                 TA.set_state(t["ta_state"][0], t["ta_state"][1])
                 a_next = torch.stack([TA(obs[k]) for k in range(Bn + n + L)][Bn + n:])
                 if sigma > 0:
-                    z = torch.as_tensor(t3.normal(a_next.numel(), seed, 0, it).reshape(a_next.shape))
+                    z = torch.as_tensor(tn.normal(a_next.numel(), seed, 0, it).reshape(a_next.shape))
                     a_next = torch.clamp(a_next + torch.clamp(sigma * z, -clip_c, clip_c), -1.0, 1.0)
                 acts = torch.cat((act[:Bn + n], a_next), 0)
                 TC1.set_state(t["tc_state"][0], t["tc_state"][1])
@@ -154,12 +131,13 @@ def _load(net, sd):
 def test_oracle_matches_torch_autograd(sigma, clip_c):
     pc, a, c, c2 = _port_params(seed=4)
     batches = [ref_port.synthetic_batch(pc, seed=10 + i) for i in range(4)]
-    probe = t3.TD3Oracle(a, c, critic2=c2, twin=True, burn_in=pc.burn_in, learning=pc.learning, n_step=pc.n_step,
-                         grad_clip=1e30)
+    probe = lo.OracleLearner(a, c, critic2=c2, twin=True, burn_in=pc.burn_in, learning=pc.learning, n_step=pc.n_step,
+                             grad_clip=1e30)
     probe.iteration(batches[0])
     max_norm = 0.1 * min(probe.norms.values())             # both clip from the first iteration on
-    ol = t3.TD3Oracle(a, c, critic2=c2, twin=True, sigma=sigma, noise_clip=clip_c, seed=3, target_tau=0.05,
-                      grad_clip=max_norm, burn_in=pc.burn_in, learning=pc.learning, n_step=pc.n_step, target_interval=1)
+    ol = lo.OracleLearner(a, c, critic2=c2, twin=True, target_noise=sigma, target_noise_clip=clip_c, target_noise_seed=3,
+                          target_tau=0.05, grad_clip=max_norm, burn_in=pc.burn_in, learning=pc.learning,
+                          n_step=pc.n_step, target_interval=1)
     for b in batches:
         ol.iteration(b)
     want = _autograd_run(pc, a, c, c2, batches, sigma=sigma, clip_c=clip_c, seed=3, tau=0.05, interval=1,
@@ -171,8 +149,8 @@ def test_oracle_matches_torch_autograd(sigma, clip_c):
         errs[f"m/critic2/{k}"] = rel_l2(ol.critic2_adam["m/" + k], want["m_critic2"][i])
     assert max(errs.values()) < 1e-10, {k: v for k, v in errs.items() if v >= 1e-10}
     # the options visibly matter: the same run without the twin's minimum or without noise ends elsewhere
-    plain = t3.TD3Oracle(a, c, critic2=c2, twin=True, target_tau=0.05, grad_clip=max_norm, burn_in=pc.burn_in,
-                         learning=pc.learning, n_step=pc.n_step, target_interval=1)
+    plain = lo.OracleLearner(a, c, critic2=c2, twin=True, target_tau=0.05, grad_clip=max_norm, burn_in=pc.burn_in,
+                             learning=pc.learning, n_step=pc.n_step, target_interval=1)
     for b in batches:
         plain.iteration(b)
     assert rel_l2(plain.critic["l3.weight"], ol.critic["l3.weight"]) > 1e-6
@@ -211,15 +189,15 @@ def test_td3_environment():
 
 
 def test_dropin_learner_reads_td3_options(monkeypatch, tmp_path):
-    c = _dropin_learner(monkeypatch, tmp_path, R2D2_TWIN_CRITIC="1", R2D2_TARGET_NOISE="0.2",
+    c = fake_engine_learner(monkeypatch, tmp_path, R2D2_TWIN_CRITIC="1", R2D2_TARGET_NOISE="0.2",
                         R2D2_TARGET_NOISE_CLIP="0.5", R2D2_TARGET_NOISE_SEED="4").engine.cfg
     assert (c.twin_critic, c.target_noise, c.target_noise_clip, c.target_noise_seed) == (True, 0.2, 0.5, 4)
     for k in ("R2D2_TWIN_CRITIC", "R2D2_TARGET_NOISE", "R2D2_TARGET_NOISE_CLIP", "R2D2_TARGET_NOISE_SEED"):
         monkeypatch.delenv(k)
-    c = _dropin_learner(monkeypatch, tmp_path).engine.cfg
+    c = fake_engine_learner(monkeypatch, tmp_path).engine.cfg
     assert (c.twin_critic, c.target_noise) == (False, 0.0)
     with pytest.raises(ValueError, match="0, 1"):
-        _dropin_learner(monkeypatch, tmp_path, R2D2_TWIN_CRITIC="2")
+        fake_engine_learner(monkeypatch, tmp_path, R2D2_TWIN_CRITIC="2")
 
 
 def test_checkpoint_twin_mismatch_is_refused():
@@ -238,33 +216,23 @@ TD3_KERNELS = ("target_smoothing_kernel", "q_min_kernel")
 
 
 def test_td3_kernels_do_not_spill():
-    nvcc = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.isfile("/usr/local/cuda/bin/nvcc") else None)
-    if not nvcc:
-        pytest.skip("nvcc unavailable")
-    res = subprocess.run([nvcc, "-O3", "-std=c++17", "-I", os.path.join(ROOT, "include"), "-gencode",
-                          "arch=compute_90a,code=sm_90a", "-Xptxas", "-v", "-c", os.path.join(CSRC, "td3.cu"),
-                          "-o", os.devnull], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-2000:]
+    report, stderr = ptxas_report("td3.cu")
     found = dict.fromkeys(TD3_KERNELS, 0)
-    for m in re.finditer(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
-                         r"(\d+) bytes spill loads", res.stderr):
+    for m in report:
         for k in TD3_KERNELS:
             if k in m.group(1):
                 found[k] += 1
                 assert m.group(2) == m.group(3) == m.group(4) == "0", m.group(0)
-    assert found == dict.fromkeys(TD3_KERNELS, 1), res.stderr[-2000:]
+    assert found == dict.fromkeys(TD3_KERNELS, 1), stderr[-2000:]
 
 
 def test_td3_sass_present_without_local_memory():
-    from r2d2_b200 import native
-    sass = subprocess.run(["cuobjdump", "-sass", native.LIB_PATH], capture_output=True, text=True).stdout
-    if not sass:
-        pytest.skip("cuobjdump unavailable")
+    sass = library_sass()
     for k in TD3_KERNELS:
-        funcs = _functions(sass, k)
+        funcs = functions(sass, k)
         assert len(funcs) == 1, (k, sorted(funcs))
         for name, body in funcs.items():
-            ops = [op for op, _ in _ops(body)]
-            assert not [op for op in ops if op.startswith(("LDL", "STL"))], f"local-memory traffic in {name}"
+            body_ops = [op for op, _ in ops(body)]
+            assert not [op for op in body_ops if op.startswith(("LDL", "STL"))], f"local-memory traffic in {name}"
             if k == "target_smoothing_kernel":   # the precise functions, not the fast-math approximations alone
-                assert "IMAD.HI.U32" in ops or any(op.startswith("IMAD.WIDE.U32") for op in ops), name
+                assert "IMAD.HI.U32" in body_ops or any(op.startswith("IMAD.WIDE.U32") for op in body_ops), name

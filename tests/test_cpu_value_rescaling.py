@@ -4,19 +4,17 @@ against the float64 actor oracle, validation of PathConfig / the environment var
 report on every TD and actor-priority kernel instantiation (all present, no spills, no local memory)."""
 import decimal
 import itertools
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-import rescale_oracle as ro
 from conftest import rel_l2
-from test_cpu_prioritized_replay import _dropin_learner
-from test_cpu_sass_gemm import CSRC, ROOT, _functions, _ops
+from learner_harness import fake_engine_learner
+from oracle import actor_oracle
+from oracle import learner_oracle as lo
+from sass_report import functions, library_sass, ops, ptxas_report
 
 EPS = (0.0, 1e-3, 1e-2)
 MODES = [(r, m) for r in ("reference", "invertible") for m in ("squared", "abs")]
@@ -60,11 +58,11 @@ def test_oracle_matches_decimal(eps):
     e64 = float(np.float64(eps))   # the decimal side sees the same binary eps
     worst = {"h": 0.0, "h_inv": 0.0, "round_trip": 0.0}
     for x in _inputs():
-        worst["h"] = max(worst["h"], _rel(float(ro.h(x, e64)), _dec_h(x, e64)))
-        worst["h_inv"] = max(worst["h_inv"], _rel(float(ro.h_inv(x, e64)), _dec_h_inv(x, e64)))
-        worst["round_trip"] = max(worst["round_trip"], _rel(float(ro.h(ro.h_inv(x, e64), e64)), x))
+        worst["h"] = max(worst["h"], _rel(float(lo.h_eps(x, e64)), _dec_h(x, e64)))
+        worst["h_inv"] = max(worst["h_inv"], _rel(float(lo.h_eps_inv(x, e64)), _dec_h_inv(x, e64)))
+        worst["round_trip"] = max(worst["round_trip"], _rel(float(lo.h_eps(lo.h_eps_inv(x, e64), e64)), x))
     assert max(worst.values()) < 1e-14, worst
-    assert ro.h(0.0, eps) == 0.0 and ro.h_inv(0.0, eps) == 0.0
+    assert lo.h_eps(0.0, eps) == 0.0 and lo.h_eps_inv(0.0, eps) == 0.0
 
 
 # ------------------------------------------------------------------------------------------------ 2. float32 utils
@@ -74,8 +72,8 @@ def test_float32_utils_match_oracle(eps):
     x32 = _inputs().astype(np.float32)
     x = torch.from_numpy(x32)
     e = float(np.float32(eps))     # torch applies the python scalar in float32
-    for name, got, want in (("h", utils.value_rescale(x, eps).numpy(), ro.h(x32.astype(np.float64), e)),
-                            ("h_inv", utils.inverse_value_rescale(x, eps).numpy(), ro.h_inv(x32.astype(np.float64), e))):
+    for name, got, want in (("h", utils.value_rescale(x, eps).numpy(), lo.h_eps(x32.astype(np.float64), e)),
+                            ("h_inv", utils.inverse_value_rescale(x, eps).numpy(), lo.h_eps_inv(x32.astype(np.float64), e))):
         assert got.dtype == np.float32
         err = np.abs(got - want) / np.maximum(np.abs(want), 1e-300)
         err[want == 0] = np.abs(got[want == 0])
@@ -125,13 +123,13 @@ def test_actor_calc_priorities_match_oracle(monkeypatch, tmp_path, rescaling, me
     a.calc_priorities()
     rew = np.asarray([row[2][0] for row in a.sequence])
     sd = lambda m: {k: v.numpy() for k, v in m.state_dict().items()}  # noqa: E731
-    want = ro.episode_priorities(sd(a.critic), sd(a.target_actor), sd(a.target_critic), obs, act, rew, term,
+    want = actor_oracle.episode_priorities(sd(a.critic), sd(a.target_actor), sd(a.target_critic), obs, act, rew, term,
                                  burn_in=a.burn_in_length, learning=a.learning_length, n_step=n, gamma=a.gamma,
                                  rescaling=rescaling, eps=eps, metric=metric)
     got = np.asarray(a.priority, np.float64)
     assert got.shape == want.shape == (E - 60,)
     assert rel_l2(got, want) < 1e-4, rel_l2(got, want)
-    other = ro.episode_priorities(sd(a.critic), sd(a.target_actor), sd(a.target_critic), obs, act, rew, term,
+    other = actor_oracle.episode_priorities(sd(a.critic), sd(a.target_actor), sd(a.target_critic), obs, act, rew, term,
                                   burn_in=a.burn_in_length, learning=a.learning_length, n_step=n, gamma=a.gamma,
                                   rescaling="reference" if rescaling == "invertible" else "invertible", eps=0.01,
                                   metric=metric)
@@ -172,16 +170,16 @@ def test_path_config_td_options_are_validated():
 
 
 def test_dropin_learner_reads_td_options(monkeypatch, tmp_path):
-    c = _dropin_learner(monkeypatch, tmp_path, R2D2_VALUE_RESCALING="invertible", R2D2_RESCALING_EPS="0.002",
+    c = fake_engine_learner(monkeypatch, tmp_path, R2D2_VALUE_RESCALING="invertible", R2D2_RESCALING_EPS="0.002",
                         R2D2_PRIORITY_METRIC="abs").engine.cfg
     assert (c.value_rescaling, c.rescaling_eps, c.priority_metric) == ("invertible", 0.002, "abs")
     for k in ("R2D2_VALUE_RESCALING", "R2D2_RESCALING_EPS", "R2D2_PRIORITY_METRIC"):
         monkeypatch.delenv(k)
-    c = _dropin_learner(monkeypatch, tmp_path).engine.cfg
+    c = fake_engine_learner(monkeypatch, tmp_path).engine.cfg
     assert (c.value_rescaling, c.rescaling_eps, c.priority_metric) == ("reference", 1e-3, "squared")
     for bad in (dict(R2D2_VALUE_RESCALING="inverse"), dict(R2D2_PRIORITY_METRIC="l1"), dict(R2D2_RESCALING_EPS="-1")):
         with pytest.raises(ValueError):
-            _dropin_learner(monkeypatch, tmp_path, **bad)
+            fake_engine_learner(monkeypatch, tmp_path, **bad)
         monkeypatch.delenv(next(iter(bad)))
 
 
@@ -232,35 +230,25 @@ def _default_actor_kernel(name):
 
 
 def test_td_kernels_do_not_spill():
-    nvcc = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.isfile("/usr/local/cuda/bin/nvcc") else None)
-    if not nvcc:
-        pytest.skip("nvcc unavailable")
-    res = subprocess.run([nvcc, "-O3", "-std=c++17", "-I", os.path.join(ROOT, "include"), "-gencode",
-                          "arch=compute_90a,code=sm_90a", "-Xptxas", "-v", "-c", os.path.join(CSRC, "elementwise.cu"),
-                          "-o", os.devnull], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[-2000:]
+    report, stderr = ptxas_report("elementwise.cu")
     found = {k: 0 for k in TD_KERNELS}
-    for m in re.finditer(r"Function properties for (\S+)\n\s*(\d+) bytes stack frame, (\d+) bytes spill stores, "
-                         r"(\d+) bytes spill loads", res.stderr):
+    for m in report:
         for k in TD_KERNELS:
             if k in m.group(1):
                 found[k] += 1
                 if not _default_actor_kernel(m.group(1)):
                     assert m.group(2) == m.group(3) == m.group(4) == "0", m.group(0)
-    assert found == TD_KERNELS, res.stderr[-2000:]
+    assert found == TD_KERNELS, stderr[-2000:]
 
 
 def test_td_sass_has_every_instantiation_and_no_local_memory():
-    from r2d2_b200 import native
-    sass = subprocess.run(["cuobjdump", "-sass", native.LIB_PATH], capture_output=True, text=True).stdout
-    if not sass:
-        pytest.skip("cuobjdump unavailable")
+    sass = library_sass()
     for k, want in TD_KERNELS.items():
-        funcs = _functions(sass, k)
+        funcs = functions(sass, k)
         flags = sorted("".join(re.findall(r"Lb([01])E", n)) for n in funcs)      # template flags, in order
         width = 1 if want == 2 else 2
         assert flags == ["".join(f) for f in itertools.product("01", repeat=width)], (k, sorted(funcs))
         for name, body in funcs.items():
-            ops = [op for op, _ in _ops(body)]
+            body_ops = [op for op, _ in ops(body)]
             if not _default_actor_kernel(name):
-                assert not [op for op in ops if op.startswith(("LDL", "STL"))], f"local-memory traffic in {name}"
+                assert not [op for op in body_ops if op.startswith(("LDL", "STL"))], f"local-memory traffic in {name}"

@@ -6,7 +6,7 @@ float64 references and the CPU port of the reference at A = 8 .. 64 (dm_control'
    importance weights;
  * the learner's A-dependent GEMMs through r2d2_gemm_f32 in the default mode, built the way net.cu builds them (layout,
    leading dimensions, pointer offsets into W1, epilogues), on both sides of every thin-kernel bucket;
- * learner iterations against oracle/ref_port.py, one importance-weighted iteration against tests/per_oracle.py;
+ * learner iterations against oracle/ref_port.py, one importance-weighted iteration against oracle/learner_oracle.py;
  * the replay gather, the actor-side priorities and r2d2_policy_step at wide A.
 
 A relative L2 norm over a whole tensor dilutes an error confined to one action column by about sqrt(A), so every output
@@ -21,11 +21,11 @@ import pytest
 import torch
 
 from conftest import rel_l2
+from learner_harness import col_err, oracle_for
 from oracle import actor_oracle
 from oracle import learner_oracle as lo
 from oracle import ref_port
 from oracle.sumtree import SumTreeOracle
-from per_oracle import weighted_iteration, weighted_td
 
 pytestmark = pytest.mark.gpu
 
@@ -61,15 +61,6 @@ def report():
     print("routes seen:")
     for case, names in SEEN.items():
         print(f"  {case}: {names}")
-
-
-def col_err(x, ref, A):
-    """max over action columns j of ||x_j - ref_j|| / (||ref|| / sqrt(A)); both reshaped to [-1, A].  Normalised by the
-    RMS column norm, so a column whose reference is near zero does not blow the ratio up."""
-    x = np.asarray(x, np.float64).reshape(-1, A)
-    ref = np.asarray(ref, np.float64).reshape(-1, A)
-    rms_col = np.linalg.norm(ref) / np.sqrt(A)
-    return float(np.linalg.norm(x - ref, axis=0).max() / max(rms_col, 1e-30))
 
 
 def check(group, name, x, ref, tol, A=None):
@@ -240,7 +231,8 @@ def test_td_priority_weighted_wide(nv, A):
     B, L, n, Bn = 33, 33, 5, 3
     inputs = td_inputs(L, B, A, Bn, n, seed=A)
     w = np.random.default_rng(A + 1).uniform(0.05, 1.0, B).astype(np.float32)
-    ref = weighted_td(f64(w))(*(f64(x) for x in inputs), burn_in=Bn, learning=L, n_step=n, gamma=0.997)
+    ref = lo.td_targets_and_priorities(*(f64(x) for x in inputs), burn_in=Bn, learning=L, n_step=n, gamma=0.997,
+                                       is_weight=f64(w))
     o = run_routed(f"td weighted A={A}", "td_column", lambda: td_call(nv, inputs, L, B, A, Bn, n, w=w))
     check_td("td_weighted", o, ref, A)
     plain = td_call(nv, inputs, L, B, A, Bn, n)
@@ -446,7 +438,8 @@ def test_weighted_learner_iteration_column_kernel(eng_mod):
     actor, critic = sd(port.actor), sd(port.critic)
     batch = ref_port.synthetic_batch(pc, seed=7)
     w = np.random.default_rng(29).uniform(0.05, 1.0, kw["batch"]).astype(np.float32)
-    eng = eng_mod.LearnerEngine(eng_mod.PathConfig(**kw, is_exponent=0.6))
+    cfg = eng_mod.PathConfig(**kw, is_exponent=0.6)
+    eng = eng_mod.LearnerEngine(cfg)
     eng.load_state_dicts(actor, critic)
     eng.set_batch(dict(batch, is_weight=w))
     eng.step()
@@ -456,8 +449,7 @@ def test_weighted_learner_iteration_column_kernel(eng_mod):
     plain.step()
     torch.cuda.synchronize()
     assert torch.equal(eng.td_sq, plain.td_sq) and torch.equal(eng.priority, plain.priority)
-    ol = lo.OracleLearner(actor, critic, burn_in=kw["burn_in"], learning=kw["learning"], n_step=kw["n_step"])
-    ref = weighted_iteration(ol, batch, w)
+    ref = oracle_for(cfg, actor, critic).iteration(dict(batch, is_weight=w))
     bad = check_learner("learner_weighted", eng, eng_mod, ref, kw["obs"], kw["act"])
     assert not bad, bad
     eng.close()

@@ -13,11 +13,10 @@ import numpy as np
 import pytest
 import torch
 
-import rescale_oracle as ro
 from conftest import rel_l2
+from learner_harness import oracle_for
 from oracle import learner_oracle as lo
 from oracle import ref_port
-from optim_oracle import ClipHook, PolyakOracle
 from peer_harness import PeerGroup, split_batch
 
 pytestmark = pytest.mark.gpu
@@ -65,7 +64,7 @@ def state(eng):
     return out
 
 
-def assert_same_bits(a, b, what):
+def assert_same_state(a, b, what):
     assert a.keys() == b.keys()
     for k in a:
         assert np.array_equal(u32(a[k]), u32(b[k])), f"{what}: {k} differs"
@@ -190,7 +189,7 @@ def test_two_ranks_on_identical_shards_are_one_engine_bit_for_bit(E, option, pre
                 norms = np.asarray([got["critic_norm"], got["actor_norm"]], np.float32)
                 assert np.array_equal(u32(norms), u32(want["grad_norms"])), f"it {it} rank {r}: grad_norms"
         for r in range(2):
-            assert_same_bits(rec[r][ITERS - 1]["state"], single_state, f"rank {r} final state")
+            assert_same_state(rec[r][ITERS - 1]["state"], single_state, f"rank {r} final state")
     finally:
         g.close()
 
@@ -198,18 +197,6 @@ def test_two_ranks_on_identical_shards_are_one_engine_bit_for_bit(E, option, pre
 # ------------------------------------------------------------------------------------------------ (c) float64 parity
 GLOBAL = dict(SMALL, batch=12)
 _ORACLE = {}
-
-
-class _RawGradHook(ClipHook):
-    """ClipHook that also keeps each net's gradient before clipping, flattened in the engine's parameter order."""
-
-    def __init__(self, max_norm):
-        super().__init__(max_norm)
-        self.raw = {}
-
-    def __call__(self, net, grads):
-        self.raw[net] = np.concatenate([np.asarray(grads[k], np.float64).ravel() for k in lo.PARAM_KEYS])
-        super().__call__(net, grads)
 
 
 def _oracle(E, option):
@@ -222,18 +209,15 @@ def _oracle(E, option):
     actor = {k: v.numpy() for k, v in E.init_reference_params(cfg, False, gen).items()}
     critic = {k: v.numpy() for k, v in E.init_reference_params(cfg, True, gen).items()}
     batches = global_batches(GLOBAL, ITERS + 1, seed=90, weights=weights)
-    ol = PolyakOracle(actor, critic, burn_in=cfg.burn_in, learning=cfg.learning, n_step=cfg.n_step,
-                      target_interval=cfg.target_interval, target_tau=float(np.float32(cfg.target_tau)))
+    ol = oracle_for(cfg, actor, critic)
+    flat = lambda g: np.concatenate([np.asarray(g[k], np.float64).ravel() for k in lo.PARAM_KEYS])  # noqa: E731
     per_it = []
     for it in range(ITERS):
-        b = batches[it]
-        hook = _RawGradHook(cfg.grad_clip_norm)
-        w = None if not weights else np.asarray(b["is_weight"], np.float64)
-        ref = ro.iteration(ol, b, cfg.value_rescaling, float(np.float32(cfg.rescaling_eps)), cfg.priority_metric, w,
-                           grad_hook=hook)
+        ref = ol.iteration(batches[it])
         per_it.append(dict(q_value=ref["q_value"], target_q_value=ref["target_q_value"], td_sq=ref["average_td_loss"],
-                           losses=(ref["critic_loss"], ref["actor_loss"]), critic_grad=hook.raw["critic"],
-                           actor_grad=hook.raw["actor"], norms=(hook.norms["critic"], hook.norms["actor"])))
+                           losses=(ref["critic_loss"], ref["actor_loss"]),
+                           critic_grad=flat(ref["pre_clip_grad"]["critic"]), actor_grad=flat(ref["pre_clip_grad"]["actor"]),
+                           norms=(ol.norms["critic"], ol.norms["actor"])))
     final = {}
     for net in ("actor", "critic"):
         final["flat." + net] = getattr(ol, net)
@@ -275,7 +259,7 @@ def test_disjoint_shards_against_float64(E, W, option, prefetch):
     def replicas(it):
         s0 = state(g.engines[0])
         for r in range(1, W):
-            assert_same_bits(state(g.engines[r]), s0, f"it {it} rank {r} vs rank 0")
+            assert_same_state(state(g.engines[r]), s0, f"it {it} rank {r} vs rank 0")
 
     def on_iteration(it):
         o = ref[it]
@@ -345,7 +329,7 @@ def test_attach_rejects_bad_arguments_and_the_learner_still_steps(E):
         e.step()
         e.step()
     torch.cuda.synchronize()
-    assert_same_bits(state(eng), state(plain), "after refused attaches")
+    assert_same_state(state(eng), state(plain), "after refused attaches")
     assert not any(b.any() for b in bufs), "a refused attach wrote into a peer buffer"
     eng.close()
     plain.close()

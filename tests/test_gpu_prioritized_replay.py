@@ -1,40 +1,25 @@
 """Prioritized replay on the GPU: the priority exponent alpha on the sum-tree leaves, the importance-sampling weights
 of the weighted draw, the weighted critic loss of the learner, and that the defaults (alpha = 1, beta = 0) are the
 unweighted library bit for bit."""
-import os
-import tempfile
 from collections import deque
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import golden_batch, golden_params, load_golden, rel_l2
+from conftest import rel_l2
+from learner_harness import (REPLAY, SMALL, TOL, assert_two_gpu_replicas_stay_identical, episode, golden_case, oracle_for,
+                             port_case, replay_fed_run, trained_dropin_learner)
 from oracle import learner_oracle as lo
-from oracle import ref_port
 from oracle.sumtree import SumTreeOracle
-from per_oracle import weighted_iteration, weighted_td
 
 pytestmark = pytest.mark.gpu
-
-TOL = 1e-3
 
 
 @pytest.fixture(scope="module")
 def eng_mod():
     from r2d2_b200 import engine
     return engine
-
-
-def episode(rng, cfg, E, p_lo=0.01):
-    n_rows = E + cfg.n_step
-    term = np.zeros(n_rows, np.float32)
-    term[E:] = 1
-    return (rng.standard_normal((n_rows, cfg.obs)).astype(np.float32),
-            rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32),
-            rng.standard_normal(n_rows).astype(np.float32), term,
-            (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32),
-            rng.uniform(p_lo, 1.0, E - (cfg.burn_in + cfg.learning)).astype(np.float32))
 
 
 class RawMirror:
@@ -98,41 +83,19 @@ def test_default_exponent_is_the_unexponentiated_tree(eng_mod):
         assert np.array_equal(la.view(np.uint32), lb.view(np.uint32))
 
 
-def _replay_fed_run(eng_mod, kw, weighted):
-    cfg_rp = eng_mod.PathConfig(**kw)
-    cfg = eng_mod.PathConfig(**kw, is_exponent=0.6 if weighted else 0.0)
-    ep_len = 120
-    rng = np.random.default_rng(5)
-    rp = eng_mod.DeviceReplay(cfg_rp, capacity_rows=24 * (ep_len + cfg.n_step))
-    rp.add_episodes([episode(rng, cfg, ep_len) for _ in range(24)])
-    eng = eng_mod.LearnerEngine(cfg, seed=7)
-    assert eng.importance_weighting == weighted
-    gen = torch.Generator(device="cuda").manual_seed(11)
-
-    def hook(e, used):
-        rp.update_priorities(used.leaf_idx, used.priority)
-        rp.sample_into(e, generator=gen, beta=0.0)
-
-    rp.sample_into(eng, generator=gen, beta=0.0)
-    for _ in range(6):
-        eng.step(prefetch=hook)
-    torch.cuda.synchronize()
-    out = {k: getattr(eng, k).clone() for k in ("q_value", "target_q_value", "td_sq", "priority", "losses", "leaf_idx")}
-    out.update({f"flat.{n}": eng.flat[n].clone() for n in ("actor", "critic", "target_actor", "target_critic")})
-    out["launches"] = eng.launches_per_iteration
-    if weighted:
-        assert torch.equal(eng.is_weight, torch.ones_like(eng.is_weight))
-    rp.close()
-    eng.close()
-    return out
-
-
 @pytest.mark.parametrize("hidden,batch", [(256, 64), (512, 32)])
 def test_weighting_at_beta_zero_is_the_unweighted_run(eng_mod, hidden, batch):
-    kw = dict(obs=11, act=3, hidden=hidden, batch=batch, burn_in=10, learning=20, n_step=3)
-    off, on = _replay_fed_run(eng_mod, kw, False), _replay_fed_run(eng_mod, kw, True)
-    assert off.pop("launches") == on.pop("launches")
-    for k in off:
+    runs = []
+    for weighted in (False, True):
+        def setup(eng, weighted=weighted):
+            assert eng.importance_weighting == weighted
+        runs.append(replay_fed_run(eng_mod, 6, setup=setup, beta=0.0, hidden=hidden, batch=batch,
+                                   replay_cfg=eng_mod.PathConfig(**dict(REPLAY, hidden=hidden, batch=batch)),
+                                   keep=("td_sq", "leaf_idx", "is_weight"), is_exponent=0.6 if weighted else 0.0))
+    off, on = runs
+    assert torch.equal(on["is_weight"], torch.ones_like(on["is_weight"]))
+    for k in ("launches", "q_value", "target_q_value", "td_sq", "priority", "losses", "leaf_idx", "flat.actor",
+              "flat.critic", "flat.target_actor", "flat.target_critic"):
         assert torch.equal(off[k], on[k]), k
 
 
@@ -217,7 +180,7 @@ def test_importance_weights(eng_mod):
 
 
 # ---------------------------------------------------------------------------------------------------- 5. learner parity
-def _check_weighted_iteration(eng_mod, cfg, actor, critic, batch, w, it_kw):
+def _check_weighted_iteration(eng_mod, cfg, actor, critic, batch, w):
     """One weighted iteration against the float64 oracle; td_sq / priorities bit-identical to the unweighted engine."""
     eng = eng_mod.LearnerEngine(cfg)
     eng.load_state_dicts(actor, critic)
@@ -229,8 +192,7 @@ def _check_weighted_iteration(eng_mod, cfg, actor, critic, batch, w, it_kw):
     plain.step()
     torch.cuda.synchronize()
     assert torch.equal(eng.td_sq, plain.td_sq) and torch.equal(eng.priority, plain.priority)
-    ol = lo.OracleLearner(actor, critic, **it_kw)
-    ref = weighted_iteration(ol, batch, w)
+    ref = oracle_for(cfg, actor, critic).iteration(dict(batch, is_weight=w))
     errs = {"q": rel_l2(eng.q_value.cpu().numpy(), ref["q_value"]),
             "target": rel_l2(eng.target_q_value.cpu().numpy(), ref["target_q_value"]),
             "prio": rel_l2(eng.priority.cpu().numpy(), ref["priority"]),
@@ -255,10 +217,11 @@ def _check_weighted_iteration(eng_mod, cfg, actor, critic, batch, w, it_kw):
     nv.check(nv.lib().r2d2_td_priority_weighted(P(q), P(qn), P(rew), P(term), P(wt), L, B, A, cfg.burn_in, cfg.n_step,
                                                 cfg.gamma, cfg.eta, P(target), P(dq), P(td_sq), P(prio), P(loss),
                                                 nv.current_stream()))
-    _, loss_ref, dq_ref, _, _ = weighted_td(w)(ref["q_value"].reshape(L, B, A), ref["q_next"],
-                                               np.asarray(batch["rew"], np.float64).reshape(T, B),
-                                               np.asarray(batch["term"], np.float64).reshape(T, B),
-                                               burn_in=cfg.burn_in, learning=L, n_step=cfg.n_step, gamma=cfg.gamma)
+    _, loss_ref, dq_ref, _, _ = lo.td_targets_and_priorities(ref["q_value"].reshape(L, B, A), ref["q_next"],
+                                                             np.asarray(batch["rew"], np.float64).reshape(T, B),
+                                                             np.asarray(batch["term"], np.float64).reshape(T, B),
+                                                             burn_in=cfg.burn_in, learning=L, n_step=cfg.n_step,
+                                                             gamma=cfg.gamma, is_weight=w)
     torch.cuda.synchronize()
     errs["dq"] = rel_l2(dq.cpu().numpy(), dq_ref)
     errs["abi_loss"] = abs(loss.item() - loss_ref) / abs(loss_ref)
@@ -269,27 +232,18 @@ def _check_weighted_iteration(eng_mod, cfg, actor, critic, batch, w, it_kw):
 
 @pytest.mark.parametrize("name", ["ref_pend_h128.npz", "ref_walker_h128.npz"])
 def test_weighted_iteration_against_oracle_on_goldens(eng_mod, name):
-    g = load_golden(name)
-    kw = dict(obs=int(g["cfg/obs_size"]), act=int(g["cfg/n_actions"]), hidden=int(g["cfg/hidden"]),
-              batch=int(g["cfg/batch_size"]), burn_in=int(g["cfg/burn_in"]), learning=int(g["cfg/learning"]),
-              n_step=int(g["cfg/n_step"]))
+    kw, actor, critic, batches = golden_case(name)
     cfg = eng_mod.PathConfig(**kw, is_exponent=0.6)
     w = np.random.default_rng(17).uniform(0.05, 1.0, cfg.batch).astype(np.float32)
-    worst = _check_weighted_iteration(eng_mod, cfg, golden_params(g, "init/actor"), golden_params(g, "init/critic"),
-                                      golden_batch(g, 0), w,
-                                      dict(burn_in=cfg.burn_in, learning=cfg.learning, n_step=cfg.n_step))
+    worst = _check_weighted_iteration(eng_mod, cfg, actor, critic, batches[0], w)
     print(f"{name} weighted: worst relative error {worst:.3e}")
 
 
 def test_weighted_iteration_against_oracle_cfg2(eng_mod):
     kw = dict(obs=17, act=6, hidden=256, batch=256, burn_in=40, learning=80, n_step=5)
-    pc = ref_port.PathConfig(**kw)
-    port = ref_port.PortLearner(pc, seed=1)
-    sd = lambda m: {k: v.detach().numpy() for k, v in m.state_dict().items()}  # noqa: E731
+    actor, critic, batches = port_case(kw, n_batches=1)
     w = np.random.default_rng(19).uniform(0.05, 1.0, 256).astype(np.float32)
-    worst = _check_weighted_iteration(eng_mod, eng_mod.PathConfig(**kw, is_exponent=0.6), sd(port.actor),
-                                      sd(port.critic), ref_port.synthetic_batch(pc, seed=6), w,
-                                      dict(burn_in=40, learning=80, n_step=5))
+    worst = _check_weighted_iteration(eng_mod, eng_mod.PathConfig(**kw, is_exponent=0.6), actor, critic, batches[0], w)
     print(f"cfg-2 weighted: worst relative error {worst:.3e}")
 
 
@@ -346,84 +300,19 @@ def test_pipelined_weighted_run_matches_sequential(eng_mod):
 
 # ---------------------------------------------------------------------------------------------------- 7. drop-in
 def test_dropin_learner_with_prioritized_replay(monkeypatch):
-    import sys
-    for k, v in dict(R2D2_OBS_SIZE="5", R2D2_N_ACTIONS="2", R2D2_HIDDEN="64", R2D2_BATCH="4",
-                     R2D2_PRIORITY_EXPONENT="0.9", R2D2_IS_EXPONENT="0.6").items():
-        monkeypatch.setenv(k, v)
-    mods = ("actor", "learner", "replay_memory", "models", "utils")
-    for m in mods:
-        sys.modules.pop(m, None)
-    import actor as dropin_actor
-    import learner as dropin_learner
-    with tempfile.TemporaryDirectory() as d:
-        cwd = os.getcwd()
-        os.chdir(d)
-        try:
-            os.makedirs("model_data")
-            os.makedirs("memory_data")
-            lr = dropin_learner.Learner(n_actors=2)
-            assert lr.engine.importance_weighting and lr.engine.cfg.is_exponent == 0.6
-            for aid in range(2):
-                a = dropin_actor.Actor(aid)
-                a.env.episode_len = 150
-                a.run(max_episodes=5)
-            lr.model_save_interval = 2
-            lr.memory_update_interval = 2
-            lr.run(max_steps=4)
-            torch.cuda.synchronize()
-            assert lr.engine.step_count == 4
-            assert np.isfinite(lr.engine.losses.cpu().numpy()).all()
-            w = lr.engine.is_weight.cpu().numpy()
-            assert (w > 0).all() and (w <= 1).all() and w.max() == 1.0
-            p00 = lr.memory.priority[0][0]                                    # the stored leaf, p^alpha
-            assert np.isfinite(p00) and p00 >= 0
-            lr.memory.priority[0][0] = 0.25                                   # a raw write is raised on the way in
-            torch.cuda.synchronize()
-            assert abs(lr.memory.priority[0][0] / 0.25 ** 0.9 - 1) < 1e-6
-            out = lr.memory.sample()
-            assert len(out) == 10
-        finally:
-            os.chdir(cwd)
-            for m in mods:
-                sys.modules.pop(m, None)
+    with trained_dropin_learner(monkeypatch, R2D2_PRIORITY_EXPONENT="0.9", R2D2_IS_EXPONENT="0.6") as (lr, _):
+        assert lr.engine.importance_weighting and lr.engine.cfg.is_exponent == 0.6
+        w = lr.engine.is_weight.cpu().numpy()
+        assert (w > 0).all() and (w <= 1).all() and w.max() == 1.0
+        p00 = lr.memory.priority[0][0]                                    # the stored leaf, p^alpha
+        assert np.isfinite(p00) and p00 >= 0
+        lr.memory.priority[0][0] = 0.25                                   # a raw write is raised on the way in
+        torch.cuda.synchronize()
+        assert abs(lr.memory.priority[0][0] / 0.25 ** 0.9 - 1) < 1e-6
+        out = lr.memory.sample()
+        assert len(out) == 10
 
 
 # ---------------------------------------------------------------------------------------------------- 8. two GPUs
-def _dp_worker(rank, world, port, out_dir):
-    import torch.distributed as dist
-    from r2d2_b200 import engine
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device(f"cuda:{rank}"))
-    cfg = engine.PathConfig(obs=6, act=2, hidden=64, batch=8, burn_in=4, learning=6, n_step=2,
-                            priority_exponent=0.9, is_exponent=0.6)
-    eng = engine.LearnerEngine(cfg, device=f"cuda:{rank}", seed=5)
-    eng.enable_data_parallel()
-    rng = np.random.default_rng(100 + rank)                                  # every rank its own shard
-    rp = engine.DeviceReplay(cfg, capacity_rows=8000, device=f"cuda:{rank}")
-    rp.add_episodes([episode(rng, cfg, int(rng.integers(30, 90))) for _ in range(30)])
-    gen = torch.Generator(device=f"cuda:{rank}").manual_seed(7 + rank)
-
-    def hook(e, used):
-        rp.update_priorities(used.leaf_idx, used.priority)
-        rp.sample_into(e, generator=gen)
-
-    rp.sample_into(eng, generator=gen)
-    for _ in range(4):
-        eng.step(prefetch=hook)
-    torch.cuda.synchronize()
-    ok = bool(eng.replicas_identical()) and eng.peer_status() == 0
-    np.save(os.path.join(out_dir, f"rank{rank}.npy"), np.array([ok, (eng.is_weight < 1).any().item()]))
-    dist.barrier()
-    dist.destroy_process_group()
-
-
 def test_two_gpu_weighted_replicas_stay_identical():
-    if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    with tempfile.TemporaryDirectory() as d:
-        mp.spawn(_dp_worker, args=(2, 29700 + os.getpid() % 100, d), nprocs=2, join=True)
-        for r in range(2):
-            ok, _ = np.load(os.path.join(d, f"rank{r}.npy"))
-            assert ok, f"rank {r}: replicas diverged"
+    assert_two_gpu_replicas_stay_identical(dict(SMALL, priority_exponent=0.9, is_exponent=0.6))

@@ -3,7 +3,7 @@ absolute-TD-error priorities, through the C ABI, the learner engine, the actor s
 
  * the defaults give the bits of the entries without options and of an engine that never heard of them;
  * h_eps(h_eps^-1(q')) = q' on the device over 36 decades, on both TD routes;
- * the TD kernels against float64 (tests/rescale_oracle.py) in every mode x metric, weighted and not, on both sides of
+ * the TD kernels against float64 (oracle/learner_oracle.py) in every mode x metric, weighted and not, on both sides of
    the 48 KB shared-memory switch, each case asserting the kernel instantiation that served it (observed under
    torch.profiler in a fresh process, the `routes` fixture);
  * the actor-side kernel against float64, and ActorPool's memory files in the environment's mode;
@@ -19,19 +19,18 @@ import numpy as np
 import pytest
 import torch
 
-import rescale_oracle as ro
-from conftest import golden_batch, golden_params, load_golden, rel_l2
+from conftest import rel_l2
+from learner_harness import (SMALL, assert_pipelined_matches_sequential, assert_resumed_run_is_bit_identical,
+                             assert_same_bits, check_against_oracle, col_err, golden_case, port_case, replay_fed_run,
+                             snapshot, trained_dropin_learner)
+from oracle import actor_oracle
+from oracle import learner_oracle as lo
 from oracle import ref_port
-from optim_oracle import ClipHook, PolyakOracle
-from test_gpu_action_width import col_err
-from test_gpu_optimiser_step import _assert_same_bits, _snapshot
-from test_gpu_prioritized_replay import episode
 
 pytestmark = pytest.mark.gpu
 
 MODES = [(r, m) for r in ("reference", "invertible") for m in ("squared", "abs")]
 NATIVE = {"reference": 0, "invertible": 1, "squared": 0, "abs": 1}
-SMALL = dict(obs=6, act=2, hidden=64, batch=8, burn_in=4, learning=6, n_step=2)
 NEW = dict(value_rescaling="invertible", rescaling_eps=1e-3, priority_metric="abs")
 
 
@@ -237,35 +236,12 @@ def test_ex_defaults_are_the_plain_entries_bits(nv, A, weighted):
         _bits(base, td_call(nv, inputs, L, B, A, Bn, n, opts=opts, w=w))
 
 
-def _replay_fed(eng_mod, steps, extra=None, setters=None, seed=7):
-    cfg = eng_mod.PathConfig(obs=11, act=3, hidden=128, batch=32, burn_in=10, learning=20, n_step=3, target_interval=3,
-                             **(extra or {}))
-    rng = np.random.default_rng(5)
-    rp = eng_mod.DeviceReplay(cfg, capacity_rows=24 * (120 + cfg.n_step))
-    rp.add_episodes([episode(rng, cfg, 120) for _ in range(24)])
-    eng = eng_mod.LearnerEngine(cfg, seed=seed)
-    if setters is not None:
-        nv_lib = eng.lib
-        assert nv_lib.r2d2_learner_set_value_rescaling(eng._h, setters[0], setters[1]) == 0
-        assert nv_lib.r2d2_learner_set_priority_metric(eng._h, setters[2]) == 0
-    gen = torch.Generator(device="cuda").manual_seed(11)
-
-    def hook(e, used):
-        rp.update_priorities(used.leaf_idx, used.priority)
-        rp.sample_into(e, generator=gen)
-
-    rp.sample_into(eng, generator=gen)
-    for _ in range(steps):
-        eng.step(prefetch=hook)
-    out = _snapshot(eng)
-    out["launches"] = torch.tensor([eng.launches_per_iteration])
-    rp.close()
-    eng.close()
-    return out
-
-
 def test_engine_default_setters_keep_the_bits(eng_mod):
-    _assert_same_bits(_replay_fed(eng_mod, 5), _replay_fed(eng_mod, 5, setters=(0, 0.0, 0)))
+    def setters(eng):
+        assert eng.lib.r2d2_learner_set_value_rescaling(eng._h, 0, 0.0) == 0
+        assert eng.lib.r2d2_learner_set_priority_metric(eng._h, 0) == 0
+    kw = dict(target_interval=3)
+    assert_same_bits(replay_fed_run(eng_mod, 5, **kw), replay_fed_run(eng_mod, 5, setup=setters, **kw))
 
 
 def test_launch_count_is_the_same_in_every_mode(eng_mod):
@@ -331,8 +307,9 @@ def test_td_against_float64(nv, routes, A, td_sq, weighted, rescaling, metric):
     L, B, Bn, n, eps = 33, 77, 3, 5, 1e-3
     inputs = td_inputs(L, B, A, Bn, n, seed=A * 31 + weighted)
     w = np.random.default_rng(A + 1).uniform(0.05, 1.0, B).astype(np.float32) if weighted else None
-    ref = ro.td(rescaling, float(np.float32(eps)), metric, None if w is None else f64(w))(
-        *(f64(x) for x in inputs), burn_in=Bn, learning=L, n_step=n, gamma=0.997)
+    ref = lo.td_targets_and_priorities(*(f64(x) for x in inputs), burn_in=Bn, learning=L, n_step=n, gamma=0.997,
+                                       rescaling=rescaling, eps=float(np.float32(eps)), metric=metric,
+                                       is_weight=None if w is None else f64(w))
     want = ("y", "dq", "td", "p", "loss") if td_sq else ("y", "dq", "p", "loss")
     assert_route(routes, td_route_key(A, td_sq, weighted, rescaling, metric),
                  expected_kernels(A, td_sq, rescaling, metric))
@@ -393,9 +370,9 @@ def test_actor_priorities_ex_against_float64(nv, routes, rescaling, metric):
     got = actor_call(nv, q, qt, rew, term, rescaling, metric)
     for b, N in enumerate(c["lens"]):
         E = N - c["n"]
-        want = ro.window_priorities(f64(q[:E, b]), f64(qt[:N, b]), f64(rew[:N, b]), f64(term[:N, b]), burn_in=c["Bn"],
-                                    learning=c["L"], n_step=c["n"], gamma=c["gamma"], rescaling=rescaling,
-                                    eps=float(np.float32(c["eps"])), metric=metric)
+        want = actor_oracle.window_priorities(f64(q[:E, b]), f64(qt[:N, b]), f64(rew[:N, b]), f64(term[:N, b]), burn_in=c["Bn"],
+                                              learning=c["L"], n_step=c["n"], gamma=c["gamma"], rescaling=rescaling,
+                                              eps=float(np.float32(c["eps"])), metric=metric)
         assert rel_l2(got[b, :want.size], want) < 1e-5, (b, rel_l2(got[b, :want.size], want))
         assert (got[b, want.size:] == 0).all()
 
@@ -437,120 +414,46 @@ def test_actor_pool_files_use_the_environment_mode(monkeypatch, tmp_path):
 
 # ------------------------------------------------------------------------------------------------ 5. learner vs oracle
 def _check_learner(eng_mod, kw, actor, critic, batches, iters, *, tau=1.0, interval=500, clip=0.0, beta=False):
-    cfg = eng_mod.PathConfig(**kw, **NEW, target_tau=tau, target_interval=interval, grad_clip_norm=clip,
-                             is_exponent=0.6 if beta else 0.0)
-    eng = eng_mod.LearnerEngine(cfg)
-    eng.load_state_dicts(actor, critic)
-    ol = PolyakOracle(actor, critic, burn_in=kw["burn_in"], learning=kw["learning"], n_step=kw["n_step"],
-                      target_interval=interval, target_tau=float(np.float32(tau)))
-    hook = ClipHook(clip)
+    """From the second iteration on, with fresh importance weights every iteration when beta."""
     rng = np.random.default_rng(3)
-    errs = {}
-    for it in range(iters):
-        batch = dict(batches[it % len(batches)])
-        w = rng.uniform(0.05, 1.0, kw["batch"]).astype(np.float32) if beta else None
-        if beta:
-            batch["is_weight"] = w
-        eng.set_batch(batch)
-        eng.step()
-        ref = ro.iteration(ol, batch, "invertible", float(np.float32(1e-3)), "abs", None if w is None else f64(w),
-                           grad_hook=hook)
-        torch.cuda.synchronize()
-        if it:
-            errs[f"q/{it}"] = rel_l2(eng.q_value.cpu().numpy(), ref["q_value"])
-            errs[f"target/{it}"] = rel_l2(eng.target_q_value.cpu().numpy(), ref["target_q_value"])
-            errs[f"prio/{it}"] = rel_l2(eng.priority.cpu().numpy(), ref["priority"])
-    for net in ("actor", "critic"):
-        for what, mine, theirs in (("params", eng.views(net), getattr(ol, net)),
-                                   ("target", eng.views("target_" + net), getattr(ol, "target_" + net)),
-                                   ("m", eng.views(net, "exp_avg"), {k: ol.__dict__[net + "_adam"]["m/" + k] for k in eng_mod.PARAM_KEYS}),
-                                   ("v", eng.views(net, "exp_avg_sq"), {k: ol.__dict__[net + "_adam"]["v/" + k] for k in eng_mod.PARAM_KEYS})):
-            for k in eng_mod.PARAM_KEYS:
-                errs[f"{what}/{net}/{k}"] = rel_l2(mine[k].cpu().numpy(), theirs[k])
-    eng.close()
-    bad = {k: v for k, v in errs.items() if not v < 1e-3}
-    assert not bad, bad
-    return max(errs.values())
-
-
-def _golden_kw(g):
-    return dict(obs=int(g["cfg/obs_size"]), act=int(g["cfg/n_actions"]), hidden=int(g["cfg/hidden"]),
-                batch=int(g["cfg/batch_size"]), burn_in=int(g["cfg/burn_in"]), learning=int(g["cfg/learning"]),
-                n_step=int(g["cfg/n_step"]))
+    weights = (lambda it: rng.uniform(0.05, 1.0, kw["batch"]).astype(np.float32)) if beta else None
+    return check_against_oracle(eng_mod, dict(kw, **NEW, target_tau=tau, target_interval=interval, grad_clip_norm=clip,
+                                              is_exponent=0.6 if beta else 0.0),
+                                actor, critic, batches, iters, weights=weights, first=1)
 
 
 @pytest.mark.parametrize("extras", [False, True], ids=["plain", "weights_polyak_clip"])
 @pytest.mark.parametrize("name", ["ref_pend_h128.npz", "ref_walker_h128.npz"])
 def test_learner_against_oracle_on_goldens(eng_mod, name, extras):
-    g = load_golden(name)
-    n_it = len({k.split("/")[0] for k in g if k.startswith("it")})
-    kw = dict(tau=0.05, interval=1, clip=0.5, beta=True) if extras else {}
-    worst = _check_learner(eng_mod, _golden_kw(g), golden_params(g, "init/actor"), golden_params(g, "init/critic"),
-                           [golden_batch(g, i) for i in range(n_it)], 12, **kw)
+    kw, actor, critic, batches = golden_case(name)
+    extra = dict(tau=0.05, interval=1, clip=0.5, beta=True) if extras else {}
+    worst = _check_learner(eng_mod, kw, actor, critic, batches, 12, **extra)
     print(f"{name} extras={extras}: worst relative error {worst:.3e}")
 
 
 def test_learner_against_oracle_cfg2(eng_mod):
     kw = dict(obs=17, act=6, hidden=256, batch=256, burn_in=40, learning=80, n_step=5)
-    pc = ref_port.PathConfig(**kw)
-    port = ref_port.PortLearner(pc, seed=1)
-    sd = lambda m: {k: v.detach().numpy() for k, v in m.state_dict().items()}  # noqa: E731
-    worst = _check_learner(eng_mod, kw, sd(port.actor), sd(port.critic),
-                           [ref_port.synthetic_batch(pc, seed=6 + i) for i in range(3)], 6)
+    worst = _check_learner(eng_mod, kw, *port_case(kw), 6)
     print(f"cfg-2: worst relative error {worst:.3e}")
 
 
 # ------------------------------------------------------------------------------------------------ 6. determinism
 def test_pipelined_step_matches_sequential_bit_for_bit(eng_mod):
-    cfg = eng_mod.PathConfig(**SMALL, **NEW, target_interval=1000)
-    pc = ref_port.PathConfig(**SMALL)
-    steps = 6
-    batches = [ref_port.synthetic_batch(pc, seed=40 + it) for it in range(steps + 1)]
-    seq = eng_mod.LearnerEngine(cfg, seed=3)
-    seq_prio = []
-    for it in range(steps):
-        seq.set_batch(batches[it])
-        seq.step()
-        seq_prio.append(seq.priority.clone())
-    pip = eng_mod.LearnerEngine(cfg, seed=3)
-    pip_prio = []
-    pip.set_batch(batches[0])
-    for it in range(steps):
-        def hook(eng, used, it=it):
-            pip_prio.append(used.priority.clone())
-            eng.set_batch(batches[it + 1])
-        pip.step(prefetch=hook)
-    torch.cuda.synchronize()
-    for a, b in zip(seq_prio, pip_prio):
-        assert torch.equal(a, b)
-    _assert_same_bits(_snapshot(seq), _snapshot(pip))
+    assert_pipelined_matches_sequential(eng_mod, eng_mod.PathConfig(**SMALL, **NEW, target_interval=1000), 6)
 
 
 def test_replay_fed_runs_are_bitwise_reproducible(eng_mod):
-    a, b = _replay_fed(eng_mod, 7, NEW), _replay_fed(eng_mod, 7, NEW)
-    _assert_same_bits(a, b)
-    assert not torch.equal(a["priority"], _replay_fed(eng_mod, 7)["priority"])      # the options do change the run
+    a, b = replay_fed_run(eng_mod, 7, target_interval=3, **NEW), replay_fed_run(eng_mod, 7, target_interval=3, **NEW)
+    assert_same_bits(a, b)
+    assert not torch.equal(a["priority"], replay_fed_run(eng_mod, 7, target_interval=3)["priority"])   # the options matter
 
 
 def test_resumed_run_is_bit_identical(eng_mod):
-    cfg = eng_mod.PathConfig(**SMALL, **NEW, target_interval=3)
-    pc = ref_port.PathConfig(**SMALL)
-    a = eng_mod.LearnerEngine(cfg, seed=9)
-    for it in range(2):
-        a.set_batch(ref_port.synthetic_batch(pc, seed=it))
-        a.step()
-    st = a.training_state()
-    assert (st["value_rescaling"], st["priority_metric"]) == ("invertible", "abs")
-    b = eng_mod.LearnerEngine(cfg, seed=123)
-    b.load_training_state(st)
-    with pytest.raises(ValueError, match="invertible"):
-        eng_mod.LearnerEngine(eng_mod.PathConfig(**SMALL), seed=1).load_training_state(st)
-    for it in range(2, 7):
-        batch = ref_port.synthetic_batch(pc, seed=it)
-        for e in (a, b):
-            e.set_batch(batch)
-            e.step()
-    _assert_same_bits(_snapshot(a), _snapshot(b))
+    def check_state(st):
+        assert (st["value_rescaling"], st["priority_metric"]) == ("invertible", "abs")
+        with pytest.raises(ValueError, match="invertible"):
+            eng_mod.LearnerEngine(eng_mod.PathConfig(**SMALL), seed=1).load_training_state(st)
+    assert_resumed_run_is_bit_identical(eng_mod, eng_mod.PathConfig(**SMALL, **NEW, target_interval=3), check_state)
 
 
 def test_options_may_change_between_iterations(eng_mod):
@@ -571,44 +474,18 @@ def test_options_may_change_between_iterations(eng_mod):
         for e in (a, b):
             e.set_batch(batch)
             e.step()
-    _assert_same_bits(_snapshot(a), _snapshot(b))
+    assert_same_bits(snapshot(a), snapshot(b))
 
 
 # ------------------------------------------------------------------------------------------------ 7. drop-in
 def test_dropin_learner_trains_with_the_options(monkeypatch):
-    for k, v in dict(R2D2_OBS_SIZE="5", R2D2_N_ACTIONS="2", R2D2_HIDDEN="64", R2D2_BATCH="4",
-                     R2D2_VALUE_RESCALING="invertible", R2D2_RESCALING_EPS="0.001", R2D2_PRIORITY_METRIC="abs").items():
-        monkeypatch.setenv(k, v)
-    mods = ("actor", "learner", "replay_memory", "models", "utils")
-    for m in mods:
-        sys.modules.pop(m, None)
-    import actor as dropin_actor
-    import learner as dropin_learner
-    with tempfile.TemporaryDirectory() as d:
-        cwd = os.getcwd()
-        os.chdir(d)
-        try:
-            os.makedirs("model_data")
-            os.makedirs("memory_data")
-            lr = dropin_learner.Learner(n_actors=2)
-            c = lr.engine.cfg
-            assert (c.value_rescaling, c.rescaling_eps, c.priority_metric) == ("invertible", 0.001, "abs")
-            for aid in range(2):
-                a = dropin_actor.Actor(aid)
-                assert a.td_options == lr.td_options
-                a.env.episode_len = 150
-                a.run(max_episodes=5)
-            lr.model_save_interval = 2
-            lr.memory_update_interval = 2
-            lr.run(max_steps=4)
-            torch.cuda.synchronize()
-            assert lr.engine.step_count == 4
-            assert np.isfinite(lr.engine.losses.cpu().numpy()).all()
-            p = lr.engine.priority.cpu().numpy()
-            assert np.isfinite(p).all() and (p > 0).all()
-            st = torch.load("model_data/learner_state.pt", weights_only=False)
-            assert (st["value_rescaling"], st["priority_metric"]) == ("invertible", "abs")
-        finally:
-            os.chdir(cwd)
-            for m in mods:
-                sys.modules.pop(m, None)
+    with trained_dropin_learner(monkeypatch, R2D2_VALUE_RESCALING="invertible", R2D2_RESCALING_EPS="0.001",
+                                R2D2_PRIORITY_METRIC="abs") as (lr, actors):
+        c = lr.engine.cfg
+        assert (c.value_rescaling, c.rescaling_eps, c.priority_metric) == ("invertible", 0.001, "abs")
+        for a in actors:
+            assert a.td_options == lr.td_options
+        p = lr.engine.priority.cpu().numpy()
+        assert np.isfinite(p).all() and (p > 0).all()
+        st = torch.load("model_data/learner_state.pt", weights_only=False)
+        assert (st["value_rescaling"], st["priority_metric"]) == ("invertible", "abs")
