@@ -101,6 +101,47 @@ def net_forward(p, x, h0, c0, *, critic: bool, repeat: int = 1):
     return {"x": x, "z1": z1, "gates": gates, "hs": hs, "cs": cs, "out": out, "repeat": repeat}
 
 
+def lstm_scan(gin, whh, h0=None, c0=None, dh_head=None, *, repeat=1, head_first_step=0):
+    """The recurrence alone, as r2d2_lstm_scan_forward / _backward compute it: gates_s = gin[s // repeat] + h_{s-1}
+    W_hh^T for s < S = T * repeat (h0 / c0 None: zero state).  Step s >= head_first_step with (s - head_first_step) %
+    repeat == repeat - 1 adds dh_head row (s - head_first_step) // repeat to dL/dh_s (dh_head None: forward only).
+    Returns hs, cs [S+1,B,H] (slot 0 = initial state), gates [S,B,4H] post-activation (i, f, g, o), head_in [T,B,H] =
+    tanh(h) after the last step of each row and, with dh_head, dgates [S,B,4H] and dgin [T,B,4H] (dgates summed per
+    input row)."""
+    T, B, H4 = gin.shape
+    H, S = H4 // 4, T * repeat
+    hs, cs = np.zeros((S + 1, B, H)), np.zeros((S + 1, B, H))
+    gates = np.empty((S, B, H4))
+    if h0 is not None:
+        hs[0] = h0
+    if c0 is not None:
+        cs[0] = c0
+    for s in range(S):
+        pre = gin[s // repeat] + hs[s] @ whh.T
+        i, f, g, o = _sigmoid(pre[:, :H]), _sigmoid(pre[:, H:2 * H]), np.tanh(pre[:, 2 * H:3 * H]), _sigmoid(pre[:, 3 * H:])
+        cs[s + 1] = f * cs[s] + i * g
+        hs[s + 1] = o * np.tanh(cs[s + 1])
+        gates[s] = np.concatenate((i, f, g, o), 1)
+    out = {"hs": hs, "cs": cs, "gates": gates, "head_in": np.tanh(hs[repeat::repeat])}
+    if dh_head is None:
+        return out
+    dgates, dgin = np.empty_like(gates), np.zeros_like(gin)
+    dh_rec, dc_next = np.zeros((B, H)), np.zeros((B, H))
+    for s in range(S - 1, -1, -1):
+        i, f, g, o = gates[s, :, :H], gates[s, :, H:2 * H], gates[s, :, 2 * H:3 * H], gates[s, :, 3 * H:]
+        rel = s - head_first_step
+        dh = dh_rec + (dh_head[rel // repeat] if rel >= 0 and rel % repeat == repeat - 1 else 0.0)
+        tc = np.tanh(cs[s + 1])
+        dc = dc_next + dh * o * (1 - tc * tc)
+        dgates[s] = np.concatenate((dc * g * i * (1 - i), dc * cs[s] * f * (1 - f), dc * i * (1 - g * g),
+                                    dh * tc * o * (1 - o)), 1)
+        dc_next = dc * f
+        dh_rec = dgates[s] @ whh
+        dgin[s // repeat] += dgates[s]
+    out.update(dgates=dgates, dgin=dgin)
+    return out
+
+
 def net_backward(p, sv, d_out, *, critic: bool, want_wgrad: bool = True, want_dx: bool = False):
     """Manual BPTT.  d_out [S,B,A] (zero rows where the output is unused)."""
     x, z1, gates, hs, cs, out, repeat = (sv[k] for k in ("x", "z1", "gates", "hs", "cs", "out", "repeat"))

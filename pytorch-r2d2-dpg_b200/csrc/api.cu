@@ -30,6 +30,17 @@ int num_sms() {
   }
   return n;
 }
+int max_smem_optin() {
+  static std::atomic<int> cache[64];   // 0 = not queried yet
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 232448;
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess || n <= 0) n = 232448;
+    cache[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 }  // namespace r2d2
 
 using namespace r2d2;

@@ -58,6 +58,8 @@ struct PerDeviceOnce {
 // streaming multiprocessors of the current device (cached per device): sizes grids of the grid-stride kernels and
 // split-K factors
 int num_sms();
+// opt-in shared memory per block of the current device in bytes (cached per device; 227 KB on an H100)
+int max_smem_optin();
 
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 static inline long long ceil_div_ll(long long a, long long b) { return (a + b - 1) / b; }

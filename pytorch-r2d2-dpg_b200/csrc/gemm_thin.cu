@@ -456,10 +456,13 @@ int launch_thin_tn(const float* X, long long ldx, int P, const float* Y, long lo
   return R2D2_OK;
 }
 
+int smalln_np(int N) { return N <= 8 ? 8 : N <= 16 ? 16 : 32; }
+size_t smalln_smem_bytes(int N, int K) { return (size_t)smalln_np(N) * (ceil_div(K, 128) * 128) * sizeof(float); }
+
 template <bool NN, int NP>
 int launch_thin_smalln(const GemmParams& p, cudaStream_t stream) {
   const int kpad = ceil_div(p.K, 128) * 128;
-  const size_t smem = (size_t)NP * kpad * sizeof(float);
+  const size_t smem = smalln_smem_bytes(p.N, p.K);
   if (smem > 48 * 1024)   // rare (N = 32 with K > 384): not worth caching per device
     R2D2_CUDA_TRY(cudaFuncSetAttribute(thin_smalln_kernel<NN, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int groups = ceil_div(p.M, 32 / NP);
@@ -502,7 +505,10 @@ int gemm_thin_try(const GemmParams& p, GemmLayout layout, cudaStream_t stream, b
     if (p.K == 256) return nn ? launch_thin_rowdot<true, 8>(p, stream) : launch_thin_rowdot<false, 8>(p, stream);
     return nn ? launch_thin_rowdot<true, 16>(p, stream) : launch_thin_rowdot<false, 16>(p, stream);
   }
-  if (p.N <= 32 && p.K2 == 0 && p.K >= 64 && p.K <= 2048 && (p.K % 4 == 0) && aligned16(p.A, p.lda)) {
+  // the [NP][kpad] weight tile must fit the opt-in shared memory (N > 16 with K > 1792 on an H100 does not): those
+  // products fall through to the mma.sync kernel (N < 32) or wgmma (N = 32)
+  if (p.N <= 32 && p.K2 == 0 && p.K >= 64 && p.K <= 2048 && (p.K % 4 == 0) && aligned16(p.A, p.lda) &&
+      smalln_smem_bytes(p.N, p.K) <= (size_t)max_smem_optin()) {
     *handled = true;
     if (p.N <= 8)  return nn ? launch_thin_smalln<true, 8>(p, stream) : launch_thin_smalln<false, 8>(p, stream);
     if (p.N <= 16) return nn ? launch_thin_smalln<true, 16>(p, stream) : launch_thin_smalln<false, 16>(p, stream);

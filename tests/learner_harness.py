@@ -1,6 +1,7 @@
-"""Helpers shared by the learner tests: the float64 oracle of a PathConfig and the one check of an engine against it,
-bit snapshots of an engine, replay episodes and fed runs, the schedule comparisons (pipelined, resumed), the drop-in
-learner on a fake engine (CPU) and trained for a few steps (GPU), and the two-GPU NCCL replica check."""
+"""Helpers shared by the learner tests: error bounds local to one action column, batch tile or unit group, the float64
+oracle of a PathConfig and the one check of an engine against it, bit snapshots of an engine, replay episodes and fed
+runs, the schedule comparisons (pipelined, resumed), the drop-in learner on a fake engine (CPU) and trained for a few
+steps (GPU), and the two-GPU NCCL replica check."""
 import contextlib
 import os
 import socket
@@ -31,6 +32,36 @@ def col_err(x, ref, A):
     ref = np.asarray(ref, np.float64).reshape(-1, A)
     rms_col = np.linalg.norm(ref) / np.sqrt(A)
     return float(np.linalg.norm(x - ref, axis=0).max() / max(rms_col, 1e-30))
+
+
+def _worst_group(x, ref, axis, size):
+    """max over consecutive groups of `size` indices along `axis` (the last group may be shorter) of the relative L2
+    norm within the group."""
+    x = np.moveaxis(np.asarray(x, np.float64), axis, 0)
+    ref = np.moveaxis(np.asarray(ref, np.float64), axis, 0)
+    worst = 0.0
+    for g in range(0, x.shape[0], size):
+        d, r = np.linalg.norm(x[g:g + size] - ref[g:g + size]), np.linalg.norm(ref[g:g + size])
+        worst = max(worst, float(d / max(r, 1e-30)))
+    return worst
+
+
+def tile_err(x, ref, NB, axis=-2):
+    """Worst relative L2 over the batch tiles of NB rows (one scan cluster each) along the batch axis, the ragged last
+    tile counted on its own: a whole-tensor norm dilutes an error confined to one tile of B / NB by sqrt(B / NB)."""
+    return _worst_group(x, ref, axis, NB)
+
+
+def unit_group_err(x, ref, H, axis=-1):
+    """Worst relative L2 over the groups of 32 hidden units (one cluster CTA each) along a unit axis of length H or 4H;
+    on a 4H axis the groups are taken per gate block (i, f, g, o), so no group straddles two gates."""
+    x, ref = np.asarray(x, np.float64), np.asarray(ref, np.float64)
+    n = x.shape[axis]
+    assert n in (H, 4 * H), f"unit axis of length {n} at H = {H}"
+    if n == H:
+        return _worst_group(x, ref, axis, 32)
+    return max(_worst_group(np.take(x, range(q * H, (q + 1) * H), axis), np.take(ref, range(q * H, (q + 1) * H), axis),
+                            axis, 32) for q in range(4))
 
 
 # ------------------------------------------------------------------------------------------------ cases

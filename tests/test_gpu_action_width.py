@@ -13,7 +13,6 @@ A relative L2 norm over a whole tensor dilutes an error confined to one action c
 with an action axis is also bounded per column (col_err).  Each kernel-level case runs under torch.profiler (run_routed)
 and asserts the kernel that served it, so a dispatch change that moves a case off its route fails by name instead of
 silently dropping the coverage.  Run with -s for the routes seen and the worst errors per group."""
-import re
 from collections import defaultdict
 
 import numpy as np
@@ -26,6 +25,7 @@ from oracle import actor_oracle
 from oracle import learner_oracle as lo
 from oracle import ref_port
 from oracle.sumtree import SumTreeOracle
+from route_check import RouteLog
 
 pytestmark = pytest.mark.gpu
 
@@ -34,21 +34,9 @@ LEARNER_TOL = 1e-3
 NT, NN, TN = 0, 1, 2
 EPI_NONE, EPI_TANH, EPI_MUL_DTANH = 0, 1, 2
 
-# route name -> kernel (base name) that serves it
-ROUTE_KERNELS = {
-    "td_column": "td_priority_column_kernel",
-    "td_two_pass": "td_elem_kernel",
-    "smallk": "thin_smallk_kernel",
-    "smalln": "thin_smalln_kernel",
-    "rowdot4": "thin_rowdot4_kernel",
-    "thin_tn": "thin_tn_kernel",
-    "mma": "gemm_bf16x3_kernel",
-    "wgmma": "gemm_packed_kernel",
-}
-
 WORST = defaultdict(lambda: [0.0, 0.0])   # group -> [worst rel_l2, worst col_err]
-SEEN = {}                                 # case -> route kernels the profiler saw
-LOST_SESSIONS = []                        # cases whose profiler session came back without a route kernel (repeated)
+ROUTES = RouteLog()
+run_routed = ROUTES.run_routed
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -57,10 +45,7 @@ def report():
     print("\nworst errors per group (rel_l2, col_err):")
     for g, (r, c) in sorted(WORST.items()):
         print(f"  {g:18s} {r:.2e}  {c:.2e}")
-    print(f"profiler sessions repeated: {len(LOST_SESSIONS)} {LOST_SESSIONS}")
-    print("routes seen:")
-    for case, names in SEEN.items():
-        print(f"  {case}: {names}")
+    ROUTES.report()
 
 
 def check(group, name, x, ref, tol, A=None):
@@ -97,50 +82,6 @@ def nv():
 def eng_mod():
     from r2d2_b200 import engine
     return engine
-
-
-# ------------------------------------------------------------------------------------------------ route check
-def _ran(names, base, bucket):
-    """Did a kernel `base` with template bucket `bucket` (None: any) run?  Accepts demangled and Itanium-mangled names."""
-    for n in names:
-        if base not in n:
-            continue
-        if bucket is None:
-            return True
-        if re.search(re.escape(base) + r"<[^>]*\b%d>" % bucket, n) or \
-           re.search(re.escape(base) + r"I(?:L[bi]\d+E)*Li%dE" % bucket, n):
-            return True
-    return False
-
-
-def run_routed(case, route, fn):
-    """Run fn (idempotent) under the CUDA profiler and assert that, of the route kernels, exactly the expected one served
-    it.  route: key of ROUTE_KERNELS, optionally "key:bucket" (NP of thin_smalln, QP of thin_tn).  torch.profiler now and
-    then returns a session without any of the kernels it ran (on an H100 with torch 2.11 / CUDA 12.8, about one session
-    in a hundred, and then often the next few sessions too): a session that recorded no route kernel at all is repeated
-    after a growing pause, five sessions in all, and then fails.  A session that recorded a different route kernel fails
-    at once.  Every session runs fn in full; the caller checks the values of the last one."""
-    import time
-    from torch.autograd import DeviceType
-    from torch.profiler import ProfilerActivity, profile
-    key, _, bucket = route.partition(":")
-    bucket = int(bucket) if bucket else None
-    for pause in (0.1, 0.3, 1.0, 3.0, None):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            out = fn()
-            torch.cuda.synchronize()
-        names = sorted({e.name for e in prof.events() if e.device_type == DeviceType.CUDA})
-        seen = sorted(k for k in ROUTE_KERNELS if any(ROUTE_KERNELS[k] in n for n in names))
-        if seen or pause is None:
-            break
-        LOST_SESSIONS.append(case)
-        time.sleep(pause)
-    assert seen, f"{case}: the profiler recorded no route kernel in five sessions (kernels recorded: {names})"
-    SEEN[case] = [n for n in names if any(b in n for b in ROUTE_KERNELS.values())]
-    assert seen == [key], f"{case}: expected route {key} ({ROUTE_KERNELS[key]}), the kernels that ran: {SEEN[case]}"
-    assert _ran(names, ROUTE_KERNELS[key], bucket), f"{case}: expected {ROUTE_KERNELS[key]} bucket {bucket}: {SEEN[case]}"
-    return out
 
 
 def gemm(nv, layout, M, N, K, A, lda, B, ldb, C, ldc, *, A2=None, lda2=0, B2=None, ldb2=0, K2=0, bias=None, Z=None,

@@ -18,6 +18,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from conftest import GOLDEN, rel_l2  # noqa: E402
+from oracle import learner_oracle as lo  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -36,10 +37,6 @@ CASES = {
 }
 
 
-def _sigmoid(x):
-    return 1.0 / (1.0 + np.exp(-x))
-
-
 def inputs(H, B, T, repeat, head_first_step):
     rng = np.random.default_rng(H * 131 + B * 7 + repeat)
     f32 = lambda a: np.asarray(a, np.float32)  # noqa: E731
@@ -48,37 +45,6 @@ def inputs(H, B, T, repeat, head_first_step):
     h0, c0 = f32(0.3 * rng.standard_normal((B, H))), f32(0.3 * rng.standard_normal((B, H)))
     dh_head = f32(rng.standard_normal(((T * repeat - head_first_step) // repeat, B, H)))
     return gin, whh, h0, c0, dh_head
-
-
-def oracle(gin, whh, h0, c0, dh_head, repeat, head_first_step):
-    """float64 forward (hs[1..S]) and BPTT (dG summed per input row) of gates_s = gin[s // repeat] + h_{s-1} W_hh^T;
-    step s >= head_first_step with (s - head_first_step) % repeat == repeat - 1 adds dh_head row
-    (s - head_first_step) // repeat."""
-    T, B, H4 = gin.shape
-    H, S = H4 // 4, T * repeat
-    h, c = h0.copy(), c0.copy()
-    hs, gs, cs = np.empty((S, B, H)), np.empty((S, B, H4)), np.empty((S + 1, B, H))
-    cs[0] = c
-    for s in range(S):
-        pre = gin[s // repeat] + h @ whh.T
-        i, f, g, o = _sigmoid(pre[:, :H]), _sigmoid(pre[:, H:2 * H]), np.tanh(pre[:, 2 * H:3 * H]), _sigmoid(pre[:, 3 * H:])
-        c = f * c + i * g
-        h = o * np.tanh(c)
-        hs[s], cs[s + 1] = h, c
-        gs[s] = np.concatenate((i, f, g, o), 1)
-    dgin = np.zeros_like(gin)
-    dh_rec, dc_next = np.zeros((B, H)), np.zeros((B, H))
-    for s in range(S - 1, -1, -1):
-        i, f, g, o = gs[s, :, :H], gs[s, :, H:2 * H], gs[s, :, 2 * H:3 * H], gs[s, :, 3 * H:]
-        rel = s - head_first_step
-        dh = dh_rec + (dh_head[rel // repeat] if rel >= 0 and rel % repeat == repeat - 1 else 0.0)
-        tc = np.tanh(cs[s + 1])
-        dc = dc_next + dh * o * (1 - tc * tc)
-        dg = np.concatenate((dc * g * i * (1 - i), dc * cs[s] * f * (1 - f), dc * i * (1 - g * g), dh * tc * o * (1 - o)), 1)
-        dc_next = dc * f
-        dh_rec = dg @ whh
-        dgin[s // repeat] += dg
-    return hs, dgin
 
 
 def run_chain(nv, H, B, T, repeat, head_first_step):
@@ -133,9 +99,10 @@ def test_bwd_stage_matches_oracle_and_golden_bits(nv, golden, name):
     H, B, T, repeat, hfs = CASES[name]
     hs, dgates, dgin = run_chain(nv, H, B, T, repeat, hfs)
     assert scan_status(nv) == 0, "a bounded hand-off wait expired inside a scan kernel"
-    hs_ref, dgin_ref = oracle(*(a.astype(np.float64) for a in inputs(H, B, T, repeat, hfs)), repeat, hfs)
-    assert rel_l2(hs[1:], hs_ref) < TOL_FWD
-    assert rel_l2(dgin, dgin_ref) < TOL_BWD
+    ref = lo.lstm_scan(*(a.astype(np.float64) for a in inputs(H, B, T, repeat, hfs)), repeat=repeat,
+                       head_first_step=hfs)
+    assert rel_l2(hs[1:], ref["hs"][1:]) < TOL_FWD
+    assert rel_l2(dgin, ref["dgin"]) < TOL_BWD
     assert digests(dgates, dgin) == golden[name], "BPTT bits differ from the recorded ones"
 
 
