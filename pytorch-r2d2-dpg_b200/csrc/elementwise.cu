@@ -453,6 +453,8 @@ int check_td_options(const TdOptions& opt) {
 int td_priority(const TdPriorityParams& params, cudaStream_t stream, const TdOptions& opt) {
   R2D2_REQUIRE(params.q && params.q_next && params.rew && params.term, "null input");
   R2D2_REQUIRE(params.L > 0 && params.B > 0 && params.A > 0, "shape");
+  R2D2_REQUIRE(!params.priority || params.L >= 2, "a priority output needs L >= 2: the [b:-1:B] series of the last "
+                                                  "batch element drops its last TD step, so L = 1 leaves it empty");
   R2D2_TRY(check_td_options(opt));
   const bool inv = opt.rescaling == kRescaleInvertible, abs_ = opt.priority_metric == kPriorityAbs;
   TdPriorityParams p = params;

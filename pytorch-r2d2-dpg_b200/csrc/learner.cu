@@ -37,6 +37,8 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg, bool twin_crit
   R2D2_REQUIRE(out && cfg, "null");
   R2D2_REQUIRE(cfg->obs_size > 0 && cfg->n_actions > 0 && cfg->hidden > 0 && cfg->hidden % 4 == 0, "sizes");
   R2D2_REQUIRE(cfg->batch > 0 && cfg->burn_in >= 0 && cfg->learning > 0 && cfg->n_step > 0, "window");
+  R2D2_REQUIRE(cfg->learning >= 2, "learning >= 2: the [b:-1:B] priority series of the last batch element drops its "
+                                   "last TD step, so a one-step window leaves it empty");
   R2D2_REQUIRE(cfg->actor_params && cfg->critic_params && cfg->target_actor_params && cfg->target_critic_params,
                "parameter buffers");
   R2D2_REQUIRE(cfg->actor_grads && cfg->critic_grads && cfg->actor_exp_avg && cfg->actor_exp_avg_sq &&

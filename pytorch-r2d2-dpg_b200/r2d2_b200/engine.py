@@ -73,6 +73,12 @@ class PathConfig:
     target_noise_seed: int = 0
 
     def __post_init__(self):
+        for name, least in (("burn_in", 0), ("learning", 2), ("n_step", 1)):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < least:
+                raise ValueError("%s must be an integer >= %d, got %r%s" % (
+                    name, least, v, " (the priority series [b:-1:B] of the last batch element drops its last TD step, "
+                                    "so a one-step window leaves it empty)" if name == "learning" else ""))
         td_options.validate(self.value_rescaling, self.rescaling_eps, self.priority_metric)
         if not isinstance(self.twin_critic, bool):
             raise ValueError("twin_critic must be True or False, got %r" % (self.twin_critic,))

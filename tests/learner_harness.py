@@ -52,6 +52,17 @@ def tile_err(x, ref, NB, axis=-2):
     return _worst_group(x, ref, axis, NB)
 
 
+def step_err(x, ref, axis=0):
+    """Worst relative L2 over the single time rows along `axis`: a whole-tensor norm over T rows dilutes an error confined
+    to one step by about sqrt(T).  A row is measured against its own reference norm, or against 1e-3 of the RMS row norm
+    when its own is smaller (far from the head a BPTT row can decay below fp32's range, where float64 still has digits)."""
+    x = np.moveaxis(np.asarray(x, np.float64), axis, 0).reshape(np.shape(x)[axis], -1)
+    ref = np.moveaxis(np.asarray(ref, np.float64), axis, 0).reshape(x.shape)
+    rn = np.linalg.norm(ref, axis=1)
+    floor = 1e-3 * np.sqrt(np.mean(rn * rn))
+    return float((np.linalg.norm(x - ref, axis=1) / np.maximum(np.maximum(rn, floor), 1e-30)).max())
+
+
 def unit_group_err(x, ref, H, axis=-1):
     """Worst relative L2 over the groups of 32 hidden units (one cluster CTA each) along a unit axis of length H or 4H;
     on a 4H axis the groups are taken per gate block (i, f, g, o), so no group straddles two gates."""
