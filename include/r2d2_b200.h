@@ -35,6 +35,8 @@ extern "C" {
 typedef void* r2d2_stream_t; /* cudaStream_t */
 
 int r2d2_version(void);                /* 100 * major + minor */
+/* kernels this process has launched through the library so far (launch budgets of the entry points) */
+long long r2d2_launch_count(void);
 const char* r2d2_arch(void);           /* "sm_90a" */
 const char* r2d2_last_error(void);
 int r2d2_device_sm_count(int* out);
@@ -262,6 +264,40 @@ int r2d2_replay_decode(r2d2_replay_t* r, const long long* leaf_idx_host, int n, 
 /* raw device views for tests: tree level pointer/size, leaf priorities */
 int r2d2_replay_tree_level(r2d2_replay_t* r, int level, const float** dev_ptr, long long* n);
 
+/* Global sampling over the replay shards of W data-parallel ranks (off unless a shard is attached to a group).  The W
+ * shard roots form one more tree level above the shards, in rank order: global draw j of W*B takes r = u_j * total
+ * (total the left-to-right fp32 sum of the roots), walks the roots as the tree walks 32 children and descends the
+ * owning shard's tree with the residual; rank c trains on draws c*B .. c*B+B-1, drawn with rank c's own B uniforms.
+ * At W = 1 the draw, the batch and the weights are r2d2_replay_sample(_weighted)'s bit for bit.
+ * Every rank allocates `bytes` of zeroed device memory that every rank maps and attaches all W base addresses; the
+ * rank's two batch slots live in that buffer (r2d2_learner_set_slot_buffers), so that the owner of a drawn row stores
+ * it straight into the consumer's slot.  Every kernel runs in the caller's stream; no host synchronisation. */
+typedef struct {
+  size_t bytes;            /* per rank: exchange block + two batch slots */
+  size_t slot_offset[2];   /* byte offset of each batch slot in the buffer */
+  /* byte offsets inside a slot: obs [T,B,O], act [T,B,A], rew [T,B], term [T,B], states [4,2,B,H], leaf_idx [B]
+   * (int64), shard [B] (int32), is_weight [B], uniforms [B] - every one 256-byte aligned */
+  size_t off_obs, off_act, off_rew, off_term, off_states, off_leaf_idx, off_shard, off_is_weight, off_uniforms;
+} r2d2_global_layout;
+/* rows = burn_in + learning + n_step (host arithmetic only) */
+int r2d2_global_layout_for(int rows, int batch, int obs_size, int n_actions, int hidden, int world, r2d2_global_layout* out);
+/* buffer_bytes: the size every rank allocated; it must equal r2d2_global_layout_for(...).bytes of this shard's shape */
+int r2d2_replay_attach_group(r2d2_replay_t* r, int rank, int world, int batch, void* const* peer_bases,
+                             size_t buffer_bytes);
+/* Write-back of the batch this rank trained on: DEVICE leaf_idx [B], shard [B] (its slot's), raw priority [B].  Stage 0
+ * publishes the B records to every rank, stage 1 waits for every rank's records and applies those of this shard in
+ * global-index order (the highest index wins on a duplicate leaf); -1 runs both.  Must alternate with draws. */
+int r2d2_replay_global_write_back(r2d2_replay_t* r, int stage, const long long* leaf_idx, const int* shard,
+                                  const float* priority, r2d2_stream_t stream);
+/* Draw the next batch into batch slot `slot` (its uniforms [B] hold this rank's draws).  Stage 0 publishes this shard's
+ * root (after the write-back and any ingest) and the uniforms, stage 1 waits for every root, draws, gathers this
+ * shard's rows into the consumers' slots and signals delivery with the minimum drawn leaf, stage 2 waits for every
+ * owner's delivery and, with `weighted`, turns the leaf values into (min / leaf)^beta over the global batch; -1 runs
+ * all three.  7 kernels per iteration with the write-back (2 + 5). */
+int r2d2_replay_global_draw(r2d2_replay_t* r, int stage, int slot, int weighted, float beta, r2d2_stream_t stream);
+/* 0 = fine, 1 = a bounded wait (4 s) for a peer's flag expired (synchronises the stream) */
+int r2d2_replay_global_status(r2d2_replay_t* r, int* status, r2d2_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Learner iteration engine (learner.py:84-139 minus file I/O).  Parameters, gradients and Adam
  * moments are caller-owned flat device buffers; the engine owns batch buffers and workspaces.
@@ -352,6 +388,10 @@ int r2d2_learner_select_batch(r2d2_learner_t* l, int slot);
  * r2d2_replay_sample_weighted or memcpy; 1 after create).  The critic phase reads the selected slot's weights only
  * while importance weighting is on; off (the default) it runs the unweighted TD kernels. */
 int r2d2_learner_is_weights(r2d2_learner_t* l, int slot, float** out);
+/* Move batch slot `slot` into caller-owned device memory (global sampling: the slots in the buffer every rank maps):
+ * obs .. uniforms of `b` (the other fields are ignored) and is_weight [B].  Refused while a prefetched batch's target
+ * chains are pending; the default slots stay allocated in the learner's arena. */
+int r2d2_learner_set_slot_buffers(r2d2_learner_t* l, int slot, const r2d2_learner_buffers* b, float* is_weight);
 int r2d2_learner_set_importance_weighting(r2d2_learner_t* l, int on);
 /* Polyak target update (utils.py:4-6): on the iterations of the hard copy (step % target_update_interval == 0) each
  * target becomes fl(fl(target * (float)(1 - (double)tau)) + fl(param' * tau)), param' the net's post-Adam weight, fused

@@ -53,6 +53,7 @@ static inline NetShape shape_of(const r2d2_net_shape* s) {
 extern "C" {
 
 int r2d2_version(void) { return 100; }
+long long r2d2_launch_count(void) { return launch_count(); }
 const char* r2d2_arch(void) { return "sm_90a"; }
 const char* r2d2_last_error(void) { return last_error(); }
 
@@ -277,6 +278,33 @@ int r2d2_replay_tree_level(r2d2_replay_t* r, int level, const float** dev_ptr, l
   return replay_tree_level(reinterpret_cast<Replay*>(r), level, dev_ptr, n);
 }
 
+int r2d2_global_layout_for(int rows, int batch, int obs_size, int n_actions, int hidden, int world, r2d2_global_layout* out) {
+  R2D2_REQUIRE(out, "null");
+  R2D2_REQUIRE(world >= 1 && world <= kGlobalMaxWorld && batch > 0 && rows > 0 && obs_size > 0 && n_actions > 0 &&
+               hidden > 0, "global sampling layout arguments");
+  const GlobalLayout l = global_layout(rows, batch, obs_size, n_actions, hidden, world);
+  out->bytes = l.bytes;
+  out->slot_offset[0] = l.slot(0); out->slot_offset[1] = l.slot(1);
+  out->off_obs = l.off_obs; out->off_act = l.off_act; out->off_rew = l.off_rew; out->off_term = l.off_term;
+  out->off_states = l.off_states; out->off_leaf_idx = l.off_leaf; out->off_shard = l.off_shard;
+  out->off_is_weight = l.off_weight; out->off_uniforms = l.off_slot_uniforms;
+  return R2D2_OK;
+}
+int r2d2_replay_attach_group(r2d2_replay_t* r, int rank, int world, int batch, void* const* peer_bases,
+                             size_t buffer_bytes) {
+  return replay_attach_group(reinterpret_cast<Replay*>(r), rank, world, batch, peer_bases, buffer_bytes);
+}
+int r2d2_replay_global_write_back(r2d2_replay_t* r, int stage, const long long* leaf_idx, const int* shard,
+                                  const float* priority, r2d2_stream_t stream) {
+  return replay_global_write_back(reinterpret_cast<Replay*>(r), stage, leaf_idx, shard, priority, S(stream));
+}
+int r2d2_replay_global_draw(r2d2_replay_t* r, int stage, int slot, int weighted, float beta, r2d2_stream_t stream) {
+  return replay_global_draw(reinterpret_cast<Replay*>(r), stage, slot, weighted, beta, S(stream));
+}
+int r2d2_replay_global_status(r2d2_replay_t* r, int* status, r2d2_stream_t stream) {
+  return replay_global_status(reinterpret_cast<Replay*>(r), status, S(stream));
+}
+
 // ---- learner ----
 int r2d2_learner_create(r2d2_learner_t** out, const r2d2_learner_config* cfg) {
   return learner_create(reinterpret_cast<Learner**>(out), cfg);
@@ -332,6 +360,19 @@ int r2d2_learner_is_weights(r2d2_learner_t* lh, int slot, float** out) {
   R2D2_REQUIRE(lh && out && (slot == 0 || slot == 1), "batch slot");
   *out = reinterpret_cast<Learner*>(lh)->slots[slot].is_weight;
   return R2D2_OK;
+}
+int r2d2_learner_set_slot_buffers(r2d2_learner_t* lh, int slot, const r2d2_learner_buffers* b, float* is_weight) {
+  R2D2_REQUIRE(lh && b && is_weight && (slot == 0 || slot == 1), "batch slot buffers");
+  R2D2_REQUIRE(b->obs && b->act && b->rew && b->term && b->states && b->leaf_idx && b->uniforms, "null slot buffer");
+  Learner* l = reinterpret_cast<Learner*>(lh);
+  if (l->targets_slot >= 0 || l->c1_inputs_slot >= 0) {
+    set_last_error("a prefetched batch's chains are pending: move the batch slots before the first step");
+    return R2D2_ERR_STATE;
+  }
+  Learner::BatchSlot& s = l->slots[slot];
+  s.obs = b->obs; s.act = b->act; s.rew = b->rew; s.term = b->term; s.states = b->states;
+  s.leaf_idx = b->leaf_idx; s.uniforms = b->uniforms; s.is_weight = is_weight;
+  return learner_select_batch(l, l->cur_slot);
 }
 int r2d2_learner_set_importance_weighting(r2d2_learner_t* l, int on) {
   R2D2_REQUIRE(l, "null");

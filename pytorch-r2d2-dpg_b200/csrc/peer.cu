@@ -1,5 +1,6 @@
 // Gradient exchange over NVLink peer memory - see peer.cuh.
 #include "peer.cuh"
+#include "peer_sync.cuh"
 
 namespace r2d2 {
 
@@ -13,37 +14,11 @@ constexpr int kFlagStatus = 66;   // [1]      1 = a bounded wait expired
 // diagnostics (u64, byte offset 512): [0..1] ns the slice-sum kernel of block b waited for the peers' "gradients
 // complete", [2..3] ns it ran in total, [4..5] ns the wait kernel of block b waited for "slice delivered", [6] start stamp
 constexpr size_t kCounterBytes = 512;
-constexpr unsigned long long kSpinLimitNs = 4000000000ull;
 
-__device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_sys(unsigned* p, unsigned v) {
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
 __device__ __forceinline__ float4 ld_peer(const float4* p) {
   float4 v;
   asm volatile("ld.volatile.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
-}
-__device__ __forceinline__ unsigned long long global_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-// epochs only grow; a peer is at most one ahead
-__device__ __forceinline__ void spin_until(const unsigned* flag, unsigned value, unsigned* status) {
-  const unsigned long long t0 = global_ns();
-  if (*reinterpret_cast<volatile unsigned*>(status)) return;   // a wait already expired: the run is lost, do not stall it further
-  while ((int)(ld_acquire_sys(flag) - value) < 0) {
-    if (global_ns() - t0 > kSpinLimitNs) {
-      *status = 1u;
-      return;
-    }
-    __nanosleep(100);
-  }
 }
 
 __global__ void peer_signal_kernel(PeerPtrs p, int world, int rank, size_t off_word, unsigned value) {

@@ -12,21 +12,17 @@
 #include <map>
 #include <vector>
 
+#include "peer_sync.cuh"
 #include "replay.cuh"
 
 namespace r2d2 {
 
 namespace {
 
-// kLeafValue: also return the value of the drawn leaf (the weighted draw turns it into an importance weight)
+// Descent from the root with residual r: the leaf index, and in *v (kLeafValue) the drawn leaf's value.
 template <bool kLeafValue>
-__global__ void __launch_bounds__(256) tree_sample_kernel(TreeView tv, const float* __restrict__ u, int batch,
-                                                          long long* __restrict__ leaf, float* __restrict__ leaf_val) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= batch) return;
+__device__ __forceinline__ long long tree_descend(const TreeView& tv, float r, float* leaf_val) {
   const int top = tv.levels - 1;
-  const float total = tv.lvl[top][0];
-  float r = __fmul_rn(u[i], total);
   long long idx = 0;
   float v = 0.f;   // value of the picked child; after the level-1 pass that is the leaf itself
   for (int l = top; l >= 1; --l) {
@@ -56,8 +52,85 @@ __global__ void __launch_bounds__(256) tree_sample_kernel(TreeView tv, const flo
     }
     idx = idx * TREE_K + pick;
   }
-  leaf[i] = idx;
+  if (kLeafValue) *leaf_val = v;
+  return idx;
+}
+
+// kLeafValue: also return the value of the drawn leaf (the weighted draw turns it into an importance weight)
+template <bool kLeafValue>
+__global__ void __launch_bounds__(256) tree_sample_kernel(TreeView tv, const float* __restrict__ u, int batch,
+                                                          long long* __restrict__ leaf, float* __restrict__ leaf_val) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= batch) return;
+  const float total = tv.lvl[tv.levels - 1][0];
+  float v = 0.f;
+  leaf[i] = tree_descend<kLeafValue>(tv, __fmul_rn(u[i], total), &v);
   if (kLeafValue) leaf_val[i] = v;
+}
+
+// Global draw (one CTA): the W shard roots are one more tree level above the shards, in rank order.  Every rank
+// computes all W*B shard choices from the same totals and uniforms, so all ranks agree on the owner of every draw; the
+// owner descends its own tree only for its draws, writes (leaf, shard, leaf value) into consumer j / B's fill slot,
+// column j % B, and records the drawn leaf for the gather (-1 for the draws of other shards).  The walk over the roots
+// is tree_descend's walk over 32 children, with one difference in the rounding fallback: it takes the last non-empty
+// shard with the residual as it stood before that shard (the shard's own descent then clamps it), so that at W = 1 the
+// residual reaching the shard is u * total unchanged - today's draw bit for bit.
+template <bool kLeafValue>
+__global__ void __launch_bounds__(1024) global_draw_kernel(TreeView tv, GlobalPeers p, GlobalLayout lay, int world,
+                                                           int rank, int B, int slot, unsigned epoch) {
+  __shared__ float s_min[32];
+  char* own = p.base[rank];
+  unsigned* flags = reinterpret_cast<unsigned*>(own);
+  if ((int)threadIdx.x < world) spin_until(flags + kGlobalFlagTot + threadIdx.x, epoch, flags + kGlobalStatus);
+  __syncthreads();
+  const float* totals = reinterpret_cast<const float*>(own + kGlobalOffTotals);
+  const float* u = reinterpret_cast<const float*>(own + lay.off_uniforms);
+  long long* draw_leaf = reinterpret_cast<long long*>(own + lay.off_draw_leaf);
+  float root[kGlobalMaxWorld];
+  float total = 0.f;
+  for (int k = 0; k < world; ++k) { root[k] = *reinterpret_cast<const volatile float*>(totals + k); total = __fadd_rn(total, root[k]); }
+  float m = INFINITY;
+  for (int j = threadIdx.x; j < world * B; j += blockDim.x) {
+    const float r0 = __fmul_rn(*reinterpret_cast<const volatile float*>(u + j), total);
+    float r = r0;
+    int pick = -1;
+    for (int k = 0; k < world; ++k) {
+      if (pick < 0) {
+        if (r < root[k]) pick = k;
+        else r = __fsub_rn(r, root[k]);
+      }
+    }
+    if (pick < 0) {   // rounding pushed the residual past the last root: the last non-empty shard, residual before it
+      for (int k = 0; k < world; ++k)
+        if (root[k] > 0.f) pick = k;
+      if (pick < 0) pick = 0;
+      r = r0;
+      for (int k = 0; k < pick; ++k) r = __fsub_rn(r, root[k]);
+    }
+    if (pick != rank) { draw_leaf[j] = -1; continue; }
+    float v = 0.f;
+    const long long leaf = tree_descend<kLeafValue>(tv, r, &v);
+    draw_leaf[j] = leaf;
+    char* dst = p.base[j / B] + lay.slot(slot);
+    reinterpret_cast<long long*>(dst + lay.off_leaf)[j % B] = leaf;
+    reinterpret_cast<int*>(dst + lay.off_shard)[j % B] = rank;
+    if (kLeafValue) {
+      reinterpret_cast<float*>(dst + lay.off_weight)[j % B] = v;
+      if (v > 0.f) m = fminf(m, v);
+    }
+  }
+  if (kLeafValue) {   // the owner's minimum drawn leaf, sent with its delivery signal (global_deliver)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int k = 1; k < (int)(blockDim.x >> 5); ++k) m = fminf(m, s_min[k]);
+      *reinterpret_cast<float*>(own + kGlobalOffOwnMin) = fminf(m, s_min[0]);
+    }
+  } else if (threadIdx.x == 0) {
+    *reinterpret_cast<float*>(own + kGlobalOffOwnMin) = INFINITY;
+  }
 }
 
 // Leaf stored for a priority p under the exponent alpha.  Zero stays zero (rows that start no sequence must stay
@@ -107,26 +180,43 @@ __device__ __forceinline__ float node_sum(const float* __restrict__ children) {
 // executes the writes in batch order), then refresh every ancestor level by level.  The leaf indices sit in shared
 // memory: the last-writer test is a broadcast scan of the later entries (B^2 / 2 shared reads instead of global ones).
 // kExponent: the shard stores p^alpha (r2d2_replay_set_priority_exponent); without it the leaf is prio[i] as given.
-template <bool kExponent>
+// kShardFilter (global sampling): the batch is the W*B records of all ranks in global-index order, published into
+// this rank's exchange block; the kernel first waits for every rank's "records published" flag (`flags` + world words,
+// `epoch`, expiry -> *status), then applies only the records whose shard is `owner` (the others take part as -1).
+template <bool kExponent, bool kShardFilter = false>
 __global__ void __launch_bounds__(1024) tree_update_kernel(TreeView tv, const long long* __restrict__ leaf,
-                                                           const float* __restrict__ prio, int batch, float alpha) {
+                                                           const float* __restrict__ prio, int batch, float alpha,
+                                                           const int* __restrict__ shard = nullptr, int owner = 0,
+                                                           const unsigned* flags = nullptr, int world = 0,
+                                                           unsigned epoch = 0, unsigned* status = nullptr) {
   extern __shared__ long long s_leaf[];
-  for (int i = threadIdx.x; i < batch; i += blockDim.x) s_leaf[i] = leaf[i];
+  if (kShardFilter) {
+    if ((int)threadIdx.x < world) spin_until(flags + threadIdx.x, epoch, status);
+    __syncthreads();
+  }
+  for (int i = threadIdx.x; i < batch; i += blockDim.x) {
+    if (kShardFilter) s_leaf[i] = *reinterpret_cast<const volatile int*>(shard + i) == owner
+                                      ? *reinterpret_cast<const volatile long long*>(leaf + i) : -1;
+    else s_leaf[i] = leaf[i];
+  }
   __syncthreads();
   for (int i = threadIdx.x; i < batch; i += blockDim.x) {
     const long long li = s_leaf[i];
+    if (kShardFilter && li < 0) continue;
     bool winner = true;
     for (int j = i + 1; j < batch; ++j)
       if (s_leaf[j] == li) { winner = false; break; }
     if (winner) {
-      if (kExponent) tv.lvl[0][li] = raise_priority(prio[i], alpha);
-      else tv.lvl[0][li] = prio[i];
+      const float p = kShardFilter ? *reinterpret_cast<const volatile float*>(prio + i) : prio[i];
+      if (kExponent) tv.lvl[0][li] = raise_priority(p, alpha);
+      else tv.lvl[0][li] = p;
     }
   }
   __syncthreads();
   long long div = TREE_K;
   for (int l = 1; l < tv.levels; ++l) {
     for (int i = threadIdx.x; i < batch; i += blockDim.x) {
+      if (kShardFilter && s_leaf[i] < 0) continue;
       const long long node = s_leaf[i] / div;
       tv.lvl[l][node] = node_sum(tv.lvl[l - 1] + node * TREE_K);
     }
@@ -148,11 +238,16 @@ __global__ void __launch_bounds__(256) tree_recompute_range_kernel(TreeView tv, 
 // lane-contiguous accesses (16-byte vectors when the row width is a multiple of 4 floats: a row start is then 16-byte
 // aligned in both the shard and the batch), lane 0 moves the reward / terminal scalars.  Tasks >= T*B move the stored
 // recurrent states: task T*B + nh*B + b copies state_rows[leaf[b]][nh][:] to out[nh][b][:].  No division per element.
+// kPerDraw (global sampling): B counts the W*Bc global draws; draw b goes to rank b / Bc's slot (dst_base[b / Bc] plus
+// the slot offsets), column b % Bc, and draws with leaf[b] < 0 belong to another shard and are skipped.
 struct GatherParams {
   const float *obs_rows, *act_rows, *rew_rows, *term_rows, *state_rows;
   const long long* leaf;
   float *obs, *act, *rew, *term, *states;
   int T, B, O, A, H;
+  int Bc;
+  size_t off_obs, off_act, off_rew, off_term, off_states;
+  GlobalPeers dst;
 };
 
 __device__ __forceinline__ void warp_copy_row(const float* __restrict__ src, float* __restrict__ dst, int n, int lane) {
@@ -165,6 +260,7 @@ __device__ __forceinline__ void warp_copy_row(const float* __restrict__ src, flo
   }
 }
 
+template <bool kPerDraw = false>
 __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
@@ -174,17 +270,30 @@ __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
   int t = (int)(warp0 / g.B), b = (int)(warp0 % g.B);                    // one division per warp, then carried
   const int dt = (int)(n_warps / g.B), db = (int)(n_warps % g.B);
   for (long long task = warp0; task < total; task += n_warps) {
-    if (task < row_tasks) {
-      const long long r = g.leaf[b] + t;
-      const long long o = (long long)t * g.B + b;
-      if (g.obs) warp_copy_row(g.obs_rows + r * g.O, g.obs + o * g.O, g.O, lane);
-      if (g.act) warp_copy_row(g.act_rows + r * g.A, g.act + o * g.A, g.A, lane);
+    // destination of draw b: the batch's own buffers, column b of B; per draw, rank b / Bc's slot, column b % Bc
+    const long long leaf = g.leaf[b];
+    float *obs = g.obs, *act = g.act, *rew = g.rew, *term = g.term, *states = g.states;
+    int col = b, ld = g.B;
+    if (kPerDraw) {
+      char* d = g.dst.base[b / g.Bc];
+      obs = reinterpret_cast<float*>(d + g.off_obs); act = reinterpret_cast<float*>(d + g.off_act);
+      rew = reinterpret_cast<float*>(d + g.off_rew); term = reinterpret_cast<float*>(d + g.off_term);
+      states = reinterpret_cast<float*>(d + g.off_states);
+      col = b % g.Bc; ld = g.Bc;
+    }
+    if (kPerDraw && leaf < 0) {
+      // another shard's draw
+    } else if (task < row_tasks) {
+      const long long r = leaf + t;
+      const long long o = (long long)t * ld + col;
+      if (obs) warp_copy_row(g.obs_rows + r * g.O, obs + o * g.O, g.O, lane);
+      if (act) warp_copy_row(g.act_rows + r * g.A, act + o * g.A, g.A, lane);
       if (lane == 0) {
-        if (g.rew) g.rew[o] = __ldg(g.rew_rows + r);
-        if (g.term) g.term[o] = __ldg(g.term_rows + r);
+        if (rew) rew[o] = __ldg(g.rew_rows + r);
+        if (term) term[o] = __ldg(g.term_rows + r);
       }
     } else {
-      warp_copy_row(g.state_rows + (g.leaf[b] * 8 + (t - g.T)) * g.H, g.states + ((long long)(t - g.T) * g.B + b) * g.H, g.H, lane);
+      warp_copy_row(g.state_rows + (leaf * 8 + (t - g.T)) * g.H, states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
     }
     t += dt; b += db;
     if (b >= g.B) { b -= g.B; ++t; }
@@ -221,6 +330,15 @@ struct Replay {
   long long rows_used = 0;
   long long evicted_total = 0;
   float alpha = 1.0f;   // priority exponent: leaves hold p^alpha (1 = the raw priority, no pow on any path)
+  struct Group {        // global sampling (r2d2_replay_attach_group)
+    int rank = 0, world = 1, batch = 0;
+    GlobalPeers peers{};
+    GlobalLayout lay;
+    unsigned wb_epoch = 0, draw_epoch = 0;
+    int wb_stage = 0, draw_stage = 0;   // next stage of the write-back / draw that is in progress
+    bool drawn_since_wb = true;         // a write-back needs a draw since the last one (the record block is reused)
+  };
+  Group* group = nullptr;
 };
 
 static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leaves, cudaStream_t stream) {
@@ -301,6 +419,7 @@ int replay_destroy(Replay* r) {
   if (!r) return R2D2_OK;
   cudaFree(r->obs_rows); cudaFree(r->act_rows); cudaFree(r->rew_rows); cudaFree(r->term_rows); cudaFree(r->state_rows);
   for (float* p : r->level_alloc) cudaFree(p);
+  delete r->group;
   delete r;
   return R2D2_OK;
 }
@@ -473,7 +592,7 @@ int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, f
     g.obs = obs; g.act = act; g.rew = rew; g.term = term; g.states = states;
     g.T = T; g.B = batch; g.O = O; g.A = A; g.H = H;
     const long long tasks = (long long)T * batch + (states ? (long long)8 * batch : 0);
-    gather_batch_kernel<<<grid_for(tasks * 32), 256, 0, stream>>>(g);
+    gather_batch_kernel<false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
     count_launch();
   }
   R2D2_CUDA_TRY(cudaGetLastError());
@@ -554,6 +673,163 @@ int replay_tree_level(Replay* r, int level, const float** dev_ptr, long long* n)
   R2D2_REQUIRE(r && level >= 0 && level < r->tv.levels, "level");
   *dev_ptr = r->tv.lvl[level];
   *n = r->tv.n[level];
+  return R2D2_OK;
+}
+
+GlobalLayout global_layout(int T, int B, int O, int A, int H, int world) {
+  GlobalLayout l;
+  const size_t n = (size_t)world * B;
+  auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+  size_t off = 512;
+  l.off_uniforms = off; off = up(off + sizeof(float) * n);
+  l.off_rec_leaf = off; off = up(off + sizeof(long long) * n);
+  l.off_rec_shard = off; off = up(off + sizeof(int) * n);
+  l.off_rec_prio = off; off = up(off + sizeof(float) * n);
+  l.off_draw_leaf = off; off = up(off + sizeof(long long) * n);
+  l.exchange_bytes = off;
+  off = 0;
+  l.off_obs = off; off = up(off + sizeof(float) * (size_t)T * B * O);
+  l.off_act = off; off = up(off + sizeof(float) * (size_t)T * B * A);
+  l.off_rew = off; off = up(off + sizeof(float) * (size_t)T * B);
+  l.off_term = off; off = up(off + sizeof(float) * (size_t)T * B);
+  l.off_states = off; off = up(off + sizeof(float) * (size_t)8 * B * H);
+  l.off_leaf = off; off = up(off + sizeof(long long) * B);
+  l.off_shard = off; off = up(off + sizeof(int) * B);
+  l.off_weight = off; off = up(off + sizeof(float) * B);
+  l.off_slot_uniforms = off; off = up(off + sizeof(float) * B);
+  l.slot_bytes = off;
+  l.bytes = l.exchange_bytes + 2 * l.slot_bytes;
+  return l;
+}
+
+int replay_attach_group(Replay* r, int rank, int world, int batch, void* const* peer_bases, size_t buffer_bytes) {
+  R2D2_REQUIRE(r && peer_bases, "null argument");
+  R2D2_REQUIRE(world >= 1 && world <= kGlobalMaxWorld && rank >= 0 && rank < world, "global sampling rank / world");
+  R2D2_REQUIRE(batch > 0 && (long long)world * batch <= 5120,
+               "global batch W * B must lie in [1, 5120] (the write-back's shared-memory index table)");
+  R2D2_REQUIRE(!r->group, "replay shard already attached to a group");
+  Replay::Group* g = new Replay::Group();
+  g->rank = rank; g->world = world; g->batch = batch;
+  g->lay = global_layout(r->rows_per_window, batch, r->cfg.obs_size, r->cfg.n_actions, r->cfg.hidden, world);
+  if (buffer_bytes != g->lay.bytes) {   // the buffers were laid out for another shape: peer stores would miss
+    delete g;
+    set_last_error("global sampling buffer size does not match this shard's layout (rows, obs, act, hidden, batch, "
+                   "world): the engine and the replay shard disagree");
+    return R2D2_ERR_ARG;
+  }
+  for (int k = 0; k < world; ++k) {
+    if (!peer_bases[k]) { delete g; R2D2_REQUIRE(false, "null peer buffer"); }
+    g->peers.base[k] = static_cast<char*>(peer_bases[k]);
+  }
+  r->group = g;
+  return R2D2_OK;
+}
+
+// stage 0: publish this rank's B records into every rank's exchange block; stage 1: wait for every rank's records and
+// apply those that land in this shard (highest global index wins); -1: both.
+int replay_global_write_back(Replay* r, int stage, const long long* leaf, const int* shard, const float* prio,
+                             cudaStream_t stream) {
+  R2D2_REQUIRE(r && r->group, "replay shard is not attached to a group");
+  R2D2_REQUIRE(stage >= -1 && stage <= 1, "write-back stage is 0, 1 or -1 (both)");
+  Replay::Group& g = *r->group;
+  if (stage <= 0) {
+    R2D2_REQUIRE(leaf && shard && prio, "null record");
+    if (g.wb_stage != 0 || !g.drawn_since_wb) {
+      set_last_error("a global write-back needs a global draw since the previous one, and its stages in order");
+      return R2D2_ERR_STATE;
+    }
+    g.wb_epoch += 1;
+    R2D2_TRY(global_publish_records(g.peers, g.lay, g.world, g.rank, g.batch, leaf, shard, prio, g.wb_epoch, stream));
+    g.wb_stage = 1;
+    g.drawn_since_wb = false;
+  }
+  if (stage == 1 || stage == -1) {
+    if (g.wb_stage != 1) { set_last_error("write-back stage 1 before stage 0"); return R2D2_ERR_STATE; }
+    char* own = g.peers.base[g.rank];
+    const int n = g.world * g.batch;
+    const long long* rl = reinterpret_cast<const long long*>(own + g.lay.off_rec_leaf);
+    const int* rs = reinterpret_cast<const int*>(own + g.lay.off_rec_shard);
+    const float* rp = reinterpret_cast<const float*>(own + g.lay.off_rec_prio);
+    unsigned* flags = reinterpret_cast<unsigned*>(own);
+    const size_t smem = sizeof(long long) * (size_t)n;
+    if (r->alpha == 1.0f)
+      tree_update_kernel<false, true><<<1, 1024, smem, stream>>>(r->tv, rl, rp, n, 1.0f, rs, g.rank, flags + kGlobalFlagPub,
+                                                                 g.world, g.wb_epoch, flags + kGlobalStatus);
+    else
+      tree_update_kernel<true, true><<<1, 1024, smem, stream>>>(r->tv, rl, rp, n, r->alpha, rs, g.rank, flags + kGlobalFlagPub,
+                                                                g.world, g.wb_epoch, flags + kGlobalStatus);
+    count_launch();
+    R2D2_CUDA_TRY(cudaGetLastError());
+    g.wb_stage = 0;
+  }
+  return R2D2_OK;
+}
+
+// stage 0: publish this shard's root and this rank's B uniforms (fill slot `slot`) to every rank; stage 1: wait for
+// every rank's root, draw all W*B, gather this shard's draws into the consumers' slots and signal delivery; stage 2:
+// wait for every owner's delivery and form the importance weights; -1: all three.
+int replay_global_draw(Replay* r, int stage, int slot, int weighted, float beta, cudaStream_t stream) {
+  R2D2_REQUIRE(r && r->group, "replay shard is not attached to a group");
+  R2D2_REQUIRE(stage >= -1 && stage <= 2, "draw stage is 0, 1, 2 or -1 (all)");
+  R2D2_REQUIRE(slot == 0 || slot == 1, "batch slot");
+  R2D2_REQUIRE(weighted == 0 || weighted == 1, "weighted is 0 or 1");
+  R2D2_REQUIRE(beta >= 0.f && beta <= 1.f, "importance-sampling exponent must lie in [0, 1]");
+  Replay::Group& g = *r->group;
+  const bool all = stage == -1;
+  if (all || stage == 0) {
+    if (g.draw_stage != 0 || g.wb_stage != 0) {
+      set_last_error("a global draw needs the previous draw and write-back complete, and its stages in order");
+      return R2D2_ERR_STATE;
+    }
+    g.draw_epoch += 1;
+    R2D2_TRY(global_publish_root(g.peers, g.lay, g.world, g.rank, g.batch, slot, r->tv.lvl[r->tv.levels - 1],
+                                 g.draw_epoch, stream));
+    g.draw_stage = 1;
+  }
+  if (all || stage == 1) {
+    if (g.draw_stage != 1) { set_last_error("draw stage 1 out of order"); return R2D2_ERR_STATE; }
+    if (weighted)
+      global_draw_kernel<true><<<1, 1024, 0, stream>>>(r->tv, g.peers, g.lay, g.world, g.rank, g.batch, slot, g.draw_epoch);
+    else
+      global_draw_kernel<false><<<1, 1024, 0, stream>>>(r->tv, g.peers, g.lay, g.world, g.rank, g.batch, slot, g.draw_epoch);
+    count_launch();
+    R2D2_CUDA_TRY(cudaGetLastError());
+    GatherParams gp;
+    gp.obs_rows = r->obs_rows; gp.act_rows = r->act_rows; gp.rew_rows = r->rew_rows; gp.term_rows = r->term_rows;
+    gp.state_rows = r->state_rows;
+    char* own = g.peers.base[g.rank];
+    gp.leaf = reinterpret_cast<const long long*>(own + g.lay.off_draw_leaf);
+    gp.obs = gp.act = gp.rew = gp.term = nullptr;
+    gp.states = reinterpret_cast<float*>(own + g.lay.slot(slot) + g.lay.off_states);   // non-null: state tasks run
+    gp.T = r->rows_per_window; gp.B = g.world * g.batch; gp.O = r->cfg.obs_size; gp.A = r->cfg.n_actions;
+    gp.H = r->cfg.hidden; gp.Bc = g.batch;
+    const size_t so = g.lay.slot(slot);
+    gp.off_obs = so + g.lay.off_obs; gp.off_act = so + g.lay.off_act; gp.off_rew = so + g.lay.off_rew;
+    gp.off_term = so + g.lay.off_term; gp.off_states = so + g.lay.off_states;
+    gp.dst = g.peers;
+    const long long tasks = (long long)(gp.T + 8) * gp.B;
+    gather_batch_kernel<true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
+    count_launch();
+    R2D2_CUDA_TRY(cudaGetLastError());
+    R2D2_TRY(global_deliver(g.peers, g.world, g.rank, g.draw_epoch, stream));
+    g.draw_stage = 2;
+  }
+  if (all || stage == 2) {
+    if (g.draw_stage != 2) { set_last_error("draw stage 2 out of order"); return R2D2_ERR_STATE; }
+    R2D2_TRY(global_receive(g.peers, g.lay, g.world, g.rank, g.batch, slot, weighted != 0, beta, g.draw_epoch, stream));
+    g.draw_stage = 0;
+    g.drawn_since_wb = true;
+  }
+  return R2D2_OK;
+}
+
+int replay_global_status(Replay* r, int* out, cudaStream_t stream) {
+  R2D2_REQUIRE(r && r->group && out, "replay shard is not attached to a group");
+  unsigned v = 0;
+  R2D2_CUDA_TRY(cudaMemcpyAsync(&v, r->group->peers.base[r->group->rank] + sizeof(unsigned) * kGlobalStatus,
+                                sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
+  *out = (int)v;
   return R2D2_OK;
 }
 

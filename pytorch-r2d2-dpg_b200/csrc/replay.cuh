@@ -12,6 +12,36 @@ struct TreeView {
   int levels;
 };
 
+// Global sampling over the replay shards of W data-parallel ranks (include/r2d2_b200.h, r2d2_replay_attach_group).
+// Every rank owns one buffer of `GlobalLayout::bytes` that every rank maps: an exchange block
+//   [ flags 256 B | totals [16] | minima [16] | own min | uniforms [W*B] | records: leaf [W*B], shard [W*B], prio [W*B]
+//     | drawn leaf per global draw (-1: another shard's) [W*B] ]
+// and the rank's two batch slots (obs, act, rew, term, states, leaf_idx, shard, is_weight, uniforms), which the owners
+// of the drawn rows write with peer stores.  Global draw j = c*B + b is trained by rank c in column b.
+constexpr int kGlobalMaxWorld = 16;
+constexpr int kGlobalFlagPub = 0, kGlobalFlagTot = 16, kGlobalFlagDel = 32, kGlobalStatus = 48;   // uint32 words
+constexpr size_t kGlobalOffTotals = 256, kGlobalOffMinima = 320, kGlobalOffOwnMin = 384;
+
+struct GlobalLayout {
+  size_t bytes = 0, exchange_bytes = 0, slot_bytes = 0;
+  size_t off_uniforms = 0, off_rec_leaf = 0, off_rec_shard = 0, off_rec_prio = 0, off_draw_leaf = 0;   // exchange
+  size_t off_obs = 0, off_act = 0, off_rew = 0, off_term = 0, off_states = 0, off_leaf = 0, off_shard = 0,
+         off_weight = 0, off_slot_uniforms = 0;                                                        // in a slot
+  __host__ __device__ size_t slot(int s) const { return exchange_bytes + (size_t)s * slot_bytes; }
+};
+GlobalLayout global_layout(int T, int B, int O, int A, int H, int world);
+
+struct GlobalPeers { char* base[kGlobalMaxWorld]; };
+
+// exchange kernels (global_replay.cu)
+int global_publish_records(const GlobalPeers& p, const GlobalLayout& lay, int world, int rank, int B,
+                           const long long* leaf, const int* shard, const float* prio, unsigned epoch, cudaStream_t st);
+int global_publish_root(const GlobalPeers& p, const GlobalLayout& lay, int world, int rank, int B, int slot,
+                        const float* root, unsigned epoch, cudaStream_t st);
+int global_deliver(const GlobalPeers& p, int world, int rank, unsigned epoch, cudaStream_t st);
+int global_receive(const GlobalPeers& p, const GlobalLayout& lay, int world, int rank, int B, int slot, bool weighted,
+                   float beta, unsigned epoch, cudaStream_t st);
+
 struct Replay;
 int replay_create(Replay** out, const r2d2_replay_config* cfg);
 int replay_destroy(Replay* r);
@@ -33,5 +63,10 @@ int replay_update_priorities(Replay* r, const long long* leaf_idx, const float* 
 int replay_stats(Replay* r, r2d2_replay_stats_t* out, cudaStream_t stream);
 int replay_decode(Replay* r, const long long* leaf_host, int n, long long* episode_index, long long* sequence_index);
 int replay_tree_level(Replay* r, int level, const float** dev_ptr, long long* n);
+int replay_attach_group(Replay* r, int rank, int world, int batch, void* const* peer_bases, size_t buffer_bytes);
+int replay_global_write_back(Replay* r, int stage, const long long* leaf, const int* shard, const float* prio,
+                             cudaStream_t stream);
+int replay_global_draw(Replay* r, int stage, int slot, int weighted, float beta, cudaStream_t stream);
+int replay_global_status(Replay* r, int* out, cudaStream_t stream);
 
 }  // namespace r2d2

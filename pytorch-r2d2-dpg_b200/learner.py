@@ -16,7 +16,11 @@ rank 0 alone writes model.pt.  Nothing else crosses GPUs.
 
 Prioritized replay (R2D2's, absent from the reference): R2D2_PRIORITY_EXPONENT (alpha, default 1) and R2D2_IS_EXPONENT
 (beta, default 0) in the environment.  The defaults are the reference's behaviour; published R2D2 uses 0.9 / 0.6.
-Under data parallelism each rank normalises the weights over its own batch.
+Under data parallelism each rank normalises the weights over its own batch, and draws from its own shard - unless
+R2D2_GLOBAL_SAMPLING=1 (default 0): then the ranks draw one global batch of WORLD_SIZE * batch sequences from the union
+of the shards in proportion to p^alpha, as the reference's single replay does, every rank trains on its B of them and the
+weights are normalised over the global batch (the kernels of csrc/global_replay.cu and csrc/replay.cu, in the learner's
+stream; the batch slots live in torch symmetric memory).  A host barrier follows every ingest in that mode.
 
 Optimiser step: R2D2_TARGET_TAU (Polyak weight tau of the target update, default 1 = the reference's hard copy),
 R2D2_TARGET_INTERVAL (iterations between target updates, default 500 = the reference's target_update_inverval; DDPG-style
@@ -106,7 +110,8 @@ class Learner:
                          target_interval=self.target_update_inverval, priority_exponent=self.priority_exponent,
                          is_exponent=self.is_exponent, target_tau=self.target_tau, grad_clip_norm=self.grad_clip_norm,
                          value_rescaling=self.td_options.value_rescaling, rescaling_eps=self.td_options.rescaling_eps,
-                         priority_metric=self.td_options.priority_metric, **self.td3_options)
+                         priority_metric=self.td_options.priority_metric, **self.td3_options,
+                         global_sampling=self._global_sampling_from_environ())
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
@@ -116,6 +121,13 @@ class Learner:
         if os.environ.get("R2D2_RESUME", "0") == "1" and os.path.isfile(self.state_path):
             self.load_checkpoint()                         # every rank loads the same file: replicas stay identical
         self.save_model()
+
+    @staticmethod
+    def _global_sampling_from_environ():
+        v = os.environ.get("R2D2_GLOBAL_SAMPLING", "0")
+        if v not in ("0", "1"):
+            raise ValueError("R2D2_GLOBAL_SAMPLING must be 0 or 1, got {!r}".format(v))
+        return v == "1"
 
     def save_checkpoint(self):
         """Resumable state next to model.pt: nets + both Adam moment sets + step counter (the reference's model.pt has
@@ -171,6 +183,18 @@ class Learner:
             if self.dist_env.is_main:
                 print('learning step:', step)
 
+        ingest = self._ingest
+        if self.engine.cfg.global_sampling:
+            # every draw waits (bounded) for every rank's shard root: the ranks enter the loop together, and a slow
+            # rank's file ingest must not leave its peers' draw kernels spinning - a host barrier after each ingest
+            if self.memory._dev.group is None:                   # a second run() keeps the first one's group
+                self.memory._dev.attach_group(self.engine)
+            barrier = self.engine._dist.barrier if self.engine._dist is not None else (lambda: None)
+            barrier()
+
+            def ingest():
+                self._ingest()
+                barrier()
         run_learner_loop(self.engine, self.memory._dev, max_steps=max_steps, ingest_every=self.memory_update_interval,
-                         save_every=self.model_save_interval, ingest=self._ingest, save=save, log=log)
+                         save_every=self.model_save_interval, ingest=ingest, save=save, log=log)
         torch.cuda.synchronize()

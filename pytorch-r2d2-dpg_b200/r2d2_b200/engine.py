@@ -47,7 +47,12 @@ class PathConfig:
     TD3's target (include/r2d2_b200.h, r2d2_learner_options): `twin_critic` adds a second critic and target critic and
     bootstraps from the minimum of the two target critics; `target_noise` sigma >= 0 (0 = off) smooths the target actor's
     actions with clip(sigma z, -c, c), c = `target_noise_clip` > 0, z keyed on (`target_noise_seed`, rank) and the
-    iteration index.  TD3's usual setting: twin, sigma 0.2, c 0.5, target_tau 0.005 at target_interval 1."""
+    iteration index.  TD3's usual setting: twin, sigma 0.2, c 0.5, target_tau 0.005 at target_interval 1.
+
+    `global_sampling` (data parallel, off by default): the W ranks draw one global batch of W * B sequences from the
+    union of their replay shards in proportion to the stored leaves p^alpha, and rank c trains on global draws
+    c*B .. c*B+B-1 (DeviceReplay.attach_group).  The engine's batch slots then live in memory every rank maps; at W = 1
+    the draws, batches and weights are the local mode's bit for bit."""
     obs: int
     act: int
     hidden: int = 128
@@ -71,6 +76,7 @@ class PathConfig:
     target_noise: float = 0.0
     target_noise_clip: float = 0.5
     target_noise_seed: int = 0
+    global_sampling: bool = False
 
     def __post_init__(self):
         for name, least in (("burn_in", 0), ("learning", 2), ("n_step", 1)):
@@ -80,8 +86,9 @@ class PathConfig:
                     name, least, v, " (the priority series [b:-1:B] of the last batch element drops its last TD step, "
                                     "so a one-step window leaves it empty)" if name == "learning" else ""))
         td_options.validate(self.value_rescaling, self.rescaling_eps, self.priority_metric)
-        if not isinstance(self.twin_critic, bool):
-            raise ValueError("twin_critic must be True or False, got %r" % (self.twin_critic,))
+        for name in ("twin_critic", "global_sampling"):
+            if not isinstance(getattr(self, name), bool):
+                raise ValueError("%s must be True or False, got %r" % (name, getattr(self, name)))
         for name, lo_ok in (("target_noise", lambda v: v >= 0.0), ("target_noise_clip", lambda v: v > 0.0)):
             v = getattr(self, name)
             if isinstance(v, bool) or not isinstance(v, numbers.Real) or not (math.isfinite(v) and lo_ok(v)):
@@ -245,6 +252,52 @@ class LearnerEngine:
         self._peer_buf = None
         self._peer_hdl = None
         self._sync_actor = None
+        # global sampling: both batch slots move into one buffer per rank that every rank maps (here a plain one for a
+        # single rank; enable_data_parallel replaces it by symmetric memory); off, the slots stay in the library's arena
+        self._global_buf = self._global_hdl = None
+        self.global_peer_ptrs = None
+        if cfg.global_sampling:
+            lay = self.global_layout(1)
+            self.use_global_slots(torch.zeros(int(lay.bytes) // 4, dtype=torch.float32, device=self.device), lay)
+            self.global_peer_ptrs = [self._global_buf.data_ptr()]
+
+    def global_layout(self, world: int):
+        """Bytes and offsets of one rank's global-sampling buffer (exchange block + two batch slots) at `world` ranks."""
+        c = self.cfg
+        lay = nv.GlobalLayout()
+        nv.check(self.lib.r2d2_global_layout_for(c.rows, c.batch, c.obs, c.act, c.hidden, int(world), byref(lay)))
+        return lay
+
+    def use_global_slots(self, buf: torch.Tensor, lay):
+        """Move both batch slots into `buf` (a zeroed float32 CUDA tensor of lay.bytes, laid out by global_layout): the
+        replay shards of every rank store the drawn rows straight into them.  Only before the first step."""
+        T, B, O, A, H = self.cfg.rows, self.cfg.batch, self.cfg.obs, self.cfg.act, self.cfg.hidden
+        base, dev = buf.data_ptr(), self.device
+        for slot in (0, 1):
+            so = base + int(lay.slot_offset[slot])
+            b = nv.LearnerBuffers()
+            b.obs, b.act, b.rew, b.term = so + lay.off_obs, so + lay.off_act, so + lay.off_rew, so + lay.off_term
+            b.states, b.leaf_idx, b.uniforms = so + lay.off_states, so + lay.off_leaf_idx, so + lay.off_uniforms
+            nv.check(self.lib.r2d2_learner_set_slot_buffers(self._h, slot, byref(b), c_void_p(so + lay.off_is_weight)))
+            self._slots[slot] = {"obs": nv.view_f32(b.obs, (T, B, O), dev), "act": nv.view_f32(b.act, (T, B, A), dev),
+                                 "rew": nv.view_f32(b.rew, (T, B), dev), "term": nv.view_f32(b.term, (T, B), dev),
+                                 "states": nv.view_f32(b.states, (4, 2, B, H), dev),
+                                 "leaf_idx": nv.view_i64(b.leaf_idx, (B,), dev),
+                                 "uniforms": nv.view_f32(b.uniforms, (B,), dev),
+                                 "is_weight": nv.view_f32(so + lay.off_is_weight, (B,), dev),
+                                 "shard": torch.as_tensor(nv._RawView(so + lay.off_shard, (B,), "<i4"), device=dev)}
+            self._slots[slot]["is_weight"].fill_(1.0)
+        self._global_buf = buf
+        self._global_bytes = int(lay.bytes)
+        self._bind_slot(self._fill_slot)
+
+    def shard_of(self, leaf_idx: torch.Tensor) -> torch.Tensor:
+        """The shard ids [B] (int32) next to a slot's leaf indices (global sampling)."""
+        for s in self._slots:
+            if "shard" in s and s["leaf_idx"].data_ptr() == leaf_idx.data_ptr():
+                return s["shard"]
+        raise nv.NativeError("global sampling writes back a batch slot's own leaf indices (engine.leaf_idx of the "
+                             "trained batch); these are not a slot's")
 
     @property
     def td_options(self) -> td_options.TdOptions:
@@ -377,6 +430,8 @@ class LearnerEngine:
                 self.set_target_smoothing()
             if self._dp_mode == "peer":
                 self._attach_peers(dist)
+            if self.cfg.global_sampling:
+                self._attach_global_slots(dist)
             # both modes defer phase 3: the actor's weights are final only after it ran
             nv.check(self.lib.r2d2_learner_set_overlap_actor_inputs(self._h, 0))
             for net in ("actor", "critic", "target_actor", "target_critic"):
@@ -422,6 +477,33 @@ class LearnerEngine:
         na, nc = self.grads["actor"].numel(), self.grads["critic"].numel()
         oc, oa = int(lay.off_critic_grads) // 4, int(lay.off_actor_grads) // 4
         self.grads = {"actor": buf[oa:oa + na], "critic": buf[oc:oc + nc]}
+
+    def _attach_global_slots(self, dist):
+        """Global sampling: the batch slots and the exchange block in torch symmetric memory, one buffer per rank mapped
+        by every rank of the node.  All ranks agree on the outcome (an all-reduce, as _attach_peers does) and raise
+        together: there is no fallback, without peer mappings the option cannot run."""
+        ok, why, buf, hdl, ptrs = 1, "", None, None, None
+        lay = self.global_layout(self.world)
+        try:
+            import torch.distributed._symmetric_memory as symm
+            buf = symm.empty(int(lay.bytes) // 4, dtype=torch.float32, device=self.device)
+            buf.zero_()
+            hdl = symm.rendezvous(buf, dist.group.WORLD.group_name)
+            ptrs = [int(p) for p in hdl.buffer_ptrs]
+            if len(ptrs) != self.world or ptrs[dist.get_rank()] != buf.data_ptr():
+                raise RuntimeError("the symmetric-memory handle does not match the process group")
+        except Exception as e:  # noqa: BLE001 - any failure on any rank stops every rank
+            ok, why = 0, repr(e)[:200]
+        agreed = torch.tensor([ok], dtype=torch.int32, device=self.device)
+        dist.all_reduce(agreed, op=dist.ReduceOp.MIN)
+        if int(agreed.item()) == 0:
+            raise nv.NativeError("global sampling needs a buffer every rank maps (torch symmetric memory): "
+                                 + (why or "another rank failed to set it up"))
+        self.use_global_slots(buf, lay)
+        torch.cuda.synchronize(self.device)
+        dist.barrier()                                   # every rank's flag words are zero before anyone signals
+        self._global_hdl = hdl
+        self.global_peer_ptrs = ptrs
 
     def peer_status(self) -> int:
         """0, or 1 when a bounded wait for a peer's flag expired inside the gradient-exchange kernels."""
@@ -606,6 +688,64 @@ class DeviceReplay:
         nv.check(self.lib.r2d2_replay_create(byref(self._h), byref(rc)))
         if cfg.priority_exponent != 1.0:   # leaves hold p^alpha; actors and write-backs keep passing raw priorities
             nv.check(self.lib.r2d2_replay_set_priority_exponent(self._h, float(cfg.priority_exponent)))
+        self._group = None                 # the engine whose rank / world / buffers global sampling uses
+
+    def attach_group(self, eng: LearnerEngine):
+        """Global sampling: this shard becomes rank eng's shard of the group of eng.world ranks; from then on
+        sample_into draws the rank's B sequences of one W*B global batch from all shards, and update_priorities writes
+        the trained batch's priorities back into the shards that own its rows (a collective: every rank calls both, in
+        the same order).  The engine needs PathConfig.global_sampling."""
+        if not eng.cfg.global_sampling or eng.global_peer_ptrs is None:
+            raise nv.NativeError("attach_group needs an engine with PathConfig.global_sampling")
+        ec, rc = eng.cfg, self.cfg
+        if (ec.obs, ec.act, ec.hidden, ec.rows) != (rc.obs, rc.act, rc.hidden, rc.rows):
+            raise nv.NativeError("replay shard (obs %d act %d hidden %d rows %d) does not match the engine (obs %d act %d "
+                                 "hidden %d rows %d)" % (rc.obs, rc.act, rc.hidden, rc.rows, ec.obs, ec.act, ec.hidden, ec.rows))
+        arr = (c_void_p * eng.world)(*eng.global_peer_ptrs)
+        nv.check(self.lib.r2d2_replay_attach_group(self._h, eng._rank, eng.world, ec.batch, arr, eng._global_bytes))
+        self._group = eng
+
+    @property
+    def group(self):
+        """The engine this shard samples globally for (attach_group), or None."""
+        return self._group
+
+    def global_draw(self, eng: LearnerEngine, stage: int = -1, generator: torch.Generator | None = None,
+                    u: torch.Tensor | None = None, beta: float | None = None):
+        """Global sampling's draw into the engine's fill slot (what sample_into does once attached).  stage 0 writes
+        this rank's uniforms and publishes them with the shard root, 1 draws, gathers and signals delivery, 2 waits for
+        every owner and forms the weights; -1 runs all three.  In-process groups issue each stage for every rank before
+        the next, so that no wait spins."""
+        if self._group is None or eng is not self._group:
+            raise nv.NativeError("this shard draws globally only for the engine it was attached to")
+        eng._guard_fill()
+        if stage in (0, -1):
+            if u is None:
+                eng.uniforms.copy_(torch.rand(eng.cfg.batch, device=self.device, generator=generator))
+            else:
+                eng.uniforms.copy_(u)
+        b = eng.cfg.is_exponent if beta is None else float(beta)
+        if not 0.0 <= b <= 1.0:
+            raise ValueError("beta must lie in [0, 1], got %r" % (b,))
+        nv.check(self.lib.r2d2_replay_global_draw(self._h, int(stage), eng._fill_slot, int(eng.importance_weighting), b,
+                                                  nv.current_stream()))
+
+    def global_write_back(self, leaf_idx: torch.Tensor, prio: torch.Tensor, stage: int = -1):
+        """Global sampling's write-back of the trained batch (what update_priorities does once attached): leaf_idx is
+        that slot's engine.leaf_idx.  stage 0 publishes this rank's records, 1 waits for all and applies this shard's;
+        -1 runs both."""
+        shard = self._group.shard_of(leaf_idx)
+        nv.check(self.lib.r2d2_replay_global_write_back(self._h, int(stage), nv.dptr(leaf_idx, torch.int64),
+                                                        nv.dptr(shard, torch.int32), nv.dptr(prio),
+                                                        nv.current_stream()))
+
+    def global_status(self) -> int:
+        """0, or 1 when a bounded wait of the global-sampling kernels expired."""
+        if self._group is None:
+            return 0
+        st = c_int(0)
+        nv.check(self.lib.r2d2_replay_global_status(self._h, byref(st), nv.current_stream()))
+        return int(st.value)
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h:
@@ -679,6 +819,9 @@ class DeviceReplay:
         if (ec.obs, ec.act, ec.hidden, ec.rows) != (rc.obs, rc.act, rc.hidden, rc.rows):
             raise nv.NativeError("replay shard (obs %d act %d hidden %d rows %d) does not match the engine (obs %d act %d "
                                  "hidden %d rows %d)" % (rc.obs, rc.act, rc.hidden, rc.rows, ec.obs, ec.act, ec.hidden, ec.rows))
+        if self._group is not None:
+            self.global_draw(eng, -1, generator=generator, u=u, beta=beta)
+            return
         if u is None:
             eng.uniforms.copy_(torch.rand(eng.cfg.batch, device=self.device, generator=generator))
         else:
@@ -698,7 +841,11 @@ class DeviceReplay:
                                              nv.current_stream()))
 
     def update_priorities(self, leaf_idx: torch.Tensor, prio: torch.Tensor):
-        """Write raw priorities back; the leaves store prio^alpha (PathConfig.priority_exponent)."""
+        """Write raw priorities back; the leaves store prio^alpha (PathConfig.priority_exponent).  Global sampling:
+        leaf_idx must be the trained slot's (engine.leaf_idx); every rank's records reach the shards that own them."""
+        if self._group is not None:
+            self.global_write_back(leaf_idx, prio)
+            return
         nv.check(self.lib.r2d2_replay_update_priorities(self._h, nv.dptr(leaf_idx, torch.int64), nv.dptr(prio),
                                                         leaf_idx.numel(), nv.current_stream()))
 

@@ -65,6 +65,12 @@ class PeerLayout(Structure):
                                         "off_actor_sums")]
 
 
+class GlobalLayout(Structure):
+    _fields_ = [("bytes", c_size_t), ("slot_offset", c_size_t * 2)] + [
+        (k, c_size_t) for k in ("off_obs", "off_act", "off_rew", "off_term", "off_states", "off_leaf_idx", "off_shard",
+                                "off_is_weight", "off_uniforms")]
+
+
 class LearnerBuffers(Structure):
     _fields_ = [(k, c_void_p) for k in ("obs", "act", "rew", "term", "states", "leaf_idx", "uniforms",
                                         "q_value", "target_q_value", "td_sq", "priority", "losses")]
@@ -73,6 +79,7 @@ class LearnerBuffers(Structure):
 # name -> (restype, argtypes); every symbol include/r2d2_b200.h declares
 SIGNATURES = {
     "r2d2_version": (c_int, []),
+    "r2d2_launch_count": (c_longlong, []),
     "r2d2_arch": (c_char_p, []),
     "r2d2_last_error": (c_char_p, []),
     "r2d2_device_sm_count": (c_int, [POINTER(c_int)]),
@@ -128,6 +135,12 @@ SIGNATURES = {
     "r2d2_replay_stats": (c_int, [c_void_p, POINTER(ReplayStats), c_void_p]),
     "r2d2_replay_decode": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "r2d2_replay_tree_level": (c_int, [c_void_p, c_int, POINTER(c_void_p), POINTER(c_longlong)]),
+    "r2d2_global_layout_for": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(GlobalLayout)]),
+    "r2d2_replay_attach_group": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_void_p), c_size_t]),
+    "r2d2_replay_global_write_back": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "r2d2_replay_global_draw": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p]),
+    "r2d2_replay_global_status": (c_int, [c_void_p, POINTER(c_int), c_void_p]),
+    "r2d2_learner_set_slot_buffers": (c_int, [c_void_p, c_int, POINTER(LearnerBuffers), c_void_p]),
     "r2d2_learner_create": (c_int, [POINTER(c_void_p), POINTER(LearnerConfig)]),
     "r2d2_learner_create_ex": (c_int, [POINTER(c_void_p), POINTER(LearnerConfig), POINTER(LearnerOptions)]),
     "r2d2_learner_set_target_smoothing": (c_int, [c_void_p, c_float, c_float, c_uint, c_uint]),
@@ -223,4 +236,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "LearnerConfig", "LearnerOptions", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]

@@ -11,6 +11,11 @@ section 4).  Two rules keep the data the same as in the sequential loop:
     priorities onto rows that belong to other episodes by then.  The step in front of an ingest (and the last step of a
     bounded run) is sequential.
 
+Global sampling (PathConfig.global_sampling) relies on both rules and on one more fact of this loop: every rank runs the
+same steps, so every rank ingests on the same steps.  Its write-back and draw are collectives over the ranks' shards;
+with nothing drawn ahead of an ingest and the ingests in step, each shard publishes its root after its own write-back
+and ingest, and no rank's draw can meet rows a peer's ingest is still replacing.
+
 No CUDA, no torch: `engine` needs step(prefetch=None) + leaf_idx / priority attributes, `replay` needs sample_into(engine)
 and update_priorities(leaf_idx, priority) - tests drive it with recording fakes (tests/test_cpu_host.py).
 """
