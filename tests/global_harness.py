@@ -32,9 +32,11 @@ def global_schedule(steps: int, target_interval: int, prefetch: bool):
 
 
 def make_shard(E, cfg, rng, n_eps, p_lo, cap):
+    """(shard, the host episodes fed to it, oldest first)."""
+    eps = [episode(rng, cfg, int(rng.integers(cfg.rows + 8, cfg.rows + 60)), p_lo=p_lo) for _ in range(n_eps)]
     rp = E.DeviceReplay(cfg, capacity_rows=cap)
-    rp.add_episodes([episode(rng, cfg, int(rng.integers(cfg.rows + 8, cfg.rows + 60)), p_lo=p_lo) for _ in range(n_eps)])
-    return rp
+    rp.add_episodes(eps)
+    return rp, eps
 
 
 class GlobalRun:
@@ -47,15 +49,16 @@ class GlobalRun:
         self.bufs = [torch.zeros(int(lay.bytes) // 4, dtype=torch.float32, device="cuda") for _ in range(W)]
         ptrs = [b.data_ptr() for b in self.bufs]
         rng = np.random.default_rng(data_seed)
-        self.shards = []
+        self.shards, self.episodes = [], []     # per rank: its shard, the host episodes fed to it
         for r, eng in enumerate(self.g.engines):
             eng.use_global_slots(self.bufs[r], lay)
             eng.global_peer_ptrs, eng._rank = ptrs, r
             # unequal shards: sizes, masses (p_lo) and one small ring that wrapped and evicted
             cap = 600 if r == 1 else 6000
-            rp = make_shard(E, self.cfg, rng, 14 if r == 1 else 6 + 4 * r, 0.01 if r % 2 else 0.3, cap)
+            rp, eps = make_shard(E, self.cfg, rng, 14 if r == 1 else 6 + 4 * r, 0.01 if r % 2 else 0.3, cap)
             rp.attach_group(eng)
             self.shards.append(rp)
+            self.episodes.append(eps)
         torch.cuda.synchronize()
         self.gens = [torch.Generator(device="cuda").manual_seed(100 + r) for r in range(W)]
         self.draws = []          # per draw: (restated shard, leaf) and the device's
