@@ -200,6 +200,27 @@ typedef struct {
 } r2d2_replay_config;
 
 int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg);
+
+/* Storage precision of the recurrent states [4,2,H] of every row (obs, act, rew, term and the tree stay fp32).
+ * R2D2_STATE_F16 halves the bytes of the states, which are most of a row (91 % at O 376, A 17, H 512).  The states are
+ * rounded once at ingest (IEEE round-to-nearest-even) and widened exactly by the gather, so the batch holds exactly the
+ * fp16-rounded inputs.  The bound that makes fp16 safe: h = o tanh(c) gives |h| < 1, and c_t = f c_{t-1} + i g with
+ * f, i in (0, 1), |g| < 1 and c_0 = 0 gives |c_t| < t, so only an episode longer than 65,504 steps could overflow;
+ * the relative rounding error is at most 2^-12 (bf16's 2^-9 would exceed a 1e-3 parity bar on its own).  States from
+ * foreign actors can hold anything, so ingest in this mode checks: a finite value of magnitude >= 65520 (which would
+ * round to +-inf) refuses the whole add_episode(s) call with R2D2_ERR_ARG, naming the count, before any episode is
+ * placed, evicted or committed - the shard, its tree and its counters stay as they were.  NaN and +-inf pass through,
+ * as in fp32 storage.  Ingest in this mode copies the states into a grow-only device staging block and adds two
+ * kernels and one stream synchronisation per call; the gather is still one launch. */
+#define R2D2_STATE_F32 0
+#define R2D2_STATE_F16 1
+typedef struct {
+  int state_storage;   /* R2D2_STATE_F32 (default) or R2D2_STATE_F16; anything else is R2D2_ERR_ARG */
+} r2d2_replay_options;
+/* options NULL = r2d2_replay_create */
+int r2d2_replay_create_ex(r2d2_replay_t** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options);
+/* bytes of device memory the shard holds (rows, tree, and the fp16 mode's staging block once an ingest has used it) */
+int r2d2_replay_device_bytes(r2d2_replay_t* r, size_t* out);
 int r2d2_replay_destroy(r2d2_replay_t* r);
 /* Priority exponent alpha in [0, 1] (prioritized replay; default 1 = the raw priority): every leaf the shard writes -
  * ingest and r2d2_replay_update_priorities - holds p > 0 ? p^alpha : 0, so P(start) = p^alpha / sum p^alpha and rows

@@ -232,6 +232,12 @@ int r2d2_adam_step(float* params, const float* grads, float* exp_avg, float* exp
 int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg) {
   return replay_create(reinterpret_cast<Replay**>(out), cfg);
 }
+int r2d2_replay_create_ex(r2d2_replay_t** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options) {
+  return replay_create(reinterpret_cast<Replay**>(out), cfg, options ? options->state_storage : R2D2_STATE_F32);
+}
+int r2d2_replay_device_bytes(r2d2_replay_t* r, size_t* out) {
+  return replay_device_bytes(reinterpret_cast<Replay*>(r), out);
+}
 int r2d2_replay_destroy(r2d2_replay_t* r) { return replay_destroy(reinterpret_cast<Replay*>(r)); }
 int r2d2_replay_set_priority_exponent(r2d2_replay_t* r, float alpha) {
   return replay_set_priority_exponent(reinterpret_cast<Replay*>(r), alpha);

@@ -2,11 +2,15 @@
 //
 // HBM layout (SoA, one "row" per stored env step incl. the n_step pad rows of actor.py:173):
 //   obs_rows [cap,O]  act_rows [cap,A]  rew_rows [cap]  term_rows [cap]  state_rows [cap,4,2,H]
+// state_rows is fp32, or fp16 under R2D2_STATE_F16 (rounded once at ingest, widened back to fp32 by the gather).
 // Episodes occupy contiguous row ranges of a ring; FIFO eviction (replay_memory.py:148-152).
 // Sum tree: one leaf per ROW (priority 0 for rows that are not valid sequence starts), fan-out 32:
 // every node is the left-to-right fp32 sum of its 32 children (one 128-byte line), so the tree has
 // ceil(log32(cap)) levels (5 for 2M rows) instead of 21 dependent loads of a binary tree, and the
 // CUDA tree and its C restatement (oracle/sumtree_oracle.c) are bit-identical by construction.
+#include <cuda_fp16.h>
+#include <float.h>
+
 #include <algorithm>
 #include <deque>
 #include <map>
@@ -142,6 +146,34 @@ __global__ void __launch_bounds__(256) raise_leaves_kernel(float* __restrict__ l
   if (i < n) leaves[i] = raise_priority(leaves[i], alpha);
 }
 
+// fp16 state storage, ingest.  A finite x with |x| >= 65520 (65504 + half an fp16 ulp) rounds to +-inf under
+// round-to-nearest-even; NaN and +-inf are not counted (they pass through, as in fp32 storage).  Integer atomics, one
+// per warp: the count does not depend on the schedule.
+__global__ void __launch_bounds__(256) count_f16_overflow_kernel(const float* __restrict__ x, long long n,
+                                                                 unsigned long long* __restrict__ count) {
+  unsigned c = 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float a = fabsf(x[i]);
+    c += (a >= 65520.f && a <= FLT_MAX) ? 1u : 0u;
+  }
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, (unsigned long long)c);
+}
+
+// dst[i] = __float2half_rn(src[i]); n, src and dst are multiples of 8 elements (whole [4,2,H] rows: 8 H values), so
+// every thread moves two float4 loads into one 16-byte store.
+__global__ void __launch_bounds__(256) states_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst,
+                                                            long long n) {
+  const long long n8 = n >> 3;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const float4 a = reinterpret_cast<const float4*>(src)[2 * i];
+    const float4 b = reinterpret_cast<const float4*>(src)[2 * i + 1];
+    __half2 h[4] = {__floats2half2_rn(a.x, a.y), __floats2half2_rn(a.z, a.w), __floats2half2_rn(b.x, b.y),
+                    __floats2half2_rn(b.z, b.w)};
+    reinterpret_cast<uint4*>(dst)[i] = *reinterpret_cast<const uint4*>(h);
+  }
+}
+
 // Single CTA, in place: w[b] holds the drawn leaf value and becomes (min_b' w[b'] / w[b])^beta = (N P_b)^-beta
 // normalised by its batch maximum.  The min is order-independent, so the weights do not depend on the thread
 // schedule and the smallest leaf of the batch gets exactly 1.  Every index is read and written by the same thread.
@@ -260,7 +292,38 @@ __device__ __forceinline__ void warp_copy_row(const float* __restrict__ src, flo
   }
 }
 
-template <bool kPerDraw = false>
+// A stored fp16 state row widened into the fp32 batch (exact).  The sub-row starts at byte 2 H (8 leaf + nh) of the
+// ring and at float H (nh ld + col) of the batch, so H % 8 == 0 makes 16-byte loads (8 halves -> two float4 stores)
+// aligned at both ends, H % 4 == 0 8-byte loads (4 halves -> one float4 store); other widths go scalar.
+__device__ __forceinline__ void warp_widen_row(const __half* __restrict__ src, float* __restrict__ dst, int n, int lane) {
+  if ((n & 7) == 0) {
+    const uint4* s8 = reinterpret_cast<const uint4*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int k = lane; k < (n >> 3); k += 32) {
+      const uint4 v = __ldg(s8 + k);
+      const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+      const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+      const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&v.z));
+      const float2 d = __half22float2(*reinterpret_cast<const __half2*>(&v.w));
+      d4[2 * k] = make_float4(a.x, a.y, b.x, b.y);
+      d4[2 * k + 1] = make_float4(c.x, c.y, d.x, d.y);
+    }
+  } else if ((n & 3) == 0) {
+    const uint2* s4 = reinterpret_cast<const uint2*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int k = lane; k < (n >> 2); k += 32) {
+      const uint2 v = __ldg(s4 + k);
+      const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+      const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+      d4[k] = make_float4(a.x, a.y, b.x, b.y);
+    }
+  } else {
+    for (int k = lane; k < n; k += 32) dst[k] = __half2float(src[k]);
+  }
+}
+
+// kHalfStates: state_rows holds __half (r2d2_replay_options.state_storage = R2D2_STATE_F16); the batch stays fp32.
+template <bool kPerDraw = false, bool kHalfStates = false>
 __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
@@ -292,6 +355,9 @@ __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
         if (rew) rew[o] = __ldg(g.rew_rows + r);
         if (term) term[o] = __ldg(g.term_rows + r);
       }
+    } else if (kHalfStates) {
+      warp_widen_row(reinterpret_cast<const __half*>(g.state_rows) + (leaf * 8 + (t - g.T)) * g.H,
+                     states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
     } else {
       warp_copy_row(g.state_rows + (leaf * 8 + (t - g.T)) * g.H, states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
     }
@@ -320,6 +386,13 @@ struct Replay {
   r2d2_replay_config cfg;
   int rows_per_window;
   float *obs_rows = nullptr, *act_rows = nullptr, *rew_rows = nullptr, *term_rows = nullptr, *state_rows = nullptr;
+  // R2D2_STATE_F16: the states live in state_half (state_rows stays null), and ingest rounds them from a grow-only
+  // device staging block: [overflow count (16 B) | fp32 states of the largest call so far]
+  bool half_states = false;
+  __half* state_half = nullptr;
+  char* stage = nullptr;
+  size_t stage_bytes = 0;
+  size_t device_bytes = 0;   // every device allocation of the shard (rows, tree, staging)
   std::vector<float*> level_alloc;
   TreeView tv;
   std::deque<Episode> episodes;
@@ -354,23 +427,31 @@ static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leav
   return R2D2_OK;
 }
 
-int replay_create(Replay** out, const r2d2_replay_config* cfg) {
+int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage) {
   R2D2_REQUIRE(out && cfg, "null");
   R2D2_REQUIRE(cfg->obs_size > 0 && cfg->n_actions > 0 && cfg->hidden > 0, "sizes");
   R2D2_REQUIRE(cfg->capacity_rows > 0, "capacity_rows");
+  R2D2_REQUIRE(state_storage == R2D2_STATE_F32 || state_storage == R2D2_STATE_F16,
+               "state_storage is R2D2_STATE_F32 or R2D2_STATE_F16");
   Replay* r = new Replay();
   r->cfg = *cfg;
   r->rows_per_window = cfg->burn_in + cfg->learning + cfg->n_step;
+  r->half_states = state_storage == R2D2_STATE_F16;
   const long long cap = cfg->capacity_rows;
-  auto dmalloc = [&](float** p, long long n) -> int {
-    R2D2_CUDA_TRY(cudaMalloc(p, sizeof(float) * (size_t)n));
-    R2D2_CUDA_TRY(cudaMemset(*p, 0, sizeof(float) * (size_t)n));
+  auto dmalloc_bytes = [&](void** p, size_t bytes) -> int {
+    R2D2_CUDA_TRY(cudaMalloc(p, bytes));
+    R2D2_CUDA_TRY(cudaMemset(*p, 0, bytes));
+    r->device_bytes += bytes;
     return R2D2_OK;
+  };
+  auto dmalloc = [&](float** p, long long n) -> int {
+    return dmalloc_bytes(reinterpret_cast<void**>(p), sizeof(float) * (size_t)n);
   };
   int rc = R2D2_OK;
   if ((rc = dmalloc(&r->obs_rows, cap * cfg->obs_size)) || (rc = dmalloc(&r->act_rows, cap * cfg->n_actions)) ||
       (rc = dmalloc(&r->rew_rows, cap)) || (rc = dmalloc(&r->term_rows, cap)) ||
-      (rc = dmalloc(&r->state_rows, cap * 8 * cfg->hidden))) {
+      (rc = r->half_states ? dmalloc_bytes(reinterpret_cast<void**>(&r->state_half), sizeof(__half) * (size_t)cap * 8 * cfg->hidden)
+                           : dmalloc(&r->state_rows, cap * 8 * cfg->hidden))) {
     delete r;
     return rc;
   }
@@ -415,9 +496,58 @@ static int raise_fresh_leaves(Replay* r, long long first, long long n, cudaStrea
   return R2D2_OK;
 }
 
+// fp16 state storage: the staging block starts with the overflow count, the fp32 states follow 16 bytes in (every
+// packed row of 8 H floats then starts 16-byte aligned, as states_to_f16_kernel needs)
+constexpr size_t kStageHead = 16;
+static float* staged_states(Replay* r) { return reinterpret_cast<float*>(r->stage + kStageHead); }
+
+// Copies the call's n packed fp32 states into the staging block (grown to fit) and counts the finite values that fp16
+// would round to +-inf.  Any such value refuses the whole call with R2D2_ERR_ARG before anything is placed, evicted or
+// committed.  Synchronises the stream (the count is read on the host).
+static int stage_half_states(Replay* r, const float* states, size_t n, cudaStream_t stream) {
+  const size_t need = kStageHead + sizeof(float) * n;
+  if (need > r->stage_bytes) {
+    R2D2_CUDA_TRY(cudaFree(r->stage));   // synchronises: no conversion of an earlier call still reads the old block
+    r->stage = nullptr;
+    r->device_bytes -= r->stage_bytes;
+    r->stage_bytes = 0;
+    R2D2_CUDA_TRY(cudaMalloc(&r->stage, need));
+    r->stage_bytes = need;
+    r->device_bytes += need;
+  }
+  unsigned long long* d_count = reinterpret_cast<unsigned long long*>(r->stage);
+  R2D2_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(*d_count), stream));
+  if (n > 0) {
+    R2D2_CUDA_TRY(cudaMemcpyAsync(staged_states(r), states, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+    count_f16_overflow_kernel<<<grid_for((long long)n), 256, 0, stream>>>(staged_states(r), (long long)n, d_count);
+    count_launch();
+    R2D2_CUDA_TRY(cudaGetLastError());
+  }
+  unsigned long long count = 0;
+  R2D2_CUDA_TRY(cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
+  if (count) {
+    set_last_error(std::to_string(count) + " finite recurrent-state value(s) of magnitude >= 65520 would round to "
+                   "+-inf in fp16 state storage: nothing of this call was stored");
+    return R2D2_ERR_ARG;
+  }
+  return R2D2_OK;
+}
+
+// Rounds n_rows staged state rows (from packed row `first`) into ring rows [ring_row, ring_row + n_rows).
+static int convert_half_states(Replay* r, long long ring_row, long long first, long long n_rows, cudaStream_t stream) {
+  const long long w = 8LL * r->cfg.hidden, n = n_rows * w;
+  if (n == 0) return R2D2_OK;
+  states_to_f16_kernel<<<grid_for(n / 8), 256, 0, stream>>>(staged_states(r) + first * w, r->state_half + ring_row * w, n);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return R2D2_OK;
+}
+
 int replay_destroy(Replay* r) {
   if (!r) return R2D2_OK;
   cudaFree(r->obs_rows); cudaFree(r->act_rows); cudaFree(r->rew_rows); cudaFree(r->term_rows); cudaFree(r->state_rows);
+  cudaFree(r->state_half); cudaFree(r->stage);
   for (float* p : r->level_alloc) cudaFree(p);
   delete r->group;
   delete r;
@@ -497,6 +627,7 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
   R2D2_REQUIRE(n_state_rows >= n_starts && n_state_rows <= n_rows, "state rows");
   R2D2_REQUIRE(n_starts == 0 || priority, "priority");
   const int O = r->cfg.obs_size, A = r->cfg.n_actions, H = r->cfg.hidden;
+  if (r->half_states) R2D2_TRY(stage_half_states(r, states, (size_t)n_state_rows * 8 * H, stream));
   RangeList ranges;
   long long start = 0;
   R2D2_TRY(place_episode(r, n_rows, stream, &ranges, &start));
@@ -504,11 +635,18 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
   R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + start * A, act, sizeof(float) * (size_t)n_rows * A, cudaMemcpyHostToDevice, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + start, rew, sizeof(float) * (size_t)n_rows, cudaMemcpyHostToDevice, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + start, term, sizeof(float) * (size_t)n_rows, cudaMemcpyHostToDevice, stream));
-  R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + start * 8 * H, states, sizeof(float) * (size_t)n_state_rows * 8 * H,
-                                cudaMemcpyHostToDevice, stream));
-  if (n_state_rows < n_rows)
-    R2D2_CUDA_TRY(cudaMemsetAsync(r->state_rows + (start + n_state_rows) * 8 * H, 0,
-                                  sizeof(float) * (size_t)(n_rows - n_state_rows) * 8 * H, stream));
+  if (r->half_states) {
+    R2D2_TRY(convert_half_states(r, start, 0, n_state_rows, stream));
+    if (n_state_rows < n_rows)
+      R2D2_CUDA_TRY(cudaMemsetAsync(r->state_half + (start + n_state_rows) * 8 * H, 0,
+                                    sizeof(__half) * (size_t)(n_rows - n_state_rows) * 8 * H, stream));
+  } else {
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + start * 8 * H, states, sizeof(float) * (size_t)n_state_rows * 8 * H,
+                                  cudaMemcpyHostToDevice, stream));
+    if (n_state_rows < n_rows)
+      R2D2_CUDA_TRY(cudaMemsetAsync(r->state_rows + (start + n_state_rows) * 8 * H, 0,
+                                    sizeof(float) * (size_t)(n_rows - n_state_rows) * 8 * H, stream));
+  }
   if (n_starts > 0) {
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + start, priority, sizeof(float) * (size_t)n_starts,
                                   cudaMemcpyHostToDevice, stream));
@@ -542,6 +680,11 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     R2D2_REQUIRE(n_starts[e] >= 0 && n_starts[e] <= n_rows[e] - r->rows_per_window + 1, "n_starts exceeds valid window starts");
     R2D2_REQUIRE(n_rows[e] <= r->cfg.capacity_rows, "episode larger than the ring");
   }
+  if (r->half_states && n_episodes > 0) {
+    long long R = 0;
+    for (int e = 0; e < n_episodes; ++e) R += n_rows[e];
+    R2D2_TRY(stage_half_states(r, states, (size_t)R * 8 * H, stream));
+  }
   const long long evicted0 = r->evicted_total;
   RangeList ranges;
   long long src = 0;                    // first packed row of the current run
@@ -553,8 +696,11 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + run_start * A, act + src * A, sizeof(float) * n * A, cudaMemcpyHostToDevice, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + run_start, rew + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + run_start, term + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + run_start * 8 * H, states + src * 8 * H, sizeof(float) * n * 8 * H,
-                                  cudaMemcpyHostToDevice, stream));
+    if (r->half_states)
+      R2D2_TRY(convert_half_states(r, run_start, src, run_rows, stream));
+    else
+      R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + run_start * 8 * H, states + src * 8 * H, sizeof(float) * n * 8 * H,
+                                    cudaMemcpyHostToDevice, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + run_start, leaf_prio + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
     R2D2_TRY(raise_fresh_leaves(r, run_start, run_rows, stream));
     ranges.push_back({run_start, run_rows});
@@ -581,6 +727,18 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
   return R2D2_OK;
 }
 
+// GatherParams keeps its fp32 state pointer (so that the fp32 gather compiles as before); the fp16 instantiations
+// read it as __half
+static const float* state_source(const Replay* r) {
+  return r->half_states ? reinterpret_cast<const float*>(r->state_half) : r->state_rows;
+}
+
+int replay_device_bytes(Replay* r, size_t* out) {
+  R2D2_REQUIRE(r && out, "null");
+  *out = r->device_bytes;
+  return R2D2_OK;
+}
+
 int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, float* act, float* rew, float* term,
                   float* states, cudaStream_t stream) {
   R2D2_REQUIRE(r && leaf_idx && batch > 0, "args");
@@ -588,11 +746,14 @@ int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, f
   if (obs || act || rew || term || states) {
     GatherParams g;
     g.obs_rows = r->obs_rows; g.act_rows = r->act_rows; g.rew_rows = r->rew_rows; g.term_rows = r->term_rows;
-    g.state_rows = r->state_rows; g.leaf = leaf_idx;
+    g.state_rows = state_source(r); g.leaf = leaf_idx;
     g.obs = obs; g.act = act; g.rew = rew; g.term = term; g.states = states;
     g.T = T; g.B = batch; g.O = O; g.A = A; g.H = H;
     const long long tasks = (long long)T * batch + (states ? (long long)8 * batch : 0);
-    gather_batch_kernel<false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
+    if (r->half_states)
+      gather_batch_kernel<false, true><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
+    else
+      gather_batch_kernel<false, false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
     count_launch();
   }
   R2D2_CUDA_TRY(cudaGetLastError());
@@ -796,7 +957,7 @@ int replay_global_draw(Replay* r, int stage, int slot, int weighted, float beta,
     R2D2_CUDA_TRY(cudaGetLastError());
     GatherParams gp;
     gp.obs_rows = r->obs_rows; gp.act_rows = r->act_rows; gp.rew_rows = r->rew_rows; gp.term_rows = r->term_rows;
-    gp.state_rows = r->state_rows;
+    gp.state_rows = state_source(r);
     char* own = g.peers.base[g.rank];
     gp.leaf = reinterpret_cast<const long long*>(own + g.lay.off_draw_leaf);
     gp.obs = gp.act = gp.rew = gp.term = nullptr;
@@ -808,7 +969,10 @@ int replay_global_draw(Replay* r, int stage, int slot, int weighted, float beta,
     gp.off_term = so + g.lay.off_term; gp.off_states = so + g.lay.off_states;
     gp.dst = g.peers;
     const long long tasks = (long long)(gp.T + 8) * gp.B;
-    gather_batch_kernel<true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
+    if (r->half_states)
+      gather_batch_kernel<true, true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
+    else
+      gather_batch_kernel<true, false><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
     count_launch();
     R2D2_CUDA_TRY(cudaGetLastError());
     R2D2_TRY(global_deliver(g.peers, g.world, g.rank, g.draw_epoch, stream));

@@ -43,7 +43,8 @@ int global_receive(const GlobalPeers& p, const GlobalLayout& lay, int world, int
                    float beta, unsigned epoch, cudaStream_t st);
 
 struct Replay;
-int replay_create(Replay** out, const r2d2_replay_config* cfg);
+int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage = R2D2_STATE_F32);
+int replay_device_bytes(Replay* r, size_t* out);
 int replay_destroy(Replay* r);
 int replay_set_priority_exponent(Replay* r, float alpha);
 int replay_add_episode(Replay* r, const float* obs, const float* act, const float* rew, const float* term,

@@ -38,6 +38,11 @@ bootstraps from the minimum of the two), R2D2_TARGET_NOISE (target policy smooth
 R2D2_TARGET_NOISE_CLIP (default 0.5) and R2D2_TARGET_NOISE_SEED (default 0).  model.pt keeps its four reference keys
 (critic 1 is the reference's critic); the resumable checkpoint holds critic 2 as well, and a resume across a twin /
 single-critic change is refused.
+
+Replay storage: R2D2_REPLAY_STATE_DTYPE=float32|float16 (default float32).  float16 keeps the four nets' stored (h, c) of
+every replay row in fp16 - nearly twice the rows in the same HBM (the ring is capped at 60 % of free HBM) - rounded once
+at ingest; an actor file holding a finite state of magnitude >= 65520 is refused whole.  Any other value raises.  The
+replay is not part of the checkpoint, so the setting may change across a resume.
 """
 import os
 from time import sleep, time
@@ -101,6 +106,7 @@ class Learner:
         self.is_exponent = float(os.environ.get("R2D2_IS_EXPONENT", 0.0))
         self.target_tau = float(os.environ.get("R2D2_TARGET_TAU", 1.0))
         self.grad_clip_norm = float(os.environ.get("R2D2_GRAD_CLIP", 0.0))
+        self.replay_state_dtype = self._replay_state_dtype_from_environ()
         from r2d2_b200 import td3_options, td_options
         self.td_options = td_options.from_environ()
         self.td3_options = td3_options.from_environ()
@@ -111,12 +117,14 @@ class Learner:
                          is_exponent=self.is_exponent, target_tau=self.target_tau, grad_clip_norm=self.grad_clip_norm,
                          value_rescaling=self.td_options.value_rescaling, rescaling_eps=self.td_options.rescaling_eps,
                          priority_metric=self.td_options.priority_metric, **self.td3_options,
-                         global_sampling=self._global_sampling_from_environ())
+                         global_sampling=self._global_sampling_from_environ(),
+                         replay_state_dtype=self.replay_state_dtype)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
                                           obs_size=self.obs_size, n_actions=self.n_actions, hidden=self.hidden,
-                                          device=self.engine.device, priority_exponent=self.priority_exponent)
+                                          device=self.engine.device, priority_exponent=self.priority_exponent,
+                                          state_dtype=self.replay_state_dtype)
         self.state_path = self.model_path + 'learner_state.pt'
         if os.environ.get("R2D2_RESUME", "0") == "1" and os.path.isfile(self.state_path):
             self.load_checkpoint()                         # every rank loads the same file: replicas stay identical
@@ -128,6 +136,13 @@ class Learner:
         if v not in ("0", "1"):
             raise ValueError("R2D2_GLOBAL_SAMPLING must be 0 or 1, got {!r}".format(v))
         return v == "1"
+
+    @staticmethod
+    def _replay_state_dtype_from_environ():
+        v = os.environ.get("R2D2_REPLAY_STATE_DTYPE", "float32")
+        if v not in ("float32", "float16"):
+            raise ValueError("R2D2_REPLAY_STATE_DTYPE must be float32 or float16, got {!r}".format(v))
+        return v
 
     def save_checkpoint(self):
         """Resumable state next to model.pt: nets + both Adam moment sets + step counter (the reference's model.pt has

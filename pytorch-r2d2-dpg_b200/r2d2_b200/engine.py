@@ -13,7 +13,7 @@ from __future__ import annotations
 import math
 import numbers
 from collections import OrderedDict
-from ctypes import byref, c_int, c_longlong, c_void_p
+from ctypes import byref, c_int, c_longlong, c_size_t, c_void_p
 from dataclasses import dataclass
 
 import numpy as np
@@ -21,6 +21,9 @@ import torch
 
 from . import native as nv
 from . import td_options
+
+# PathConfig.replay_state_dtype -> r2d2_replay_options.state_storage
+REPLAY_STATE_DTYPES = {"float32": nv.STATE_F32, "float16": nv.STATE_F16}
 
 PARAM_KEYS = ("l1.weight", "l1.bias", "l2.weight_ih", "l2.weight_hh", "l2.bias_ih", "l2.bias_hh",
               "l3.weight", "l3.bias")
@@ -52,7 +55,12 @@ class PathConfig:
     `global_sampling` (data parallel, off by default): the W ranks draw one global batch of W * B sequences from the
     union of their replay shards in proportion to the stored leaves p^alpha, and rank c trains on global draws
     c*B .. c*B+B-1 (DeviceReplay.attach_group).  The engine's batch slots then live in memory every rank maps; at W = 1
-    the draws, batches and weights are the local mode's bit for bit."""
+    the draws, batches and weights are the local mode's bit for bit.
+
+    `replay_state_dtype` (replay shard, include/r2d2_b200.h r2d2_replay_options): "float32" (default) stores the four
+    nets' recurrent states of every row in fp32; "float16" stores them in fp16 - nearly twice the rows in the same HBM -
+    rounded once at ingest and widened exactly by the gather, so training sees the fp16-rounded states.  An actor file
+    with a finite state of magnitude >= 65520 is refused whole in that mode."""
     obs: int
     act: int
     hidden: int = 128
@@ -77,6 +85,7 @@ class PathConfig:
     target_noise_clip: float = 0.5
     target_noise_seed: int = 0
     global_sampling: bool = False
+    replay_state_dtype: str = "float32"
 
     def __post_init__(self):
         for name, least in (("burn_in", 0), ("learning", 2), ("n_step", 1)):
@@ -86,6 +95,9 @@ class PathConfig:
                     name, least, v, " (the priority series [b:-1:B] of the last batch element drops its last TD step, "
                                     "so a one-step window leaves it empty)" if name == "learning" else ""))
         td_options.validate(self.value_rescaling, self.rescaling_eps, self.priority_metric)
+        if not isinstance(self.replay_state_dtype, str) or self.replay_state_dtype not in REPLAY_STATE_DTYPES:
+            raise ValueError("replay_state_dtype must be one of %s, got %r" % (", ".join(REPLAY_STATE_DTYPES),
+                                                                              self.replay_state_dtype))
         for name in ("twin_critic", "global_sampling"):
             if not isinstance(getattr(self, name), bool):
                 raise ValueError("%s must be True or False, got %r" % (name, getattr(self, name)))
@@ -685,7 +697,8 @@ class DeviceReplay:
         rc = nv.ReplayConfig(cfg.obs, cfg.act, cfg.hidden, cfg.burn_in, cfg.learning, cfg.n_step,
                              int(capacity_rows), int(max_sequences))
         self._h = c_void_p()
-        nv.check(self.lib.r2d2_replay_create(byref(self._h), byref(rc)))
+        opt = nv.ReplayOptions(REPLAY_STATE_DTYPES[cfg.replay_state_dtype])
+        nv.check(self.lib.r2d2_replay_create_ex(byref(self._h), byref(rc), byref(opt)))
         if cfg.priority_exponent != 1.0:   # leaves hold p^alpha; actors and write-backs keep passing raw priorities
             nv.check(self.lib.r2d2_replay_set_priority_exponent(self._h, float(cfg.priority_exponent)))
         self._group = None                 # the engine whose rank / world / buffers global sampling uses
@@ -848,6 +861,12 @@ class DeviceReplay:
             return
         nv.check(self.lib.r2d2_replay_update_priorities(self._h, nv.dptr(leaf_idx, torch.int64), nv.dptr(prio),
                                                         leaf_idx.numel(), nv.current_stream()))
+
+    def device_bytes(self) -> int:
+        """Bytes of device memory the shard holds: rows, tree, and the fp16 mode's ingest staging once used."""
+        n = c_size_t(0)
+        nv.check(self.lib.r2d2_replay_device_bytes(self._h, byref(n)))
+        return int(n.value)
 
     def stats(self) -> dict:
         st = nv.ReplayStats()

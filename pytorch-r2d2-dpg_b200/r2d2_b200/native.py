@@ -56,6 +56,13 @@ class TdOptions(Structure):
     _fields_ = [("rescaling", c_int), ("eps", c_float), ("priority_metric", c_int)]
 
 
+class ReplayOptions(Structure):
+    _fields_ = [("state_storage", c_int)]
+
+
+STATE_F32, STATE_F16 = 0, 1   # ReplayOptions.state_storage (R2D2_STATE_F32 / R2D2_STATE_F16)
+
+
 class LearnerOptions(Structure):
     _fields_ = [("twin_critic", c_int)]
 
@@ -120,6 +127,8 @@ SIGNATURES = {
     "r2d2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_float, c_float, c_float,
                                c_float, c_float, c_void_p]),
     "r2d2_replay_create": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig)]),
+    "r2d2_replay_create_ex": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig), POINTER(ReplayOptions)]),
+    "r2d2_replay_device_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
     "r2d2_replay_destroy": (c_int, [c_void_p]),
     "r2d2_replay_set_priority_exponent": (c_int, [c_void_p, c_float]),
     "r2d2_replay_add_episodes": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -236,4 +245,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "ReplayOptions", "STATE_F32", "STATE_F16", "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]

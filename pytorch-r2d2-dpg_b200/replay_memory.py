@@ -134,7 +134,7 @@ class _TotalPriority:
 
 class LearnerReplayMemory:
     def __init__(self, memory_sequence_size=500000, batch_size=32, obs_size=None, n_actions=None, hidden=128,
-                 capacity_rows=None, device=None, priority_exponent=None):
+                 capacity_rows=None, device=None, priority_exponent=None, state_dtype="float32"):
         self.path = './memory_data/'
         self.memory_sequence_size = memory_sequence_size
         self.sequence_counter = 0
@@ -146,6 +146,7 @@ class LearnerReplayMemory:
         if priority_exponent is None:
             priority_exponent = float(os.environ.get("R2D2_PRIORITY_EXPONENT", 1.0))
         self.priority_exponent = float(priority_exponent)
+        self.state_dtype = state_dtype                      # recurrent states in HBM: "float32" or "float16"
         self._cfg()                                         # rejects an exponent outside [0, 1] before any ingest
         self._dev = None          # DeviceReplay, created when the row width is known
         self._episodes = deque()  # (row_start, n_rows, n_starts) in FIFO order, mirrors the native ring
@@ -175,7 +176,7 @@ class LearnerReplayMemory:
         from r2d2_b200.engine import PathConfig
         return PathConfig(obs=self._obs, act=self._act, hidden=self._hidden, batch=self.batch_size,
                           burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
-                          priority_exponent=self.priority_exponent)
+                          priority_exponent=self.priority_exponent, replay_state_dtype=self.state_dtype)
 
     def _ensure_device(self, obs_size, n_actions, hidden):
         """Create the HBM shard on first use.  Sizes given to the constructor are binding: an actor file of another
@@ -196,14 +197,17 @@ class LearnerReplayMemory:
         """Ring rows for `memory_sequence_size` sequences (one stored row per sequence start plus the 64 rows per
         episode that start no sequence: x1.3), capped at 60 % of the free HBM.  The reference keeps up to
         memory_sequence_size sequences in host RAM (replay_memory.py:148); when the cap applies, FIFO eviction starts
-        earlier than there - said out loud, and documented in INTEGRATION.md."""
+        earlier than there - said out loud, and documented in INTEGRATION.md.  fp16 state storage halves the
+        recurrent states [4,2,H] of a row, so the same cap holds nearly twice the rows."""
         want = int(self.memory_sequence_size * 1.3) + 4096
-        bytes_per_row = 4 * (obs_size + n_actions + 2 + 8 * hidden) + 5      # rows + leaf + ancestors
+        state_bytes = 16 if self.state_dtype == "float16" else 32              # (h, c) of four nets, per unit of H
+        bytes_per_row = 4 * (obs_size + n_actions + 2) + state_bytes * hidden + 5   # rows + leaf + ancestors
         free = torch.cuda.mem_get_info(self._device)[0] if torch.cuda.is_available() else 0
         fit = int(0.6 * free / bytes_per_row)
         if 0 < fit < want:
-            print("LearnerReplayMemory: ring capped at %d rows (%.1f GB of HBM) for memory_sequence_size=%d; FIFO "
-                  "eviction starts earlier than the reference's" % (fit, fit * bytes_per_row / 1e9, self.memory_sequence_size))
+            print("LearnerReplayMemory: ring capped at %d rows (%.1f GB of HBM, %s recurrent states) for "
+                  "memory_sequence_size=%d; FIFO eviction starts earlier than the reference's"
+                  % (fit, fit * bytes_per_row / 1e9, self.state_dtype, self.memory_sequence_size))
             return fit
         return want
 
