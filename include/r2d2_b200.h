@@ -285,6 +285,44 @@ int r2d2_replay_decode(r2d2_replay_t* r, const long long* leaf_idx_host, int n, 
 /* raw device views for tests: tree level pointer/size, leaf priorities */
 int r2d2_replay_tree_level(r2d2_replay_t* r, int level, const float** dev_ptr, long long* n);
 
+/* Snapshots: a shard's whole state to the host and back (a resumed run continues bit for bit).  That state is the live
+ * episodes' rows, their leaves (p^alpha; the raw priorities are not kept) and the bookkeeping below: every other leaf is
+ * 0 and every tree node is the left-to-right fp32 sum of its children, so the restore rebuilds the tree from the leaves.
+ * Export: r2d2_replay_export_info, the episode table in FIFO order, and any contiguous ring range of rows into HOST
+ * buffers (pinned for speed) - obs [n,O], act [n,A], rew [n], term [n], states [n,4,2,H] in the STORED type (fp16 under
+ * R2D2_STATE_F16), leaves [n]; plain copies, synchronises the stream.
+ * Import into an EMPTY shard (else R2D2_ERR_STATE) of the same obs / act / hidden / burn-in / learning / n-step and the
+ * same priority exponent (else R2D2_ERR_ARG), in three parts:
+ *   begin  the snapshot's info and episode table.  Same capacity_rows: every episode goes back to its row and head is
+ *          restored, so leaf indices and every tree level come back identical.  Other capacity: the episodes are
+ *          compacted from row 0 in FIFO order; while they do not fit the oldest is dropped with evict_front's counter
+ *          arithmetic (sequence_counter -= n_rows - (burn_in + learning), evicted_total += 1); *n_dropped_out counts them.
+ *   rows   the episodes' rows packed in FIFO order (the table's order, dropped episodes included), in consecutive chunks
+ *          [first, first + n), states in info->state_storage.  fp16 into an fp32 ring is widened exactly; fp32 into an
+ *          fp16 ring is rounded as ingest rounds, and a finite value of magnitude >= 65520 refuses the restore.  A leaf
+ *          that is negative, NaN or inf on a sequence start, or nonzero on any other row, refuses it.  Synchronises.
+ *   end    checks that every row arrived, rebuilds the tree over the whole ring, commits the bookkeeping.  Synchronises.
+ * Any refusal leaves the shard empty (no episode, zero counters, an all-zero tree); r2d2_last_error names the cause. */
+typedef struct {
+  int obs_size, n_actions, hidden, burn_in, learning, n_step;
+  int state_storage;                 /* R2D2_STATE_F32 / R2D2_STATE_F16 */
+  float priority_exponent;           /* alpha of the stored leaves */
+  long long capacity_rows, max_sequences;
+  long long n_episodes, head, sequence_counter, next_serial, evicted_total, rows_used;
+} r2d2_replay_snapshot_info;
+int r2d2_replay_export_info(r2d2_replay_t* r, r2d2_replay_snapshot_info* out);
+/* [n_episodes] each, FIFO order */
+int r2d2_replay_export_episodes(r2d2_replay_t* r, long long* row_start, int* n_rows, int* n_starts, long long* serial);
+int r2d2_replay_export_rows(r2d2_replay_t* r, long long first, long long n, float* obs, float* act, float* rew,
+                            float* term, void* states, float* leaves, r2d2_stream_t stream);
+int r2d2_replay_import_begin(r2d2_replay_t* r, const r2d2_replay_snapshot_info* info, const long long* row_start,
+                             const int* n_rows, const int* n_starts, const long long* serial, long long* n_dropped_out,
+                             r2d2_stream_t stream);
+int r2d2_replay_import_rows(r2d2_replay_t* r, long long first, long long n, const float* obs, const float* act,
+                            const float* rew, const float* term, const void* states, const float* leaves,
+                            r2d2_stream_t stream);
+int r2d2_replay_import_end(r2d2_replay_t* r, r2d2_stream_t stream);
+
 /* Global sampling over the replay shards of W data-parallel ranks (off unless a shard is attached to a group).  The W
  * shard roots form one more tree level above the shards, in rank order: global draw j of W*B takes r = u_j * total
  * (total the left-to-right fp32 sum of the roots), walks the roots as the tree walks 32 children and descends the

@@ -283,6 +283,30 @@ int r2d2_replay_decode(r2d2_replay_t* r, const long long* leaf_idx_host, int n, 
 int r2d2_replay_tree_level(r2d2_replay_t* r, int level, const float** dev_ptr, long long* n) {
   return replay_tree_level(reinterpret_cast<Replay*>(r), level, dev_ptr, n);
 }
+int r2d2_replay_export_info(r2d2_replay_t* r, r2d2_replay_snapshot_info* out) {
+  return replay_export_info(reinterpret_cast<Replay*>(r), out);
+}
+int r2d2_replay_export_episodes(r2d2_replay_t* r, long long* row_start, int* n_rows, int* n_starts, long long* serial) {
+  return replay_export_episodes(reinterpret_cast<Replay*>(r), row_start, n_rows, n_starts, serial);
+}
+int r2d2_replay_export_rows(r2d2_replay_t* r, long long first, long long n, float* obs, float* act, float* rew,
+                            float* term, void* states, float* leaves, r2d2_stream_t stream) {
+  return replay_export_rows(reinterpret_cast<Replay*>(r), first, n, obs, act, rew, term, states, leaves, S(stream));
+}
+int r2d2_replay_import_begin(r2d2_replay_t* r, const r2d2_replay_snapshot_info* info, const long long* row_start,
+                             const int* n_rows, const int* n_starts, const long long* serial, long long* n_dropped_out,
+                             r2d2_stream_t stream) {
+  return replay_import_begin(reinterpret_cast<Replay*>(r), info, row_start, n_rows, n_starts, serial, n_dropped_out,
+                             S(stream));
+}
+int r2d2_replay_import_rows(r2d2_replay_t* r, long long first, long long n, const float* obs, const float* act,
+                            const float* rew, const float* term, const void* states, const float* leaves,
+                            r2d2_stream_t stream) {
+  return replay_import_rows(reinterpret_cast<Replay*>(r), first, n, obs, act, rew, term, states, leaves, S(stream));
+}
+int r2d2_replay_import_end(r2d2_replay_t* r, r2d2_stream_t stream) {
+  return replay_import_end(reinterpret_cast<Replay*>(r), S(stream));
+}
 
 int r2d2_global_layout_for(int rows, int batch, int obs_size, int n_actions, int hidden, int world, r2d2_global_layout* out) {
   R2D2_REQUIRE(out, "null");

@@ -174,6 +174,37 @@ __global__ void __launch_bounds__(256) states_to_f16_kernel(const float* __restr
   }
 }
 
+// Snapshot restore, fp16 file into an fp32 ring: dst[i] = (float)src[i], exact.  A restored range is whole [4,2,H] rows
+// (8 H halves = 16 H bytes each, and the staging copy starts 16 bytes into its block), so both ends are 16-byte aligned
+// for every H: each thread widens one 16-byte load of 8 halves into two float4 stores (the gather's widest route).
+__global__ void __launch_bounds__(256) states_from_f16_kernel(const __half* __restrict__ src, float* __restrict__ dst,
+                                                              long long n) {
+  const long long n8 = n >> 3;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = reinterpret_cast<const uint4*>(src)[i];
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+    const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&v.z));
+    const float2 d = __half22float2(*reinterpret_cast<const __half2*>(&v.w));
+    reinterpret_cast<float4*>(dst)[2 * i] = make_float4(a.x, a.y, b.x, b.y);
+    reinterpret_cast<float4*>(dst)[2 * i + 1] = make_float4(c.x, c.y, d.x, d.y);
+  }
+}
+
+// Snapshot restore: counts the imported leaves of one episode that no shard could have written - on its first n_valid
+// rows (the sequence starts) a negative, NaN or infinite value, on the rows after them anything but zero.  Integer
+// atomics, one per warp, as in count_f16_overflow_kernel.
+__global__ void __launch_bounds__(256) count_bad_leaves_kernel(const float* __restrict__ leaves, long long n,
+                                                               long long n_valid, unsigned long long* __restrict__ count) {
+  unsigned c = 0;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float v = leaves[i];
+    c += (i < n_valid ? !(v >= 0.f && v <= FLT_MAX) : v != 0.f) ? 1u : 0u;
+  }
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, (unsigned long long)c);
+}
+
 // Single CTA, in place: w[b] holds the drawn leaf value and becomes (min_b' w[b'] / w[b])^beta = (N P_b)^-beta
 // normalised by its batch maximum.  The min is order-independent, so the weights do not depend on the thread
 // schedule and the smallest leaf of the batch gets exactly 1.  Every index is read and written by the same thread.
@@ -412,6 +443,16 @@ struct Replay {
     bool drawn_since_wb = true;         // a write-back needs a draw since the last one (the record block is reused)
   };
   Group* group = nullptr;
+  struct Import {       // a snapshot restore between r2d2_replay_import_begin and _end
+    struct Run { long long src, dst, n; };   // packed snapshot rows [src, src + n) -> ring rows [dst, dst + n)
+    std::vector<Run> runs;
+    std::vector<Episode> kept;               // at their ring rows, FIFO order
+    std::vector<long long> kept_src;         // packed snapshot row of each kept episode
+    long long packed_rows = 0, received = 0;
+    int storage = R2D2_STATE_F32;            // the snapshot's state storage
+    long long head = 0, sequence_counter = 0, next_serial = 0, evicted_total = 0, rows_used = 0;
+  };
+  Import* import = nullptr;
 };
 
 static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leaves, cudaStream_t stream) {
@@ -504,8 +545,7 @@ static float* staged_states(Replay* r) { return reinterpret_cast<float*>(r->stag
 // Copies the call's n packed fp32 states into the staging block (grown to fit) and counts the finite values that fp16
 // would round to +-inf.  Any such value refuses the whole call with R2D2_ERR_ARG before anything is placed, evicted or
 // committed.  Synchronises the stream (the count is read on the host).
-static int stage_half_states(Replay* r, const float* states, size_t n, cudaStream_t stream) {
-  const size_t need = kStageHead + sizeof(float) * n;
+static int ensure_stage(Replay* r, size_t need) {
   if (need > r->stage_bytes) {
     R2D2_CUDA_TRY(cudaFree(r->stage));   // synchronises: no conversion of an earlier call still reads the old block
     r->stage = nullptr;
@@ -515,6 +555,11 @@ static int stage_half_states(Replay* r, const float* states, size_t n, cudaStrea
     r->stage_bytes = need;
     r->device_bytes += need;
   }
+  return R2D2_OK;
+}
+
+static int stage_half_states(Replay* r, const float* states, size_t n, cudaStream_t stream) {
+  R2D2_TRY(ensure_stage(r, kStageHead + sizeof(float) * n));
   unsigned long long* d_count = reinterpret_cast<unsigned long long*>(r->stage);
   R2D2_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(*d_count), stream));
   if (n > 0) {
@@ -550,6 +595,7 @@ int replay_destroy(Replay* r) {
   cudaFree(r->state_half); cudaFree(r->stage);
   for (float* p : r->level_alloc) cudaFree(p);
   delete r->group;
+  delete r->import;
   delete r;
   return R2D2_OK;
 }
@@ -834,6 +880,239 @@ int replay_tree_level(Replay* r, int level, const float** dev_ptr, long long* n)
   R2D2_REQUIRE(r && level >= 0 && level < r->tv.levels, "level");
   *dev_ptr = r->tv.lvl[level];
   *n = r->tv.n[level];
+  return R2D2_OK;
+}
+
+// ---- snapshots (r2d2_replay_export_* / r2d2_replay_import_*) ----------------------------------------------------------
+// The live episodes' rows, their leaves and the host bookkeeping are the whole state of a shard: every other leaf is 0
+// (ingest and evict_front zero them) and every tree node is the left-to-right sum of its children, so a full rebuild
+// from the leaves gives every level back bit for bit.
+
+int replay_export_info(Replay* r, r2d2_replay_snapshot_info* out) {
+  R2D2_REQUIRE(r && out, "null");
+  const r2d2_replay_config& c = r->cfg;
+  out->obs_size = c.obs_size; out->n_actions = c.n_actions; out->hidden = c.hidden;
+  out->burn_in = c.burn_in; out->learning = c.learning; out->n_step = c.n_step;
+  out->state_storage = r->half_states ? R2D2_STATE_F16 : R2D2_STATE_F32;
+  out->priority_exponent = r->alpha;
+  out->capacity_rows = c.capacity_rows; out->max_sequences = c.max_sequences;
+  out->n_episodes = (long long)r->episodes.size();
+  out->head = r->head; out->sequence_counter = r->sequence_counter; out->next_serial = r->next_serial;
+  out->evicted_total = r->evicted_total; out->rows_used = r->rows_used;
+  return R2D2_OK;
+}
+
+int replay_export_episodes(Replay* r, long long* row_start, int* n_rows, int* n_starts, long long* serial) {
+  R2D2_REQUIRE(r && (r->episodes.empty() || (row_start && n_rows && n_starts && serial)), "null");
+  size_t i = 0;
+  for (const Episode& e : r->episodes) {
+    row_start[i] = e.row_start; n_rows[i] = e.n_rows; n_starts[i] = e.n_starts; serial[i] = e.serial;
+    ++i;
+  }
+  return R2D2_OK;
+}
+
+int replay_export_rows(Replay* r, long long first, long long n, float* obs, float* act, float* rew, float* term,
+                       void* states, float* leaves, cudaStream_t stream) {
+  R2D2_REQUIRE(r && obs && act && rew && term && states && leaves, "null");
+  R2D2_REQUIRE(first >= 0 && n >= 0 && first + n <= r->cfg.capacity_rows, "row range outside the ring");
+  const size_t O = r->cfg.obs_size, A = r->cfg.n_actions, w = 8 * (size_t)r->cfg.hidden, k = (size_t)n;
+  R2D2_CUDA_TRY(cudaMemcpyAsync(obs, r->obs_rows + first * O, sizeof(float) * k * O, cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(act, r->act_rows + first * A, sizeof(float) * k * A, cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(rew, r->rew_rows + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(term, r->term_rows + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
+  if (r->half_states)
+    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_half + first * w, sizeof(__half) * k * w, cudaMemcpyDeviceToHost, stream));
+  else
+    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_rows + first * w, sizeof(float) * k * w, cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(leaves, r->tv.lvl[0] + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
+  return R2D2_OK;
+}
+
+// A refused restore leaves the shard empty: no episode, zero counters, every tree node 0.
+static void abandon_import(Replay* r, cudaStream_t stream) {
+  delete r->import;
+  r->import = nullptr;
+  r->episodes.clear();
+  r->by_row.clear();
+  r->head = r->sequence_counter = r->next_serial = r->evicted_total = r->rows_used = 0;
+  for (int l = 0; l < r->tv.levels; ++l) cudaMemsetAsync(r->tv.lvl[l], 0, sizeof(float) * (size_t)r->tv.n[l], stream);
+  cudaStreamSynchronize(stream);
+}
+
+static int refuse_import(Replay* r, cudaStream_t stream, const std::string& why) {
+  abandon_import(r, stream);
+  set_last_error("replay snapshot refused, the shard is left empty: " + why);
+  return R2D2_ERR_ARG;
+}
+
+int replay_import_begin(Replay* r, const r2d2_replay_snapshot_info* info, const long long* row_start,
+                        const int* n_rows, const int* n_starts, const long long* serial, long long* n_dropped_out,
+                        cudaStream_t stream) {
+  R2D2_REQUIRE(r && info, "null");
+  R2D2_REQUIRE(info->n_episodes == 0 || (row_start && n_rows && n_starts && serial), "null episode table");
+  if (!r->episodes.empty() || r->import) {
+    set_last_error("a replay snapshot can only be restored into an empty shard");
+    return R2D2_ERR_STATE;
+  }
+  const r2d2_replay_config& c = r->cfg;
+  auto refuse = [&](const std::string& why) { return refuse_import(r, stream, why); };
+  if (info->obs_size != c.obs_size || info->n_actions != c.n_actions || info->hidden != c.hidden ||
+      info->burn_in != c.burn_in || info->learning != c.learning || info->n_step != c.n_step)
+    return refuse("the snapshot's obs / act / hidden / burn-in / learning / n-step (" + std::to_string(info->obs_size) +
+                  " " + std::to_string(info->n_actions) + " " + std::to_string(info->hidden) + " " +
+                  std::to_string(info->burn_in) + " " + std::to_string(info->learning) + " " +
+                  std::to_string(info->n_step) + ") differ from the shard's (" + std::to_string(c.obs_size) + " " +
+                  std::to_string(c.n_actions) + " " + std::to_string(c.hidden) + " " + std::to_string(c.burn_in) +
+                  " " + std::to_string(c.learning) + " " + std::to_string(c.n_step) + ")");
+  if (info->priority_exponent != r->alpha)
+    return refuse("the snapshot's leaves hold p^" + std::to_string(info->priority_exponent) + ", the shard stores p^" +
+                  std::to_string(r->alpha) + " (the raw priorities are not kept)");
+  if (info->state_storage != R2D2_STATE_F32 && info->state_storage != R2D2_STATE_F16)
+    return refuse("unknown state storage " + std::to_string(info->state_storage));
+  if (info->n_episodes < 0 || info->capacity_rows <= 0 || info->head < 0 || info->head > info->capacity_rows)
+    return refuse("bad counters");
+  // the episode table: valid episodes, consecutive serials (decode indexes the FIFO by serial), disjoint ring ranges
+  Replay::Import* im = new Replay::Import();
+  r->import = im;
+  std::vector<std::pair<long long, long long>> spans;
+  long long total = 0;
+  for (long long e = 0; e < info->n_episodes; ++e) {
+    if (n_rows[e] < r->rows_per_window || n_starts[e] < 0 || n_starts[e] > n_rows[e] - r->rows_per_window + 1 ||
+        row_start[e] < 0 || row_start[e] + n_rows[e] > info->capacity_rows || serial[e] != serial[0] + e)
+      return refuse("episode " + std::to_string(e) + " of the table is malformed");
+    spans.push_back({row_start[e], row_start[e] + n_rows[e]});
+    total += n_rows[e];
+  }
+  std::sort(spans.begin(), spans.end());
+  for (size_t i = 1; i < spans.size(); ++i)
+    if (spans[i].first < spans[i - 1].second) return refuse("episodes of the table overlap in the ring");
+  if (total != info->rows_used || (info->n_episodes > 0 && info->next_serial != serial[info->n_episodes - 1] + 1))
+    return refuse("the episode table does not match the counters");
+  im->packed_rows = total;
+  im->sequence_counter = info->sequence_counter;
+  im->next_serial = info->next_serial;
+  im->evicted_total = info->evicted_total;
+  im->rows_used = total;
+  const bool same = info->capacity_rows == c.capacity_rows;
+  long long first_kept = 0, dropped = 0;
+  if (!same) {   // compacted from row 0 in FIFO order; the oldest go while the rest does not fit (evict_front's counts)
+    while (first_kept < info->n_episodes && im->rows_used > c.capacity_rows) {
+      im->sequence_counter -= n_rows[first_kept] - (c.burn_in + c.learning);
+      im->rows_used -= n_rows[first_kept];
+      ++im->evicted_total;
+      ++first_kept;
+      ++dropped;
+    }
+  }
+  long long src = 0, dst = 0;
+  for (long long e = 0; e < info->n_episodes; ++e) {
+    if (e >= first_kept) {
+      const long long at = same ? row_start[e] : dst;
+      im->kept.push_back(Episode{at, n_rows[e], n_starts[e], serial[e]});
+      im->kept_src.push_back(src);
+      if (!im->runs.empty() && im->runs.back().src + im->runs.back().n == src && im->runs.back().dst + im->runs.back().n == at)
+        im->runs.back().n += n_rows[e];
+      else
+        im->runs.push_back({src, at, (long long)n_rows[e]});
+      dst = at + n_rows[e];
+    }
+    src += n_rows[e];
+  }
+  im->head = same ? info->head : dst;
+  im->storage = info->state_storage;
+  // leaves outside the restored episodes must be 0 for the rebuild; a fresh shard already has them so
+  R2D2_CUDA_TRY(cudaMemsetAsync(r->tv.lvl[0], 0, sizeof(float) * (size_t)r->tv.n[0], stream));
+  if (n_dropped_out) *n_dropped_out = dropped;
+  return R2D2_OK;
+}
+
+int replay_import_rows(Replay* r, long long first, long long n, const float* obs, const float* act, const float* rew,
+                       const float* term, const void* states, const float* leaves, cudaStream_t stream) {
+  R2D2_REQUIRE(r && obs && act && rew && term && states && leaves, "null");
+  if (!r->import) { set_last_error("r2d2_replay_import_rows without r2d2_replay_import_begin"); return R2D2_ERR_STATE; }
+  Replay::Import& im = *r->import;
+  if (first != im.received || n <= 0 || first + n > im.packed_rows)
+    return refuse_import(r, stream, "rows [" + std::to_string(first) + ", " + std::to_string(first + n) +
+                                        ") do not continue the " + std::to_string(im.received) + " of " +
+                                        std::to_string(im.packed_rows) + " rows received so far");
+  const long long O = r->cfg.obs_size, A = r->cfg.n_actions, w = 8LL * r->cfg.hidden;
+  const bool src_half = im.storage == R2D2_STATE_F16;
+  if (src_half && !r->half_states) {            // fp16 file, fp32 ring: the halves go through the staging block
+    R2D2_TRY(ensure_stage(r, kStageHead + sizeof(__half) * (size_t)(n * w)));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->stage + kStageHead, states, sizeof(__half) * (size_t)(n * w), cudaMemcpyHostToDevice,
+                                  stream));
+  } else if (!src_half && r->half_states) {     // fp32 file, fp16 ring: ingest's range check, then its rounding
+    const int rc = stage_half_states(r, static_cast<const float*>(states), (size_t)(n * w), stream);
+    if (rc != R2D2_OK) return refuse_import(r, stream, std::string(last_error()));
+  }
+  R2D2_TRY(ensure_stage(r, kStageHead));
+  unsigned long long* d_count = reinterpret_cast<unsigned long long*>(r->stage);
+  R2D2_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(*d_count), stream));
+  for (const Replay::Import::Run& run : im.runs) {
+    const long long lo = std::max(run.src, first), hi = std::min(run.src + run.n, first + n);
+    if (lo >= hi) continue;
+    const long long s = lo - first, d = run.dst + (lo - run.src), k = hi - lo;
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->obs_rows + d * O, obs + s * O, sizeof(float) * (size_t)(k * O), cudaMemcpyHostToDevice, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + d * A, act + s * A, sizeof(float) * (size_t)(k * A), cudaMemcpyHostToDevice, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + d, rew + s, sizeof(float) * (size_t)k, cudaMemcpyHostToDevice, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + d, term + s, sizeof(float) * (size_t)k, cudaMemcpyHostToDevice, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + d, leaves + s, sizeof(float) * (size_t)k, cudaMemcpyHostToDevice, stream));
+    if (src_half == r->half_states) {
+      const size_t b = (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(k * w);
+      void* to = src_half ? static_cast<void*>(r->state_half + d * w) : static_cast<void*>(r->state_rows + d * w);
+      const char* from = static_cast<const char*>(states) + (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(s * w);
+      R2D2_CUDA_TRY(cudaMemcpyAsync(to, from, b, cudaMemcpyHostToDevice, stream));
+    } else if (src_half) {
+      const __half* staged = reinterpret_cast<const __half*>(r->stage + kStageHead) + s * w;
+      states_from_f16_kernel<<<grid_for(k * w / 8), 256, 0, stream>>>(staged, r->state_rows + d * w, k * w);
+      count_launch();
+      R2D2_CUDA_TRY(cudaGetLastError());
+    } else {
+      R2D2_TRY(convert_half_states(r, d, s, k, stream));
+    }
+  }
+  for (size_t e = 0; e < im.kept.size(); ++e) {   // every kept episode's piece of this chunk: its leaves checked
+    const Episode& ep = im.kept[e];
+    const long long lo = std::max(im.kept_src[e], first), hi = std::min(im.kept_src[e] + ep.n_rows, first + n);
+    if (lo >= hi) continue;
+    const long long valid = std::max(0LL, std::min(hi, im.kept_src[e] + ep.n_starts) - lo);
+    count_bad_leaves_kernel<<<grid_for(hi - lo), 256, 0, stream>>>(r->tv.lvl[0] + ep.row_start + (lo - im.kept_src[e]),
+                                                                   hi - lo, valid, d_count);
+    count_launch();
+    R2D2_CUDA_TRY(cudaGetLastError());
+  }
+  unsigned long long bad = 0;
+  R2D2_CUDA_TRY(cudaMemcpyAsync(&bad, d_count, sizeof(bad), cudaMemcpyDeviceToHost, stream));
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));   // the caller may refill its host buffers
+  if (bad)
+    return refuse_import(r, stream, std::to_string(bad) + " leaf value(s) are negative, NaN or infinite, or nonzero on a "
+                                    "row that starts no sequence");
+  im.received += n;
+  return R2D2_OK;
+}
+
+int replay_import_end(Replay* r, cudaStream_t stream) {
+  R2D2_REQUIRE(r, "null");
+  if (!r->import) { set_last_error("r2d2_replay_import_end without r2d2_replay_import_begin"); return R2D2_ERR_STATE; }
+  Replay::Import& im = *r->import;
+  if (im.received != im.packed_rows)
+    return refuse_import(r, stream, "only " + std::to_string(im.received) + " of " + std::to_string(im.packed_rows) +
+                                        " rows arrived");
+  R2D2_TRY(recompute_ancestors(r, 0, r->cfg.capacity_rows, stream));
+  for (const Episode& e : im.kept) {
+    r->episodes.push_back(e);
+    r->by_row[e.row_start] = e.serial;
+  }
+  r->head = im.head;
+  r->sequence_counter = im.sequence_counter;
+  r->next_serial = im.next_serial;
+  r->evicted_total = im.evicted_total;
+  r->rows_used = im.rows_used;
+  delete r->import;
+  r->import = nullptr;
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
   return R2D2_OK;
 }
 

@@ -64,6 +64,16 @@ int replay_update_priorities(Replay* r, const long long* leaf_idx, const float* 
 int replay_stats(Replay* r, r2d2_replay_stats_t* out, cudaStream_t stream);
 int replay_decode(Replay* r, const long long* leaf_host, int n, long long* episode_index, long long* sequence_index);
 int replay_tree_level(Replay* r, int level, const float** dev_ptr, long long* n);
+int replay_export_info(Replay* r, r2d2_replay_snapshot_info* out);
+int replay_export_episodes(Replay* r, long long* row_start, int* n_rows, int* n_starts, long long* serial);
+int replay_export_rows(Replay* r, long long first, long long n, float* obs, float* act, float* rew, float* term,
+                       void* states, float* leaves, cudaStream_t stream);
+int replay_import_begin(Replay* r, const r2d2_replay_snapshot_info* info, const long long* row_start,
+                        const int* n_rows, const int* n_starts, const long long* serial, long long* n_dropped_out,
+                        cudaStream_t stream);
+int replay_import_rows(Replay* r, long long first, long long n, const float* obs, const float* act, const float* rew,
+                       const float* term, const void* states, const float* leaves, cudaStream_t stream);
+int replay_import_end(Replay* r, cudaStream_t stream);
 int replay_attach_group(Replay* r, int rank, int world, int batch, void* const* peer_bases, size_t buffer_bytes);
 int replay_global_write_back(Replay* r, int stage, const long long* leaf, const int* shard, const float* prio,
                              cudaStream_t stream);

@@ -42,9 +42,24 @@ single-critic change is refused.
 Replay storage: R2D2_REPLAY_STATE_DTYPE=float32|float16 (default float32).  float16 keeps the four nets' stored (h, c) of
 every replay row in fp16 - nearly twice the rows in the same HBM (the ring is capped at 60 % of free HBM) - rounded once
 at ingest; an actor file holding a finite state of magnitude >= 65520 is refused whole.  Any other value raises.  The
-replay is not part of the checkpoint, so the setting may change across a resume.
+setting may change across a resume: a replay snapshot in the other type is converted when it is restored.
+
+Replay snapshots: R2D2_REPLAY_SNAPSHOT_INTERVAL (learner steps between snapshots, default 0 = never; a multiple of
+memory_update_interval, 50, else it raises).  After the ingest of every such step the learner writes
+./model_data/replay_snapshot/step{N}/: learner_state.pt (the training state at step N, so the weights and the replay
+belong to the same step), one shard{rank}of{world} per rank (r2d2_b200.replay_snapshot: the HBM shard, its sum-tree
+leaves, its bookkeeping and the CUDA RNG state that draws the next batch) and, once every rank has written, a COMPLETE
+marker from rank 0; the older snapshot directories are then deleted, so at most two are ever on disk.  The loop stalls
+while a snapshot is written.  With R2D2_RESUME=1 and a complete snapshot present, the learner resumes from the newest
+one - its training state (not the top-level learner_state.pt, which may be newer), its own shard and the RNG state -
+so that the run continues bit for bit as if it had not stopped, and the warm-up gate passes at once when the restored
+shard holds enough sequences.  A snapshot written at another world size is refused (re-sharding is not supported).
+Without a complete snapshot the resume loads learner_state.pt alone and the replay starts empty, as before.  Actor files
+not yet ingested stay on disk and are ingested after the resume as usual.
 """
 import os
+import re
+import shutil
 from time import sleep, time
 
 import numpy as np
@@ -66,6 +81,49 @@ def _env_sizes():
         return get_obs(env.reset().observation).shape[1], env.action_spec().shape[0]
     except ImportError:
         return WALKER_OBS, WALKER_ACT
+
+
+SNAPSHOT_INTERVAL_STEP = 50    # memory_update_interval: snapshots are taken after an ingest
+
+
+def snapshot_interval_from_environ(env=None, every=SNAPSHOT_INTERVAL_STEP) -> int:
+    """R2D2_REPLAY_SNAPSHOT_INTERVAL: 0 (the default, never) or a positive multiple of `every`."""
+    v = (os.environ if env is None else env).get("R2D2_REPLAY_SNAPSHOT_INTERVAL", "0")
+    try:
+        n = int(v)
+    except (TypeError, ValueError):
+        n = -1
+    if n < 0 or n % every:
+        raise ValueError("R2D2_REPLAY_SNAPSHOT_INTERVAL must be 0 (never) or a positive multiple of %d (the learner "
+                         "steps between ingests), got %r" % (every, v))
+    return n
+
+
+def snapshot_steps(root) -> list:
+    """[(step, directory)] of the snapshot directories under `root`, oldest first."""
+    if not os.path.isdir(root):
+        return []
+    out = []
+    for name in os.listdir(root):
+        m = re.fullmatch(r"step(\d+)", name)
+        if m and os.path.isdir(os.path.join(root, name)):
+            out.append((int(m.group(1)), os.path.join(root, name)))
+    return sorted(out)
+
+
+def latest_complete_snapshot(root):
+    """(step, directory) of the newest snapshot whose COMPLETE marker exists, or None."""
+    done = [s for s in snapshot_steps(root) if os.path.isfile(os.path.join(s[1], "COMPLETE"))]
+    return done[-1] if done else None
+
+
+def _write_synced(path, write):
+    """write(tmp) then fsync and rename into place: a path that exists is whole."""
+    tmp = "%s.tmp%d" % (path, os.getpid())
+    write(tmp)
+    with open(tmp, "rb+") as f:
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
 
 
 def learner_process(n_actors):
@@ -98,6 +156,7 @@ class Learner:
         self.memory_path = './memory_data/'
         self.model_save_interval = 50
         self.memory_update_interval = 50
+        self.replay_snapshot_interval = snapshot_interval_from_environ(every=self.memory_update_interval)
         self.target_update_inverval = int(os.environ.get("R2D2_TARGET_INTERVAL", 500))
         if self.target_update_inverval < 1:
             raise ValueError("R2D2_TARGET_INTERVAL must be >= 1, got {}".format(self.target_update_inverval))
@@ -126,8 +185,13 @@ class Learner:
                                           device=self.engine.device, priority_exponent=self.priority_exponent,
                                           state_dtype=self.replay_state_dtype)
         self.state_path = self.model_path + 'learner_state.pt'
-        if os.environ.get("R2D2_RESUME", "0") == "1" and os.path.isfile(self.state_path):
-            self.load_checkpoint()                         # every rank loads the same file: replicas stay identical
+        self.snapshot_root = self.model_path + 'replay_snapshot/'
+        if os.environ.get("R2D2_RESUME", "0") == "1":
+            snap = latest_complete_snapshot(self.snapshot_root)
+            if snap is not None:
+                self.resume_from_snapshot(*snap)
+            elif os.path.isfile(self.state_path):
+                self.load_checkpoint()                     # every rank loads the same file: replicas stay identical
         self.save_model()
 
     @staticmethod
@@ -155,6 +219,51 @@ class Learner:
 
     def load_checkpoint(self):
         self.engine.load_training_state(torch.load(self.state_path, map_location="cpu"))
+
+    def _shard_path(self, d):
+        return os.path.join(d, "shard{}of{}".format(self.dist_env.rank, self.dist_env.world))
+
+    def resume_from_snapshot(self, step, d):
+        """The training state of snapshot directory `d` (step `step`), this rank's shard and its CUDA RNG state."""
+        shard = self._shard_path(d)
+        if not os.path.isfile(shard):
+            worlds = sorted({m.group(1) for m in (re.fullmatch(r"shard\d+of(\d+)", f) for f in os.listdir(d)) if m})
+            raise ValueError("replay snapshot {} was written at world size {}, this run has world size {} (re-sharding "
+                             "a replay is not supported)".format(d, " / ".join(worlds) or "?", self.dist_env.world))
+        self.engine.load_training_state(torch.load(os.path.join(d, "learner_state.pt"), map_location="cpu"))
+        self.memory.load_snapshot(shard, world=self.dist_env.world)
+        if self.dist_env.is_main:
+            print("learner: resuming from the replay snapshot of step {} ({} sequences)".format(
+                step, self.memory.sequence_counter))
+
+    def save_replay_snapshot(self):
+        """./model_data/replay_snapshot/step{N}/ at the current step N: learner_state.pt, every rank's shard, then
+        COMPLETE; the older directories go once it is complete."""
+        step = self.engine.step_count
+        d = os.path.join(self.snapshot_root, "step{}".format(step))
+        dist = getattr(self.engine, "_dist", None)
+        barrier = dist.barrier if dist is not None else (lambda: None)
+        if self.dist_env.is_main:
+            for _, old in snapshot_steps(self.snapshot_root):      # an unfinished one from a stopped run
+                if old != d and not os.path.isfile(os.path.join(old, "COMPLETE")):
+                    shutil.rmtree(old, ignore_errors=True)
+            os.makedirs(d, exist_ok=True)
+            if os.path.isfile(os.path.join(d, "COMPLETE")):
+                os.remove(os.path.join(d, "COMPLETE"))
+            state = self.engine.training_state()
+            _write_synced(os.path.join(d, "learner_state.pt"), lambda p: torch.save(state, p))
+        barrier()
+        self.memory.save_snapshot(self._shard_path(d), world=self.dist_env.world, rank=self.dist_env.rank,
+                                  learner_step=step)
+        barrier()
+        if self.dist_env.is_main:
+            def mark(p):
+                with open(p, "w") as f:
+                    f.write("{}\n".format(step))
+            _write_synced(os.path.join(d, "COMPLETE"), mark)
+            for _, old in snapshot_steps(self.snapshot_root):
+                if old != d:
+                    shutil.rmtree(old, ignore_errors=True)
 
     # the four nets as state_dict-compatible views of the engine's flat parameter blocks
     def _sd(self, net):
@@ -210,6 +319,9 @@ class Learner:
             def ingest():
                 self._ingest()
                 barrier()
+        snap = {}
+        if self.replay_snapshot_interval:
+            snap = dict(snapshot=self.save_replay_snapshot, snapshot_every=self.replay_snapshot_interval)
         run_learner_loop(self.engine, self.memory._dev, max_steps=max_steps, ingest_every=self.memory_update_interval,
-                         save_every=self.model_save_interval, ingest=ingest, save=save, log=log)
+                         save_every=self.model_save_interval, ingest=ingest, save=save, log=log, **snap)
         torch.cuda.synchronize()

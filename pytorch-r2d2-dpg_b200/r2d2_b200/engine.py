@@ -886,3 +886,32 @@ class DeviceReplay:
         p, n = c_void_p(), c_longlong()
         nv.check(self.lib.r2d2_replay_tree_level(self._h, level, byref(p), byref(n)))
         return nv.view_f32(p.value, (n.value,), self.device)
+
+    # ---- snapshots (r2d2_b200.replay_snapshot holds the file format) -------------------------------------------------
+    def snapshot_info(self) -> dict:
+        """The shard's sizes, alpha, state storage, capacity and counters (what a snapshot's header records)."""
+        info = nv.ReplaySnapshotInfo()
+        nv.check(self.lib.r2d2_replay_export_info(self._h, byref(info)))
+        return {k: getattr(info, k) for k, _ in nv.ReplaySnapshotInfo._fields_}
+
+    def episodes(self):
+        """The live episodes in FIFO order: (row_start, n_rows, n_starts, serial) int64 arrays."""
+        E = int(self.snapshot_info()["n_episodes"])
+        rs, nr, ns, se = (np.zeros(E, np.int64), np.zeros(E, np.int32), np.zeros(E, np.int32), np.zeros(E, np.int64))
+        P = lambda a: a.ctypes.data_as(c_void_p)  # noqa: E731
+        nv.check(self.lib.r2d2_replay_export_episodes(self._h, P(rs), P(nr), P(ns), P(se)))
+        return rs, nr.astype(np.int64), ns.astype(np.int64), se
+
+    def save_snapshot(self, path, world: int = 1, rank: int = 0, learner_step: int = 0, **kw):
+        """Write the shard, with the device's CUDA RNG state, to one file (replay_snapshot.save).  The stream is idle
+        afterwards; the shard is unchanged."""
+        from . import replay_snapshot
+        return replay_snapshot.save(self, path, world=world, rank=rank, learner_step=learner_step, **kw)
+
+    def load_snapshot(self, path, world: int | None = None, restore_rng: bool = True, **kw) -> dict:
+        """Restore a snapshot into this EMPTY shard (replay_snapshot.load): the same capacity gives back every row, leaf
+        and tree level; another capacity compacts the episodes from row 0 and drops the oldest that do not fit.  A
+        different state storage is converted.  Refused (the shard stays or is left empty) for other sizes, another
+        alpha, another world size when `world` is given, a truncated file, a bad leaf or an fp16 overflow."""
+        from . import replay_snapshot
+        return replay_snapshot.load(self, path, world=world, restore_rng=restore_rng, **kw)

@@ -63,6 +63,13 @@ class ReplayOptions(Structure):
 STATE_F32, STATE_F16 = 0, 1   # ReplayOptions.state_storage (R2D2_STATE_F32 / R2D2_STATE_F16)
 
 
+class ReplaySnapshotInfo(Structure):
+    _fields_ = [(k, c_int) for k in ("obs_size", "n_actions", "hidden", "burn_in", "learning", "n_step",
+                                     "state_storage")] + [("priority_exponent", c_float)] + [
+        (k, c_longlong) for k in ("capacity_rows", "max_sequences", "n_episodes", "head", "sequence_counter",
+                                  "next_serial", "evicted_total", "rows_used")]
+
+
 class LearnerOptions(Structure):
     _fields_ = [("twin_critic", c_int)]
 
@@ -144,6 +151,15 @@ SIGNATURES = {
     "r2d2_replay_stats": (c_int, [c_void_p, POINTER(ReplayStats), c_void_p]),
     "r2d2_replay_decode": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "r2d2_replay_tree_level": (c_int, [c_void_p, c_int, POINTER(c_void_p), POINTER(c_longlong)]),
+    "r2d2_replay_export_info": (c_int, [c_void_p, POINTER(ReplaySnapshotInfo)]),
+    "r2d2_replay_export_episodes": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "r2d2_replay_export_rows": (c_int, [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]),
+    "r2d2_replay_import_begin": (c_int, [c_void_p, POINTER(ReplaySnapshotInfo), c_void_p, c_void_p, c_void_p, c_void_p,
+                                         POINTER(c_longlong), c_void_p]),
+    "r2d2_replay_import_rows": (c_int, [c_void_p, c_longlong, c_longlong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]),
+    "r2d2_replay_import_end": (c_int, [c_void_p, c_void_p]),
     "r2d2_global_layout_for": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, POINTER(GlobalLayout)]),
     "r2d2_replay_attach_group": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_void_p), c_size_t]),
     "r2d2_replay_global_write_back": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -245,4 +261,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "ReplayOptions", "STATE_F32", "STATE_F16", "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "ReplayOptions", "ReplaySnapshotInfo", "STATE_F32", "STATE_F16", "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]

@@ -16,6 +16,10 @@ same steps, so every rank ingests on the same steps.  Its write-back and draw ar
 with nothing drawn ahead of an ingest and the ingests in step, each shard publishes its root after its own write-back
 and ingest, and no rank's draw can meet rows a peer's ingest is still replacing.
 
+Replay snapshots (`snapshot`, every `snapshot_every` steps, a multiple of `ingest_every`) are taken right after the
+ingest of their step.  That step ran sequentially, so no batch is prefetched and no write-back is pending: the shard,
+the nets and the RNG that draws the next batch are all at the same point.
+
 No CUDA, no torch: `engine` needs step(prefetch=None) + leaf_idx / priority attributes, `replay` needs sample_into(engine)
 and update_priorities(leaf_idx, priority) - tests drive it with recording fakes (tests/test_cpu_host.py).
 """
@@ -23,11 +27,15 @@ from __future__ import annotations
 
 
 def run_learner_loop(engine, replay, *, max_steps=None, ingest_every: int, save_every: int, ingest, save,
-                     log=None, log_every: int = 100) -> int:
+                     log=None, log_every: int = 100, snapshot=None, snapshot_every: int = 0) -> int:
     """Returns the number of steps run.  `ingest()` / `save()` are called after the steps whose number is a multiple of
-    `ingest_every` / `save_every` (learner.py:141-149), `log(step)` before every `log_every`-th step (learner.py:79-80)."""
+    `ingest_every` / `save_every` (learner.py:141-149), `log(step)` before every `log_every`-th step (learner.py:79-80),
+    and `snapshot()`, if given, after the ingest of every `snapshot_every`-th step."""
     if ingest_every < 1 or save_every < 1:
         raise ValueError("ingest_every and save_every must be >= 1")
+    if snapshot is not None and (snapshot_every < 1 or snapshot_every % ingest_every):
+        raise ValueError("snapshot_every must be a positive multiple of ingest_every (%d), got %r"
+                         % (ingest_every, snapshot_every))
 
     def next_batch(eng, used):
         replay.update_priorities(used.leaf_idx, used.priority)      # learner.py:135-139
@@ -52,4 +60,6 @@ def run_learner_loop(engine, replay, *, max_steps=None, ingest_every: int, save_
             save()
         if step % ingest_every == 0:
             ingest()                                                # learner.py:144-149 without the sleep stall
+            if snapshot is not None and step % snapshot_every == 0:
+                snapshot()
     return step

@@ -220,6 +220,33 @@ class LearnerReplayMemory:
             self._episodes.popleft()
         self.sequence_counter = int(counter)
 
+    def save_snapshot(self, path, world=1, rank=0, learner_step=0, **kw):
+        """The HBM shard and the CUDA RNG state to one file (r2d2_b200.replay_snapshot); nothing to save before the
+        first ingest."""
+        if self._dev is None:
+            raise ValueError("LearnerReplayMemory.save_snapshot: the replay holds nothing yet")
+        return self._dev.save_snapshot(path, world=world, rank=rank, learner_step=learner_step, **kw)
+
+    def load_snapshot(self, path, world=None, restore_rng=True, **kw):
+        """Restore a snapshot into an empty replay.  The device shard is created from the file's sizes if none exists
+        yet (sizes given to the constructor stay binding), with this replay's capacity and state storage: another ring
+        size compacts the episodes, another storage type is converted.  `priority[e]`, `sample()` and `decode` then
+        see the saved shard.  Returns the snapshot's header fields (replay_snapshot.load)."""
+        from r2d2_b200 import replay_snapshot
+        if self._episodes:
+            raise ValueError("LearnerReplayMemory.load_snapshot: the replay is not empty")
+        with open(path, "rb") as f:
+            h = replay_snapshot.Header.read(f)
+        if (h.burn_in, h.learning, h.n_step) != (self.burn_in_length, self.learning_length, self.n_step):
+            raise ValueError("replay snapshot %s has burn-in / learning / n-step %r, this replay %r" % (
+                path, (h.burn_in, h.learning, h.n_step), (self.burn_in_length, self.learning_length, self.n_step)))
+        dev = self._ensure_device(h.obs_size, h.n_actions, h.hidden)
+        out = dev.load_snapshot(path, world=world, restore_rng=restore_rng, **kw)
+        rs, nr, ns, _ = dev.episodes()
+        self._episodes = deque((int(a), int(b), int(c)) for a, b, c in zip(rs, nr, ns))
+        self.sequence_counter = int(dev.snapshot_info()["sequence_counter"])
+        return out
+
     def add_episode(self, rows, states, priority):
         obs, act, rew, term, st = pack_episode(rows, states, self._hidden)
         dev = self._ensure_device(obs.shape[1], act.shape[1], st.shape[3])
