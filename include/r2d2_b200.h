@@ -231,7 +231,8 @@ int r2d2_replay_set_priority_exponent(r2d2_replay_t* r, float alpha);
 /* Append one episode (replay_memory.py:141-152).  HOST pointers: obs [n_rows,O], act [n_rows,A], rew [n_rows],
  * term [n_rows] (n_rows includes the n_step pad rows, actor.py:173), states [n_state_rows,4,2,H]
  * (actor, target_actor, critic, target_critic) x (hx,cx), priority [n_starts].  Oldest episodes are
- * evicted FIFO when the ring or max_sequences overflows.  Synchronises the stream. */
+ * evicted FIFO when the ring overflows, and after the append while the sequence counter exceeds max_sequences - the
+ * rules of a one-episode r2d2_replay_add_episodes, which may evict the new episode too.  Synchronises the stream. */
 int r2d2_replay_add_episode(r2d2_replay_t* r, const float* obs, const float* act, const float* rew,
                             const float* term, const float* states, int n_rows, int n_state_rows,
                             const float* priority, int n_starts, r2d2_stream_t stream);

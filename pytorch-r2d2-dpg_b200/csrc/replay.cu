@@ -702,8 +702,8 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
     R2D2_CUDA_TRY(cudaMemsetAsync(r->tv.lvl[0] + start + n_starts, 0, sizeof(float) * (size_t)(n_rows - n_starts), stream));
   ranges.push_back({start, (long long)n_rows});
   commit_episode(r, start, n_rows, n_starts);
-  while (r->cfg.max_sequences > 0 && r->sequence_counter > r->cfg.max_sequences && r->episodes.size() > 1)
-    R2D2_TRY(evict_front(r, stream, &ranges));
+  while (r->cfg.max_sequences > 0 && r->sequence_counter > r->cfg.max_sequences && !r->episodes.empty())
+    R2D2_TRY(evict_front(r, stream, &ranges));                               // replay_memory.py:148-152
   R2D2_TRY(refresh_ranges(r, ranges, stream));
   R2D2_CUDA_TRY(cudaStreamSynchronize(stream));  // host buffers may be released by the caller
   return R2D2_OK;
@@ -755,9 +755,12 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     return R2D2_OK;
   };
   for (int e = 0; e < n_episodes; ++e) {
+    // A placement that wraps starts a new run, and its evictions may hit episodes of the pending run: their leaves are
+    // zeroed by a memset that has to follow the run's copy, so the run is flushed before the placement.  Without a wrap
+    // the episode lands right after the run and overlaps none of it.
+    if (r->head + n_rows[e] > r->cfg.capacity_rows) R2D2_TRY(flush());
     long long start = 0;
     R2D2_TRY(place_episode(r, n_rows[e], stream, &ranges, &start));
-    if (run_rows > 0 && start != run_start + run_rows) R2D2_TRY(flush());   // the ring wrapped: new run
     if (run_rows == 0) run_start = start;
     run_rows += n_rows[e];
     commit_episode(r, start, n_rows[e], n_starts[e]);

@@ -1,6 +1,6 @@
 """Helpers shared by the learner tests: error bounds local to one action column, batch tile or unit group, the float64
-oracle of a PathConfig and the one check of an engine against it, bit snapshots of an engine, replay episodes and fed
-runs, the schedule comparisons (pipelined, resumed), the drop-in learner on a fake engine (CPU) and trained for a few
+oracle of a PathConfig and the one check of an engine against it, bit snapshots of an engine, replay episodes, draws
+and fed runs, the schedule comparisons (pipelined, resumed), the drop-in learner on a fake engine (CPU) and trained for a few
 steps (GPU), and the two-GPU NCCL replica check."""
 import contextlib
 import os
@@ -104,6 +104,38 @@ def episode(rng, cfg, E, p_lo=0.01):
             rng.standard_normal(n_rows).astype(np.float32), term,
             (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32),
             rng.uniform(p_lo, 1.0, E - (cfg.burn_in + cfg.learning)).astype(np.float32))
+
+
+def gather_out(cfg, B):
+    import torch
+    T = cfg.rows
+    return {"obs": torch.empty(T, B, cfg.obs, device="cuda"), "act": torch.empty(T, B, cfg.act, device="cuda"),
+            "rew": torch.empty(T, B, device="cuda"), "term": torch.empty(T, B, device="cuda"),
+            "states": torch.empty(4, 2, B, cfg.hidden, device="cuda")}
+
+
+def draw(rp, cfg, kind, u=None, leaf=None, beta=0.6):
+    """One draw of `kind` ("plain", "weighted", "chosen": r2d2_replay_gather at the given leaves) from DeviceReplay rp
+    into fresh buffers, as host arrays: leaf, w (weighted), obs, act, rew, term, states."""
+    import torch
+    from r2d2_b200 import native as nv
+    B = u.numel() if leaf is None else leaf.numel()
+    out = gather_out(cfg, B)
+    ptrs = [nv.dptr(out[k]) for k in ("obs", "act", "rew", "term", "states")]
+    lib, s = nv.lib(), nv.current_stream()
+    if kind == "chosen":
+        nv.check(lib.r2d2_replay_gather(rp._h, nv.dptr(leaf, torch.int64), B, *ptrs, s))
+        out["leaf"] = leaf.clone()
+    else:
+        out["leaf"] = torch.empty(B, dtype=torch.int64, device="cuda")
+        if kind == "plain":
+            nv.check(lib.r2d2_replay_sample(rp._h, nv.dptr(u), B, nv.dptr(out["leaf"], torch.int64), *ptrs, s))
+        else:
+            out["w"] = torch.empty(B, device="cuda")
+            nv.check(lib.r2d2_replay_sample_weighted(rp._h, nv.dptr(u), B, float(beta), nv.dptr(out["leaf"], torch.int64),
+                                                     nv.dptr(out["w"]), *ptrs, s))
+    torch.cuda.synchronize()
+    return {k: v.cpu().numpy() for k, v in out.items()}
 
 
 # ------------------------------------------------------------------------------------------------ float64 oracle

@@ -1,8 +1,6 @@
 """Prioritized replay on the GPU: the priority exponent alpha on the sum-tree leaves, the importance-sampling weights
 of the weighted draw, the weighted critic loss of the learner, and that the defaults (alpha = 1, beta = 0) are the
 unweighted library bit for bit."""
-from collections import deque
-
 import numpy as np
 import pytest
 import torch
@@ -11,6 +9,7 @@ from conftest import rel_l2
 from learner_harness import (REPLAY, SMALL, TOL, assert_two_gpu_replicas_stay_identical, episode, golden_case, oracle_for,
                              port_case, replay_fed_run, trained_dropin_learner)
 from oracle import learner_oracle as lo
+from oracle.replay_model import ReplayModel
 from oracle.sumtree import SumTreeOracle
 
 pytestmark = pytest.mark.gpu
@@ -22,47 +21,27 @@ def eng_mod():
     return engine
 
 
-class RawMirror:
-    """Host mirror of the raw priority behind every leaf (FIFO ring, no sequence cap: evictions come from overlap only,
-    so they always precede the writes of the call that caused them)."""
-
-    def __init__(self, cap):
-        self.raw = np.zeros(cap, np.float32)
-        self.live = deque()
-
-    def add(self, rp, eps):
-        starts, n_ev, _ = rp.add_episodes(eps)
-        news = [(s, e[0].shape[0], e[5]) for s, e in zip(starts, eps)]
-        for _ in range(n_ev):
-            s, n, p = self.live.popleft()
-            self.raw[s:s + len(p)] = 0
-        for s, n, p in news:
-            self.raw[s:s + n] = 0
-            self.raw[s:s + len(p)] = p
-            self.live.append((s, n, p))
-        return n_ev
-
-    def update(self, rp, leaf, prio):
-        rp.update_priorities(torch.as_tensor(leaf).cuda(), torch.as_tensor(prio).cuda())
-        for l, p in zip(leaf, prio):                    # in batch order: the last writer wins
-            self.raw[l] = p
-
-    def starts(self):
-        return np.flatnonzero(self.raw > 0)
+def ingest(rp, model, eps):
+    """One actor file into the shard and into its host model: the same rows, evictions and counter."""
+    got = rp.add_episodes(eps)
+    assert got == model.add_episodes(eps)
+    return got[1]
 
 
 def ingest_wrap_writeback(eng_mod, rp, cfg, cap, seed):
     """Three actor files into a small ring (the third wraps and evicts), then a write-back with duplicate leaves."""
     rng = np.random.default_rng(seed)
-    mirror = RawMirror(cap)
+    model = ReplayModel.for_config(cfg, cap)
     evicted = 0
     for n_eps in (10, 10, 12):
-        evicted += mirror.add(rp, [episode(rng, cfg, int(rng.integers(60, 160))) for _ in range(n_eps)])
-    live = mirror.starts()
+        evicted += ingest(rp, model, [episode(rng, cfg, int(rng.integers(60, 160))) for _ in range(n_eps)])
+    live = model.live_starts()
     leaf = np.concatenate([rng.choice(live, 200), rng.choice(live, 40)])
     leaf[-20:] = leaf[:20]                              # duplicates inside one write-back
-    mirror.update(rp, leaf, rng.uniform(0.05, 3.0, leaf.size).astype(np.float32))
-    return mirror, evicted
+    prio = rng.uniform(0.05, 3.0, leaf.size).astype(np.float32)
+    rp.update_priorities(torch.as_tensor(leaf).cuda(), torch.as_tensor(prio).cuda())
+    model.update_priorities(leaf, prio)
+    return model, evicted
 
 
 def tree_levels(rp):
@@ -106,11 +85,11 @@ def test_leaves_hold_priority_to_the_alpha(eng_mod, alpha):
                              priority_exponent=alpha)
     cap = 3000
     rp = eng_mod.DeviceReplay(cfg, capacity_rows=cap)
-    mirror, evicted = ingest_wrap_writeback(eng_mod, rp, cfg, cap, seed=int(alpha * 10) + 3)
+    model, evicted = ingest_wrap_writeback(eng_mod, rp, cfg, cap, seed=int(alpha * 10) + 3)
     assert evicted > 0
     leaves = rp.tree_level(0).cpu().numpy()[:cap]
-    live = mirror.raw > 0
-    want = mirror.raw[live].astype(np.float64) ** alpha
+    live = model.raw > 0
+    want = model.raw[live].astype(np.float64) ** alpha
     assert np.abs(leaves[live] / want - 1.0).max() < 1e-6
     assert (leaves[~live] == 0).all()
     oracle = SumTreeOracle(cap)
@@ -132,14 +111,14 @@ def test_draws_follow_priority_to_the_alpha(eng_mod, alpha):
                              priority_exponent=alpha)
     rng = np.random.default_rng(21)
     rp = eng_mod.DeviceReplay(cfg, capacity_rows=40000)
-    mirror = RawMirror(40000)
-    mirror.add(rp, [episode(rng, cfg, int(rng.integers(40, 120)), p_lo=2e-3) for _ in range(60)])
-    starts = mirror.starts()
+    model = ReplayModel.for_config(cfg, 40000)
+    ingest(rp, model, [episode(rng, cfg, int(rng.integers(40, 120)), p_lo=2e-3) for _ in range(60)])
+    starts = model.live_starts()
     n = 1 << 20
     u = torch.rand(n, device="cuda", generator=torch.Generator(device="cuda").manual_seed(4))
     cnt = np.bincount(rp.sample_indices(u).cpu().numpy(), minlength=40000)
     assert cnt.sum() == cnt[starts].sum()                                       # only valid starts are drawn
-    p = mirror.raw[starts].astype(np.float64) ** alpha
+    p = model.raw[starts].astype(np.float64) ** alpha
     exp = p / p.sum() * n
     chi2 = ((cnt[starts] - exp) ** 2 / exp).sum() / len(starts)
     assert 0.85 < chi2 < 1.15, chi2

@@ -13,8 +13,8 @@ import pytest
 import torch
 
 from conftest import rel_l2
-from learner_harness import (REPLAY, TOL, assert_same_bits, check_against_oracle, episode, golden_case, port_case,
-                             snapshot)
+from learner_harness import (REPLAY, TOL, assert_same_bits, check_against_oracle, draw, episode, golden_case,
+                             port_case, snapshot)
 from r2d2_b200 import engine as E
 from r2d2_b200 import native as nv
 
@@ -65,34 +65,6 @@ def shard(cfg, dtype, cap, eps=()):
     if eps:
         rp.add_episodes(list(eps))
     return rp
-
-
-def gather_out(cfg, B):
-    T = cfg.rows
-    return {"obs": torch.empty(T, B, cfg.obs, device="cuda"), "act": torch.empty(T, B, cfg.act, device="cuda"),
-            "rew": torch.empty(T, B, device="cuda"), "term": torch.empty(T, B, device="cuda"),
-            "states": torch.empty(4, 2, B, cfg.hidden, device="cuda")}
-
-
-def draw(rp, cfg, kind, u=None, leaf=None, beta=0.6):
-    """One draw of `kind` ("plain", "weighted", "chosen": r2d2_replay_gather at the given leaves) into fresh buffers."""
-    B = u.numel() if leaf is None else leaf.numel()
-    out = gather_out(cfg, B)
-    ptrs = [nv.dptr(out[k]) for k in ("obs", "act", "rew", "term", "states")]
-    lib, s = nv.lib(), nv.current_stream()
-    if kind == "chosen":
-        nv.check(lib.r2d2_replay_gather(rp._h, nv.dptr(leaf, torch.int64), B, *ptrs, s))
-        out["leaf"] = leaf.clone()
-    else:
-        out["leaf"] = torch.empty(B, dtype=torch.int64, device="cuda")
-        if kind == "plain":
-            nv.check(lib.r2d2_replay_sample(rp._h, nv.dptr(u), B, nv.dptr(out["leaf"], torch.int64), *ptrs, s))
-        else:
-            out["w"] = torch.empty(B, device="cuda")
-            nv.check(lib.r2d2_replay_sample_weighted(rp._h, nv.dptr(u), B, float(beta), nv.dptr(out["leaf"], torch.int64),
-                                                     nv.dptr(out["w"]), *ptrs, s))
-    torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in out.items()}
 
 
 def assert_fp16_draw_is_rounded_fp32_draw(a32, a16):
