@@ -214,13 +214,27 @@ int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg);
  * kernels and one stream synchronisation per call; the gather is still one launch. */
 #define R2D2_STATE_F32 0
 #define R2D2_STATE_F16 1
+/* Where the recurrent states [cap,4,2,H] live.  R2D2_STATE_MEMORY_HOST puts them in mapped, page-locked host memory
+ * (cudaHostAlloc, zeroed at creation; no fallback to HBM if it fails) while obs, act, rew, term and the whole sum tree
+ * stay in HBM.  The learner reads the states only at a window's first row, one [8,H] block per drawn sequence (7.7 % of
+ * a cfg-3 batch's gather bytes), so the gather reads them over the host link and the HBM a row needs drops to
+ * 4 (O + A + 2) + 5 bytes.  The batch is bit-identical to the device tier's.  Every write to the host rows is ordered
+ * on the caller's stream: ingest and restore stage the states in a grow-only device block (fp32 storage adds one
+ * device-to-host copy per contiguous ring run, fp16 storage writes the rounded states straight from its conversion
+ * kernel), so a write never overtakes a gather issued earlier on the same stream. */
+#define R2D2_STATE_MEMORY_DEVICE 0
+#define R2D2_STATE_MEMORY_HOST 1
 typedef struct {
   int state_storage;   /* R2D2_STATE_F32 (default) or R2D2_STATE_F16; anything else is R2D2_ERR_ARG */
+  int state_memory;    /* R2D2_STATE_MEMORY_DEVICE (default) or R2D2_STATE_MEMORY_HOST; anything else is R2D2_ERR_ARG */
 } r2d2_replay_options;
-/* options NULL = r2d2_replay_create */
+/* options NULL (or a zeroed struct) = r2d2_replay_create */
 int r2d2_replay_create_ex(r2d2_replay_t** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options);
-/* bytes of device memory the shard holds (rows, tree, and the fp16 mode's staging block once an ingest has used it) */
+/* bytes of device memory the shard holds (rows, tree, and the staging block once an ingest or restore has used it);
+ * under R2D2_STATE_MEMORY_HOST the states are not device memory and are not counted here */
 int r2d2_replay_device_bytes(r2d2_replay_t* r, size_t* out);
+/* bytes of pinned host memory the shard holds: cap * 8 H * sizeof(state) under R2D2_STATE_MEMORY_HOST, else 0 */
+int r2d2_replay_host_bytes(r2d2_replay_t* r, size_t* out);
 int r2d2_replay_destroy(r2d2_replay_t* r);
 /* Priority exponent alpha in [0, 1] (prioritized replay; default 1 = the raw priority): every leaf the shard writes -
  * ingest and r2d2_replay_update_priorities - holds p > 0 ? p^alpha : 0, so P(start) = p^alpha / sum p^alpha and rows

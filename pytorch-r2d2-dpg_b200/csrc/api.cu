@@ -233,10 +233,14 @@ int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg) {
   return replay_create(reinterpret_cast<Replay**>(out), cfg);
 }
 int r2d2_replay_create_ex(r2d2_replay_t** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options) {
-  return replay_create(reinterpret_cast<Replay**>(out), cfg, options ? options->state_storage : R2D2_STATE_F32);
+  return replay_create(reinterpret_cast<Replay**>(out), cfg, options ? options->state_storage : R2D2_STATE_F32,
+                       options ? options->state_memory : R2D2_STATE_MEMORY_DEVICE);
 }
 int r2d2_replay_device_bytes(r2d2_replay_t* r, size_t* out) {
   return replay_device_bytes(reinterpret_cast<Replay*>(r), out);
+}
+int r2d2_replay_host_bytes(r2d2_replay_t* r, size_t* out) {
+  return replay_host_bytes(reinterpret_cast<Replay*>(r), out);
 }
 int r2d2_replay_destroy(r2d2_replay_t* r) { return replay_destroy(reinterpret_cast<Replay*>(r)); }
 int r2d2_replay_set_priority_exponent(r2d2_replay_t* r, float alpha) {

@@ -2,7 +2,8 @@
 //
 // HBM layout (SoA, one "row" per stored env step incl. the n_step pad rows of actor.py:173):
 //   obs_rows [cap,O]  act_rows [cap,A]  rew_rows [cap]  term_rows [cap]  state_rows [cap,4,2,H]
-// state_rows is fp32, or fp16 under R2D2_STATE_F16 (rounded once at ingest, widened back to fp32 by the gather).
+// state_rows is fp32, or fp16 under R2D2_STATE_F16 (rounded once at ingest, widened back to fp32 by the gather); under
+// R2D2_STATE_MEMORY_HOST it lives in mapped, page-locked host memory and everything else stays in HBM.
 // Episodes occupy contiguous row ranges of a ring; FIFO eviction (replay_memory.py:148-152).
 // Sum tree: one leaf per ROW (priority 0 for rows that are not valid sequence starts), fan-out 32:
 // every node is the left-to-right fp32 sum of its 32 children (one 128-byte line), so the tree has
@@ -12,6 +13,7 @@
 #include <float.h>
 
 #include <algorithm>
+#include <cstring>
 #include <deque>
 #include <map>
 #include <vector>
@@ -353,14 +355,99 @@ __device__ __forceinline__ void warp_widen_row(const __half* __restrict__ src, f
   }
 }
 
+// Host-tier state rows (R2D2_STATE_MEMORY_HOST): the same sub-row copies, but every lane issues all its loads of a
+// chunk before its first store, so a warp's whole request (2 KB of fp32 or 1 KB of fp16 states at H = 512: four or two
+// 16-byte loads per lane) is in flight over the host link at once.  Plain loads: the rows are mapped host memory.
+constexpr int kHostLoads = 4;   // loads in flight per lane
+
+template <typename V>
+__device__ __forceinline__ void load_chunk(const V* __restrict__ src, V (&v)[kHostLoads], int k0, int n, int lane) {
+#pragma unroll
+  for (int j = 0; j < kHostLoads; ++j) {
+    const int k = k0 + j * 32 + lane;
+    if (k < n) v[j] = src[k];
+  }
+}
+
+__device__ __forceinline__ void host_copy_row(const float* __restrict__ src, float* __restrict__ dst, int n, int lane) {
+  if ((n & 3) == 0) {
+    const float4* s4 = reinterpret_cast<const float4*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int k0 = 0; k0 < (n >> 2); k0 += 32 * kHostLoads) {
+      float4 v[kHostLoads];
+      load_chunk(s4, v, k0, n >> 2, lane);
+#pragma unroll
+      for (int j = 0; j < kHostLoads; ++j)
+        if (k0 + j * 32 + lane < (n >> 2)) d4[k0 + j * 32 + lane] = v[j];
+    }
+  } else {
+    for (int k0 = 0; k0 < n; k0 += 32 * kHostLoads) {
+      float v[kHostLoads];
+      load_chunk(src, v, k0, n, lane);
+#pragma unroll
+      for (int j = 0; j < kHostLoads; ++j)
+        if (k0 + j * 32 + lane < n) dst[k0 + j * 32 + lane] = v[j];
+    }
+  }
+}
+
+__device__ __forceinline__ float4 widen4(uint2 v) {
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+
+// warp_widen_row's three routes (16-byte, 8-byte, scalar by H % 8 and H % 4) with the loads of a chunk first
+__device__ __forceinline__ void host_widen_row(const __half* __restrict__ src, float* __restrict__ dst, int n, int lane) {
+  if ((n & 7) == 0) {
+    const uint4* s8 = reinterpret_cast<const uint4*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int k0 = 0; k0 < (n >> 3); k0 += 32 * kHostLoads) {
+      uint4 v[kHostLoads];
+      load_chunk(s8, v, k0, n >> 3, lane);
+#pragma unroll
+      for (int j = 0; j < kHostLoads; ++j) {
+        const int k = k0 + j * 32 + lane;
+        if (k < (n >> 3)) {
+          d4[2 * k] = widen4(make_uint2(v[j].x, v[j].y));
+          d4[2 * k + 1] = widen4(make_uint2(v[j].z, v[j].w));
+        }
+      }
+    }
+  } else if ((n & 3) == 0) {
+    const uint2* s4 = reinterpret_cast<const uint2*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int k0 = 0; k0 < (n >> 2); k0 += 32 * kHostLoads) {
+      uint2 v[kHostLoads];
+      load_chunk(s4, v, k0, n >> 2, lane);
+#pragma unroll
+      for (int j = 0; j < kHostLoads; ++j)
+        if (k0 + j * 32 + lane < (n >> 2)) d4[k0 + j * 32 + lane] = widen4(v[j]);
+    }
+  } else {
+    for (int k0 = 0; k0 < n; k0 += 32 * kHostLoads) {
+      __half v[kHostLoads];
+      load_chunk(src, v, k0, n, lane);
+#pragma unroll
+      for (int j = 0; j < kHostLoads; ++j)
+        if (k0 + j * 32 + lane < n) dst[k0 + j * 32 + lane] = __half2float(v[j]);
+    }
+  }
+}
+
 // kHalfStates: state_rows holds __half (r2d2_replay_options.state_storage = R2D2_STATE_F16); the batch stays fp32.
-template <bool kPerDraw = false, bool kHalfStates = false>
-__global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
+// kHostStates (R2D2_STATE_MEMORY_HOST): state_rows is mapped host memory.  The 8 B state tasks then come FIRST (task
+// nh * B + b; row task t * B + b follows at 8 B + t * B + b), so that every host read is in flight from the start of the
+// launch and overlaps the HBM row copies instead of adding a host round trip after them; the row tasks are unchanged.
+// The two tiers are separate kernels (gather_batch_kernel and gather_host_states_kernel) over this one body.
+template <bool kPerDraw, bool kHalfStates, bool kHostStates>
+__device__ __forceinline__ void gather_batch(GatherParams g) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const long long row_tasks = (long long)g.T * g.B;
   const long long total = row_tasks + (g.states ? (long long)8 * g.B : 0);
+  const int lead = kHostStates && g.states ? 8 : 0;                       // state "rows" before the row tasks
   int t = (int)(warp0 / g.B), b = (int)(warp0 % g.B);                    // one division per warp, then carried
   const int dt = (int)(n_warps / g.B), db = (int)(n_warps % g.B);
   for (long long task = warp0; task < total; task += n_warps) {
@@ -377,15 +464,21 @@ __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
     }
     if (kPerDraw && leaf < 0) {
       // another shard's draw
-    } else if (task < row_tasks) {
-      const long long r = leaf + t;
-      const long long o = (long long)t * ld + col;
+    } else if (kHostStates ? t >= lead : task < row_tasks) {
+      const long long r = leaf + (t - lead);
+      const long long o = (long long)(t - lead) * ld + col;
       if (obs) warp_copy_row(g.obs_rows + r * g.O, obs + o * g.O, g.O, lane);
       if (act) warp_copy_row(g.act_rows + r * g.A, act + o * g.A, g.A, lane);
       if (lane == 0) {
         if (rew) rew[o] = __ldg(g.rew_rows + r);
         if (term) term[o] = __ldg(g.term_rows + r);
       }
+    } else if (kHostStates) {
+      if (kHalfStates)
+        host_widen_row(reinterpret_cast<const __half*>(g.state_rows) + (leaf * 8 + t) * g.H,
+                       states + ((long long)t * ld + col) * g.H, g.H, lane);
+      else
+        host_copy_row(g.state_rows + (leaf * 8 + t) * g.H, states + ((long long)t * ld + col) * g.H, g.H, lane);
     } else if (kHalfStates) {
       warp_widen_row(reinterpret_cast<const __half*>(g.state_rows) + (leaf * 8 + (t - g.T)) * g.H,
                      states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
@@ -395,6 +488,16 @@ __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
     t += dt; b += db;
     if (b >= g.B) { b -= g.B; ++t; }
   }
+}
+
+template <bool kPerDraw = false, bool kHalfStates = false>
+__global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
+  gather_batch<kPerDraw, kHalfStates, false>(g);
+}
+
+template <bool kPerDraw = false, bool kHalfStates = false>
+__global__ void __launch_bounds__(256) gather_host_states_kernel(GatherParams g) {
+  gather_batch<kPerDraw, kHalfStates, true>(g);
 }
 
 int grid_for(long long total) {
@@ -424,6 +527,11 @@ struct Replay {
   char* stage = nullptr;
   size_t stage_bytes = 0;
   size_t device_bytes = 0;   // every device allocation of the shard (rows, tree, staging)
+  // R2D2_STATE_MEMORY_HOST: state_rows / state_half point into mapped, page-locked host memory (host_alloc, freed with
+  // cudaFreeHost); ingest and restore stage the states in the device block first, so every write is stream-ordered
+  bool host_states = false;
+  void* host_alloc = nullptr;
+  size_t host_bytes = 0;
   std::vector<float*> level_alloc;
   TreeView tv;
   std::deque<Episode> episodes;
@@ -468,17 +576,38 @@ static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leav
   return R2D2_OK;
 }
 
-int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage) {
+int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage, int state_memory) {
   R2D2_REQUIRE(out && cfg, "null");
   R2D2_REQUIRE(cfg->obs_size > 0 && cfg->n_actions > 0 && cfg->hidden > 0, "sizes");
   R2D2_REQUIRE(cfg->capacity_rows > 0, "capacity_rows");
   R2D2_REQUIRE(state_storage == R2D2_STATE_F32 || state_storage == R2D2_STATE_F16,
                "state_storage is R2D2_STATE_F32 or R2D2_STATE_F16");
+  R2D2_REQUIRE(state_memory == R2D2_STATE_MEMORY_DEVICE || state_memory == R2D2_STATE_MEMORY_HOST,
+               "state_memory is R2D2_STATE_MEMORY_DEVICE or R2D2_STATE_MEMORY_HOST");
   Replay* r = new Replay();
   r->cfg = *cfg;
   r->rows_per_window = cfg->burn_in + cfg->learning + cfg->n_step;
   r->half_states = state_storage == R2D2_STATE_F16;
+  r->host_states = state_memory == R2D2_STATE_MEMORY_HOST;
   const long long cap = cfg->capacity_rows;
+  if (r->host_states) {   // first, so that a refusal leaves nothing allocated
+    const size_t bytes = (r->half_states ? sizeof(__half) : sizeof(float)) * (size_t)cap * 8 * cfg->hidden;
+    void* dev = nullptr;
+    cudaError_t e = cudaHostAlloc(&r->host_alloc, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&dev, r->host_alloc, 0);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      if (r->host_alloc) cudaFreeHost(r->host_alloc);
+      delete r;
+      set_last_error("replay shard: " + std::to_string(bytes) + " bytes of mapped pinned host memory for the recurrent "
+                     "states could not be allocated (" + cudaGetErrorString(e) + ")");
+      return R2D2_ERR_CUDA;
+    }
+    memset(r->host_alloc, 0, bytes);   // nothing can be in flight on a buffer that was just allocated
+    r->host_bytes = bytes;
+    if (r->half_states) r->state_half = static_cast<__half*>(dev);
+    else r->state_rows = static_cast<float*>(dev);
+  }
   auto dmalloc_bytes = [&](void** p, size_t bytes) -> int {
     R2D2_CUDA_TRY(cudaMalloc(p, bytes));
     R2D2_CUDA_TRY(cudaMemset(*p, 0, bytes));
@@ -491,9 +620,10 @@ int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage
   int rc = R2D2_OK;
   if ((rc = dmalloc(&r->obs_rows, cap * cfg->obs_size)) || (rc = dmalloc(&r->act_rows, cap * cfg->n_actions)) ||
       (rc = dmalloc(&r->rew_rows, cap)) || (rc = dmalloc(&r->term_rows, cap)) ||
-      (rc = r->half_states ? dmalloc_bytes(reinterpret_cast<void**>(&r->state_half), sizeof(__half) * (size_t)cap * 8 * cfg->hidden)
-                           : dmalloc(&r->state_rows, cap * 8 * cfg->hidden))) {
-    delete r;
+      (!r->host_states &&
+       (rc = r->half_states ? dmalloc_bytes(reinterpret_cast<void**>(&r->state_half), sizeof(__half) * (size_t)cap * 8 * cfg->hidden)
+                            : dmalloc(&r->state_rows, cap * 8 * cfg->hidden)))) {
+    replay_destroy(r);
     return rc;
   }
   // levels: n[0] = leaves, n[l+1] = ceil(n[l]/32), last level has one node (the total)
@@ -504,7 +634,7 @@ int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage
     const long long parents = (n + TREE_K - 1) / TREE_K;
     const long long alloc = (n > 1) ? parents * TREE_K : TREE_K;
     float* p = nullptr;
-    if ((rc = dmalloc(&p, alloc))) { delete r; return rc; }
+    if ((rc = dmalloc(&p, alloc))) { replay_destroy(r); return rc; }
     r->level_alloc.push_back(p);
     r->tv.lvl[levels] = p;
     r->tv.n[levels] = n;
@@ -589,10 +719,35 @@ static int convert_half_states(Replay* r, long long ring_row, long long first, l
   return R2D2_OK;
 }
 
+// Host tier: the call's packed fp32 states (n values, then zeros up to n_total) in the staging block, so that they reach
+// the mapped host rows by stream-ordered work (store_staged_states).  fp16 storage stages through ingest's range check.
+static int stage_host_states(Replay* r, const float* states, size_t n, size_t n_total, cudaStream_t stream) {
+  R2D2_TRY(ensure_stage(r, kStageHead + sizeof(float) * n_total));
+  if (r->half_states)
+    R2D2_TRY(stage_half_states(r, states, n, stream));
+  else if (n > 0)
+    R2D2_CUDA_TRY(cudaMemcpyAsync(staged_states(r), states, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+  if (n_total > n) R2D2_CUDA_TRY(cudaMemsetAsync(staged_states(r) + n, 0, sizeof(float) * (n_total - n), stream));
+  return R2D2_OK;
+}
+
+// Host tier: staged rows [first, first + n_rows) into ring rows [ring_row, ring_row + n_rows).  fp16 storage rounds them
+// with states_to_f16_kernel, which stores into the mapped rows; fp32 storage is one device-to-host copy.
+static int store_staged_states(Replay* r, long long ring_row, long long first, long long n_rows, cudaStream_t stream) {
+  if (r->half_states) return convert_half_states(r, ring_row, first, n_rows, stream);
+  const long long w = 8LL * r->cfg.hidden;
+  if (n_rows > 0)
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + ring_row * w, staged_states(r) + first * w,
+                                  sizeof(float) * (size_t)(n_rows * w), cudaMemcpyDefault, stream));
+  return R2D2_OK;
+}
+
 int replay_destroy(Replay* r) {
   if (!r) return R2D2_OK;
-  cudaFree(r->obs_rows); cudaFree(r->act_rows); cudaFree(r->rew_rows); cudaFree(r->term_rows); cudaFree(r->state_rows);
-  cudaFree(r->state_half); cudaFree(r->stage);
+  cudaFree(r->obs_rows); cudaFree(r->act_rows); cudaFree(r->rew_rows); cudaFree(r->term_rows);
+  if (r->host_states) cudaFreeHost(r->host_alloc);
+  else { cudaFree(r->state_rows); cudaFree(r->state_half); }
+  cudaFree(r->stage);
   for (float* p : r->level_alloc) cudaFree(p);
   delete r->group;
   delete r->import;
@@ -673,7 +828,10 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
   R2D2_REQUIRE(n_state_rows >= n_starts && n_state_rows <= n_rows, "state rows");
   R2D2_REQUIRE(n_starts == 0 || priority, "priority");
   const int O = r->cfg.obs_size, A = r->cfg.n_actions, H = r->cfg.hidden;
-  if (r->half_states) R2D2_TRY(stage_half_states(r, states, (size_t)n_state_rows * 8 * H, stream));
+  if (r->host_states)
+    R2D2_TRY(stage_host_states(r, states, (size_t)n_state_rows * 8 * H, (size_t)n_rows * 8 * H, stream));
+  else if (r->half_states)
+    R2D2_TRY(stage_half_states(r, states, (size_t)n_state_rows * 8 * H, stream));
   RangeList ranges;
   long long start = 0;
   R2D2_TRY(place_episode(r, n_rows, stream, &ranges, &start));
@@ -681,7 +839,9 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
   R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + start * A, act, sizeof(float) * (size_t)n_rows * A, cudaMemcpyHostToDevice, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + start, rew, sizeof(float) * (size_t)n_rows, cudaMemcpyHostToDevice, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + start, term, sizeof(float) * (size_t)n_rows, cudaMemcpyHostToDevice, stream));
-  if (r->half_states) {
+  if (r->host_states) {
+    R2D2_TRY(store_staged_states(r, start, 0, n_rows, stream));   // the rows past n_state_rows were staged as zeros
+  } else if (r->half_states) {
     R2D2_TRY(convert_half_states(r, start, 0, n_state_rows, stream));
     if (n_state_rows < n_rows)
       R2D2_CUDA_TRY(cudaMemsetAsync(r->state_half + (start + n_state_rows) * 8 * H, 0,
@@ -726,10 +886,11 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     R2D2_REQUIRE(n_starts[e] >= 0 && n_starts[e] <= n_rows[e] - r->rows_per_window + 1, "n_starts exceeds valid window starts");
     R2D2_REQUIRE(n_rows[e] <= r->cfg.capacity_rows, "episode larger than the ring");
   }
-  if (r->half_states && n_episodes > 0) {
+  if ((r->half_states || r->host_states) && n_episodes > 0) {
     long long R = 0;
     for (int e = 0; e < n_episodes; ++e) R += n_rows[e];
-    R2D2_TRY(stage_half_states(r, states, (size_t)R * 8 * H, stream));
+    if (r->host_states) R2D2_TRY(stage_host_states(r, states, (size_t)R * 8 * H, (size_t)R * 8 * H, stream));
+    else R2D2_TRY(stage_half_states(r, states, (size_t)R * 8 * H, stream));
   }
   const long long evicted0 = r->evicted_total;
   RangeList ranges;
@@ -742,7 +903,9 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + run_start * A, act + src * A, sizeof(float) * n * A, cudaMemcpyHostToDevice, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + run_start, rew + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + run_start, term + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    if (r->half_states)
+    if (r->host_states)
+      R2D2_TRY(store_staged_states(r, run_start, src, run_rows, stream));
+    else if (r->half_states)
       R2D2_TRY(convert_half_states(r, run_start, src, run_rows, stream));
     else
       R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + run_start * 8 * H, states + src * 8 * H, sizeof(float) * n * 8 * H,
@@ -788,6 +951,12 @@ int replay_device_bytes(Replay* r, size_t* out) {
   return R2D2_OK;
 }
 
+int replay_host_bytes(Replay* r, size_t* out) {
+  R2D2_REQUIRE(r && out, "null");
+  *out = r->host_bytes;
+  return R2D2_OK;
+}
+
 int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, float* act, float* rew, float* term,
                   float* states, cudaStream_t stream) {
   R2D2_REQUIRE(r && leaf_idx && batch > 0, "args");
@@ -799,7 +968,11 @@ int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, f
     g.obs = obs; g.act = act; g.rew = rew; g.term = term; g.states = states;
     g.T = T; g.B = batch; g.O = O; g.A = A; g.H = H;
     const long long tasks = (long long)T * batch + (states ? (long long)8 * batch : 0);
-    if (r->half_states)
+    if (r->host_states && r->half_states)
+      gather_host_states_kernel<false, true><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
+    else if (r->host_states)
+      gather_host_states_kernel<false, false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
+    else if (r->half_states)
       gather_batch_kernel<false, true><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
     else
       gather_batch_kernel<false, false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
@@ -924,10 +1097,12 @@ int replay_export_rows(Replay* r, long long first, long long n, float* obs, floa
   R2D2_CUDA_TRY(cudaMemcpyAsync(act, r->act_rows + first * A, sizeof(float) * k * A, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(rew, r->rew_rows + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(term, r->term_rows + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
+  // cudaMemcpyDefault: the host tier's rows are host memory.  Only ingest and restore write them, and both synchronise
+  // the stream before they return, so no write to these rows is in flight here
   if (r->half_states)
-    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_half + first * w, sizeof(__half) * k * w, cudaMemcpyDeviceToHost, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_half + first * w, sizeof(__half) * k * w, cudaMemcpyDefault, stream));
   else
-    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_rows + first * w, sizeof(float) * k * w, cudaMemcpyDeviceToHost, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_rows + first * w, sizeof(float) * k * w, cudaMemcpyDefault, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(leaves, r->tv.lvl[0] + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
   return R2D2_OK;
@@ -1049,6 +1224,10 @@ int replay_import_rows(Replay* r, long long first, long long n, const float* obs
   } else if (!src_half && r->half_states) {     // fp32 file, fp16 ring: ingest's range check, then its rounding
     const int rc = stage_half_states(r, static_cast<const float*>(states), (size_t)(n * w), stream);
     if (rc != R2D2_OK) return refuse_import(r, stream, std::string(last_error()));
+  } else if (r->host_states) {                  // same type, host tier: staged, then device-to-host copies
+    const size_t b = (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(n * w);
+    R2D2_TRY(ensure_stage(r, kStageHead + b));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->stage + kStageHead, states, b, cudaMemcpyHostToDevice, stream));
   }
   R2D2_TRY(ensure_stage(r, kStageHead));
   unsigned long long* d_count = reinterpret_cast<unsigned long long*>(r->stage);
@@ -1065,8 +1244,9 @@ int replay_import_rows(Replay* r, long long first, long long n, const float* obs
     if (src_half == r->half_states) {
       const size_t b = (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(k * w);
       void* to = src_half ? static_cast<void*>(r->state_half + d * w) : static_cast<void*>(r->state_rows + d * w);
-      const char* from = static_cast<const char*>(states) + (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(s * w);
-      R2D2_CUDA_TRY(cudaMemcpyAsync(to, from, b, cudaMemcpyHostToDevice, stream));
+      const char* base = r->host_states ? r->stage + kStageHead : static_cast<const char*>(states);
+      const char* from = base + (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(s * w);
+      R2D2_CUDA_TRY(cudaMemcpyAsync(to, from, b, cudaMemcpyDefault, stream));
     } else if (src_half) {
       const __half* staged = reinterpret_cast<const __half*>(r->stage + kStageHead) + s * w;
       states_from_f16_kernel<<<grid_for(k * w / 8), 256, 0, stream>>>(staged, r->state_rows + d * w, k * w);
@@ -1251,7 +1431,11 @@ int replay_global_draw(Replay* r, int stage, int slot, int weighted, float beta,
     gp.off_term = so + g.lay.off_term; gp.off_states = so + g.lay.off_states;
     gp.dst = g.peers;
     const long long tasks = (long long)(gp.T + 8) * gp.B;
-    if (r->half_states)
+    if (r->host_states && r->half_states)
+      gather_host_states_kernel<true, true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
+    else if (r->host_states)
+      gather_host_states_kernel<true, false><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
+    else if (r->half_states)
       gather_batch_kernel<true, true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
     else
       gather_batch_kernel<true, false><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);

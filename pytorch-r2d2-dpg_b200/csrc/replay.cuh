@@ -43,8 +43,10 @@ int global_receive(const GlobalPeers& p, const GlobalLayout& lay, int world, int
                    float beta, unsigned epoch, cudaStream_t st);
 
 struct Replay;
-int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage = R2D2_STATE_F32);
+int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage = R2D2_STATE_F32,
+                  int state_memory = R2D2_STATE_MEMORY_DEVICE);
 int replay_device_bytes(Replay* r, size_t* out);
+int replay_host_bytes(Replay* r, size_t* out);
 int replay_destroy(Replay* r);
 int replay_set_priority_exponent(Replay* r, float alpha);
 int replay_add_episode(Replay* r, const float* obs, const float* act, const float* rew, const float* term,

@@ -43,6 +43,13 @@ Replay storage: R2D2_REPLAY_STATE_DTYPE=float32|float16 (default float32).  floa
 every replay row in fp16 - nearly twice the rows in the same HBM (the ring is capped at 60 % of free HBM) - rounded once
 at ingest; an actor file holding a finite state of magnitude >= 65520 is refused whole.  Any other value raises.  The
 setting may change across a resume: a replay snapshot in the other type is converted when it is restored.
+R2D2_REPLAY_HOST_GB (default 0: the states stay in HBM) is the pinned host memory, in GB per rank, a replay shard may
+use for those states: above 0 every row's (h, c) lives in mapped, page-locked host memory and only obs, act, reward,
+terminal and the sum tree take HBM (1,585 bytes per row at obs 376, act 17), so the reference's 5 M sequences fit one
+GPU.  The ring is then the least of the wanted rows, 60 % of the free HBM and the rows this budget holds (16 H bytes
+per row in float16, 32 H in float32); the learner prints which applies.  The gather reads each drawn sequence's start
+states over the host link and the batch is bit-identical.  A negative, non-finite or non-numeric value raises.  It may
+change across a resume: snapshots do not depend on where the states live.
 
 Replay snapshots: R2D2_REPLAY_SNAPSHOT_INTERVAL (learner steps between snapshots, default 0 = never; a multiple of
 memory_update_interval, 50, else it raises).  After the ingest of every such step the learner writes
@@ -57,6 +64,7 @@ shard holds enough sequences.  A snapshot written at another world size is refus
 Without a complete snapshot the resume loads learner_state.pt alone and the replay starts empty, as before.  Actor files
 not yet ingested stay on disk and are ingested after the resume as usual.
 """
+import math
 import os
 import re
 import shutil
@@ -166,6 +174,7 @@ class Learner:
         self.target_tau = float(os.environ.get("R2D2_TARGET_TAU", 1.0))
         self.grad_clip_norm = float(os.environ.get("R2D2_GRAD_CLIP", 0.0))
         self.replay_state_dtype = self._replay_state_dtype_from_environ()
+        self.replay_host_gb = self._replay_host_gb_from_environ()
         from r2d2_b200 import td3_options, td_options
         self.td_options = td_options.from_environ()
         self.td3_options = td3_options.from_environ()
@@ -177,13 +186,14 @@ class Learner:
                          value_rescaling=self.td_options.value_rescaling, rescaling_eps=self.td_options.rescaling_eps,
                          priority_metric=self.td_options.priority_metric, **self.td3_options,
                          global_sampling=self._global_sampling_from_environ(),
-                         replay_state_dtype=self.replay_state_dtype)
+                         replay_state_dtype=self.replay_state_dtype,
+                         replay_state_memory="host" if self.replay_host_gb > 0 else "device")
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
                                           obs_size=self.obs_size, n_actions=self.n_actions, hidden=self.hidden,
                                           device=self.engine.device, priority_exponent=self.priority_exponent,
-                                          state_dtype=self.replay_state_dtype)
+                                          state_dtype=self.replay_state_dtype, host_gb=self.replay_host_gb)
         self.state_path = self.model_path + 'learner_state.pt'
         self.snapshot_root = self.model_path + 'replay_snapshot/'
         if os.environ.get("R2D2_RESUME", "0") == "1":
@@ -207,6 +217,18 @@ class Learner:
         if v not in ("float32", "float16"):
             raise ValueError("R2D2_REPLAY_STATE_DTYPE must be float32 or float16, got {!r}".format(v))
         return v
+
+    @staticmethod
+    def _replay_host_gb_from_environ():
+        v = os.environ.get("R2D2_REPLAY_HOST_GB", "0")
+        try:
+            gb = float(v)
+        except (TypeError, ValueError):
+            gb = float("nan")
+        if not (math.isfinite(gb) and gb >= 0):
+            raise ValueError("R2D2_REPLAY_HOST_GB must be a finite number of GB >= 0 (0 = recurrent states in HBM), "
+                             "got {!r}".format(v))
+        return gb
 
     def save_checkpoint(self):
         """Resumable state next to model.pt: nets + both Adam moment sets + step counter (the reference's model.pt has

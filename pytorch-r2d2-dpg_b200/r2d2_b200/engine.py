@@ -24,6 +24,8 @@ from . import td_options
 
 # PathConfig.replay_state_dtype -> r2d2_replay_options.state_storage
 REPLAY_STATE_DTYPES = {"float32": nv.STATE_F32, "float16": nv.STATE_F16}
+# PathConfig.replay_state_memory -> r2d2_replay_options.state_memory
+REPLAY_STATE_MEMORY = {"device": nv.STATE_MEMORY_DEVICE, "host": nv.STATE_MEMORY_HOST}
 
 PARAM_KEYS = ("l1.weight", "l1.bias", "l2.weight_ih", "l2.weight_hh", "l2.bias_ih", "l2.bias_hh",
               "l3.weight", "l3.bias")
@@ -60,7 +62,11 @@ class PathConfig:
     `replay_state_dtype` (replay shard, include/r2d2_b200.h r2d2_replay_options): "float32" (default) stores the four
     nets' recurrent states of every row in fp32; "float16" stores them in fp16 - nearly twice the rows in the same HBM -
     rounded once at ingest and widened exactly by the gather, so training sees the fp16-rounded states.  An actor file
-    with a finite state of magnitude >= 65520 is refused whole in that mode."""
+    with a finite state of magnitude >= 65520 is refused whole in that mode.
+
+    `replay_state_memory` (replay shard): "device" (default) keeps those states in HBM; "host" keeps them in mapped,
+    page-locked host memory while the rest of every row and the sum tree stay in HBM.  The gather then reads each drawn
+    sequence's start states over the host link; the batch is bit-identical to the device tier's."""
     obs: int
     act: int
     hidden: int = 128
@@ -86,6 +92,7 @@ class PathConfig:
     target_noise_seed: int = 0
     global_sampling: bool = False
     replay_state_dtype: str = "float32"
+    replay_state_memory: str = "device"
 
     def __post_init__(self):
         for name, least in (("burn_in", 0), ("learning", 2), ("n_step", 1)):
@@ -98,6 +105,9 @@ class PathConfig:
         if not isinstance(self.replay_state_dtype, str) or self.replay_state_dtype not in REPLAY_STATE_DTYPES:
             raise ValueError("replay_state_dtype must be one of %s, got %r" % (", ".join(REPLAY_STATE_DTYPES),
                                                                               self.replay_state_dtype))
+        if not isinstance(self.replay_state_memory, str) or self.replay_state_memory not in REPLAY_STATE_MEMORY:
+            raise ValueError("replay_state_memory must be one of %s, got %r" % (", ".join(REPLAY_STATE_MEMORY),
+                                                                               self.replay_state_memory))
         for name in ("twin_critic", "global_sampling"):
             if not isinstance(getattr(self, name), bool):
                 raise ValueError("%s must be True or False, got %r" % (name, getattr(self, name)))
@@ -697,7 +707,7 @@ class DeviceReplay:
         rc = nv.ReplayConfig(cfg.obs, cfg.act, cfg.hidden, cfg.burn_in, cfg.learning, cfg.n_step,
                              int(capacity_rows), int(max_sequences))
         self._h = c_void_p()
-        opt = nv.ReplayOptions(REPLAY_STATE_DTYPES[cfg.replay_state_dtype])
+        opt = nv.ReplayOptions(REPLAY_STATE_DTYPES[cfg.replay_state_dtype], REPLAY_STATE_MEMORY[cfg.replay_state_memory])
         nv.check(self.lib.r2d2_replay_create_ex(byref(self._h), byref(rc), byref(opt)))
         if cfg.priority_exponent != 1.0:   # leaves hold p^alpha; actors and write-backs keep passing raw priorities
             nv.check(self.lib.r2d2_replay_set_priority_exponent(self._h, float(cfg.priority_exponent)))
@@ -863,9 +873,16 @@ class DeviceReplay:
                                                         leaf_idx.numel(), nv.current_stream()))
 
     def device_bytes(self) -> int:
-        """Bytes of device memory the shard holds: rows, tree, and the fp16 mode's ingest staging once used."""
+        """Bytes of device memory the shard holds: rows, tree, and the ingest / restore staging block once used (not the
+        states of replay_state_memory="host")."""
         n = c_size_t(0)
         nv.check(self.lib.r2d2_replay_device_bytes(self._h, byref(n)))
+        return int(n.value)
+
+    def host_bytes(self) -> int:
+        """Bytes of pinned host memory the shard holds: the recurrent states under replay_state_memory="host", else 0."""
+        n = c_size_t(0)
+        nv.check(self.lib.r2d2_replay_host_bytes(self._h, byref(n)))
         return int(n.value)
 
     def stats(self) -> dict:

@@ -57,10 +57,11 @@ class TdOptions(Structure):
 
 
 class ReplayOptions(Structure):
-    _fields_ = [("state_storage", c_int)]
+    _fields_ = [("state_storage", c_int), ("state_memory", c_int)]
 
 
 STATE_F32, STATE_F16 = 0, 1   # ReplayOptions.state_storage (R2D2_STATE_F32 / R2D2_STATE_F16)
+STATE_MEMORY_DEVICE, STATE_MEMORY_HOST = 0, 1   # ReplayOptions.state_memory (R2D2_STATE_MEMORY_DEVICE / _HOST)
 
 
 class ReplaySnapshotInfo(Structure):
@@ -136,6 +137,7 @@ SIGNATURES = {
     "r2d2_replay_create": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig)]),
     "r2d2_replay_create_ex": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig), POINTER(ReplayOptions)]),
     "r2d2_replay_device_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
+    "r2d2_replay_host_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
     "r2d2_replay_destroy": (c_int, [c_void_p]),
     "r2d2_replay_set_priority_exponent": (c_int, [c_void_p, c_float]),
     "r2d2_replay_add_episodes": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -261,4 +263,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "ReplayOptions", "ReplaySnapshotInfo", "STATE_F32", "STATE_F16", "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "ReplayOptions", "ReplaySnapshotInfo", "STATE_F32", "STATE_F16", "STATE_MEMORY_DEVICE", "STATE_MEMORY_HOST", "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]

@@ -9,11 +9,15 @@
                         WeightedRandomSampler draw (replay_memory.py:95-114).  With a priority exponent alpha
                         (R2D2_PRIORITY_EXPONENT, default 1 = the reference) the shard stores p^alpha instead:
                         `priority[e][s]` reads the stored p^alpha, and a write of p through it stores p^alpha too.
+                        With host_gb > 0 (R2D2_REPLAY_HOST_GB) the rows' recurrent states live in pinned host memory
+                        and only the rest of each row and the tree take HBM.
 
 File format (actor.py:163-176, replay_memory.py:55-59): torch.save of
   {'replay_memory': deque[list[(obs f32[O], act f32[A], [reward], [terminal])]],
    'recurrent_state': deque[list[[[hx, cx] x 4 nets]]], 'priority': deque[list[float]], 'total_priority': list}.
 """
+import math
+import numbers
 import os
 from collections import deque
 from time import sleep
@@ -134,7 +138,7 @@ class _TotalPriority:
 
 class LearnerReplayMemory:
     def __init__(self, memory_sequence_size=500000, batch_size=32, obs_size=None, n_actions=None, hidden=128,
-                 capacity_rows=None, device=None, priority_exponent=None, state_dtype="float32"):
+                 capacity_rows=None, device=None, priority_exponent=None, state_dtype="float32", host_gb=0):
         self.path = './memory_data/'
         self.memory_sequence_size = memory_sequence_size
         self.sequence_counter = 0
@@ -146,7 +150,11 @@ class LearnerReplayMemory:
         if priority_exponent is None:
             priority_exponent = float(os.environ.get("R2D2_PRIORITY_EXPONENT", 1.0))
         self.priority_exponent = float(priority_exponent)
-        self.state_dtype = state_dtype                      # recurrent states in HBM: "float32" or "float16"
+        self.state_dtype = state_dtype                      # stored recurrent states: "float32" or "float16"
+        if isinstance(host_gb, bool) or not isinstance(host_gb, numbers.Real) or not (math.isfinite(host_gb)
+                                                                                      and host_gb >= 0):
+            raise ValueError("host_gb must be a finite number >= 0 (0 = states in HBM), got %r" % (host_gb,))
+        self.host_gb = float(host_gb)                       # > 0: the states live in this much pinned host memory
         self._cfg()                                         # rejects an exponent outside [0, 1] before any ingest
         self._dev = None          # DeviceReplay, created when the row width is known
         self._episodes = deque()  # (row_start, n_rows, n_starts) in FIFO order, mirrors the native ring
@@ -176,7 +184,8 @@ class LearnerReplayMemory:
         from r2d2_b200.engine import PathConfig
         return PathConfig(obs=self._obs, act=self._act, hidden=self._hidden, batch=self.batch_size,
                           burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
-                          priority_exponent=self.priority_exponent, replay_state_dtype=self.state_dtype)
+                          priority_exponent=self.priority_exponent, replay_state_dtype=self.state_dtype,
+                          replay_state_memory="host" if self.host_gb > 0 else "device")
 
     def _ensure_device(self, obs_size, n_actions, hidden):
         """Create the HBM shard on first use.  Sizes given to the constructor are binding: an actor file of another
@@ -198,9 +207,15 @@ class LearnerReplayMemory:
         episode that start no sequence: x1.3), capped at 60 % of the free HBM.  The reference keeps up to
         memory_sequence_size sequences in host RAM (replay_memory.py:148); when the cap applies, FIFO eviction starts
         earlier than there - said out loud, and documented in INTEGRATION.md.  fp16 state storage halves the
-        recurrent states [4,2,H] of a row, so the same cap holds nearly twice the rows."""
+        recurrent states [4,2,H] of a row, so the same cap holds nearly twice the rows.
+
+        With host_gb > 0 the states live in pinned host memory: a row then takes 4 (O + A + 2) + 5 bytes of HBM and
+        16 H (fp16) or 32 H (fp32) bytes of host memory, and the ring is the least of the wanted rows, the rows that fit
+        60 % of the free HBM and the rows that fit host_gb * 1e9 bytes; the note names the limit that applies."""
         want = int(self.memory_sequence_size * 1.3) + 4096
         state_bytes = 16 if self.state_dtype == "float16" else 32              # (h, c) of four nets, per unit of H
+        if self.host_gb > 0:
+            return self._host_tier_capacity_rows(want, obs_size, n_actions, state_bytes * hidden)
         bytes_per_row = 4 * (obs_size + n_actions + 2) + state_bytes * hidden + 5   # rows + leaf + ancestors
         free = torch.cuda.mem_get_info(self._device)[0] if torch.cuda.is_available() else 0
         fit = int(0.6 * free / bytes_per_row)
@@ -210,6 +225,23 @@ class LearnerReplayMemory:
                   % (fit, fit * bytes_per_row / 1e9, self.state_dtype, self.memory_sequence_size))
             return fit
         return want
+
+    def _host_tier_capacity_rows(self, want, obs_size, n_actions, host_row):
+        hbm_row = 4 * (obs_size + n_actions + 2) + 5                           # rows + leaf + ancestors
+        free = torch.cuda.mem_get_info(self._device)[0] if torch.cuda.is_available() else 0
+        limits = [(want, "memory_sequence_size=%d" % self.memory_sequence_size)]
+        if free > 0:
+            limits.append((int(0.6 * free / hbm_row), "60 %% of the free HBM (%.1f GB)" % (free / 1e9)))
+        limits.append((int(self.host_gb * 1e9 / host_row), "the host budget host_gb=%g" % self.host_gb))
+        rows, limit = min(limits, key=lambda x: x[0])
+        if rows < 1:
+            raise ValueError("LearnerReplayMemory: %s holds no replay row (%d bytes of %s recurrent states per row)"
+                             % (limit, host_row, self.state_dtype))
+        print("LearnerReplayMemory: ring of %d rows, limited by %s: %.2f GB of HBM (%d bytes per row) and %.2f GB of "
+              "pinned host memory (%s recurrent states, %d bytes per row)%s"
+              % (rows, limit, rows * hbm_row / 1e9, hbm_row, rows * host_row / 1e9, self.state_dtype, host_row,
+                 "" if rows == want else "; FIFO eviction starts earlier than the reference's"))
+        return rows
 
     def _register(self, starts, n_rows, n_starts, n_evicted, counter):
         """Mirror of the native FIFO: evictions (ring overlap while appending, sequence cap afterwards) always take the
