@@ -230,11 +230,10 @@ int r2d2_adam_step(float* params, const float* grads, float* exp_avg, float* exp
 
 // ---- replay ----
 int r2d2_replay_create(r2d2_replay_t** out, const r2d2_replay_config* cfg) {
-  return replay_create(reinterpret_cast<Replay**>(out), cfg);
+  return replay_create(reinterpret_cast<Replay**>(out), cfg, nullptr);
 }
 int r2d2_replay_create_ex(r2d2_replay_t** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options) {
-  return replay_create(reinterpret_cast<Replay**>(out), cfg, options ? options->state_storage : R2D2_STATE_F32,
-                       options ? options->state_memory : R2D2_STATE_MEMORY_DEVICE);
+  return replay_create(reinterpret_cast<Replay**>(out), cfg, options);
 }
 int r2d2_replay_device_bytes(r2d2_replay_t* r, size_t* out) {
   return replay_device_bytes(reinterpret_cast<Replay*>(r), out);

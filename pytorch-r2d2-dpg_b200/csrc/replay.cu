@@ -3,7 +3,10 @@
 // HBM layout (SoA, one "row" per stored env step incl. the n_step pad rows of actor.py:173):
 //   obs_rows [cap,O]  act_rows [cap,A]  rew_rows [cap]  term_rows [cap]  state_rows [cap,4,2,H]
 // state_rows is fp32, or fp16 under R2D2_STATE_F16 (rounded once at ingest, widened back to fp32 by the gather); under
-// R2D2_STATE_MEMORY_HOST it lives in mapped, page-locked host memory and everything else stays in HBM.
+// R2D2_STATE_MEMORY_HOST it lives in mapped, page-locked host memory and everything else stays in HBM.  Ingest and
+// restore write state rows through one path for both types and both tiers: stage_states decides whether the call's
+// states go through the device staging block, store_states writes a run of ring rows from wherever they are (a copy,
+// or a rounding / widening kernel), and write_rows puts a run's obs / act / rew / term next to them.
 // Episodes occupy contiguous row ranges of a ring; FIFO eviction (replay_memory.py:148-152).
 // Sum tree: one leaf per ROW (priority 0 for rows that are not valid sequence starts), fan-out 32:
 // every node is the left-to-right fp32 sum of its 32 children (one 128-byte line), so the tree has
@@ -176,20 +179,27 @@ __global__ void __launch_bounds__(256) states_to_f16_kernel(const float* __restr
   }
 }
 
-// Snapshot restore, fp16 file into an fp32 ring: dst[i] = (float)src[i], exact.  A restored range is whole [4,2,H] rows
-// (8 H halves = 16 H bytes each, and the staging copy starts 16 bytes into its block), so both ends are 16-byte aligned
-// for every H: each thread widens one 16-byte load of 8 halves into two float4 stores (the gather's widest route).
+// Exact fp16 -> fp32 widening of 4 halves (one 8-byte load) and of 8 halves (one 16-byte load)
+__device__ __forceinline__ float4 widen4(uint2 v) {
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
+  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+
+struct Float8 { float4 lo, hi; };
+__device__ __forceinline__ Float8 widen8(uint4 v) { return {widen4(make_uint2(v.x, v.y)), widen4(make_uint2(v.z, v.w))}; }
+
+// fp16 states into an fp32 ring (snapshot restore of an fp16 file): dst[i] = (float)src[i], exact.  A stored range is
+// whole [4,2,H] rows (8 H halves = 16 H bytes each, and the staging copy starts 16 bytes into its block), so both ends
+// are 16-byte aligned for every H: each thread widens one 16-byte load of 8 halves into two float4 stores (the gather's
+// widest route).
 __global__ void __launch_bounds__(256) states_from_f16_kernel(const __half* __restrict__ src, float* __restrict__ dst,
                                                               long long n) {
   const long long n8 = n >> 3;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
-    const uint4 v = reinterpret_cast<const uint4*>(src)[i];
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-    const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&v.z));
-    const float2 d = __half22float2(*reinterpret_cast<const __half2*>(&v.w));
-    reinterpret_cast<float4*>(dst)[2 * i] = make_float4(a.x, a.y, b.x, b.y);
-    reinterpret_cast<float4*>(dst)[2 * i + 1] = make_float4(c.x, c.y, d.x, d.y);
+    const Float8 f = widen8(reinterpret_cast<const uint4*>(src)[i]);
+    reinterpret_cast<float4*>(dst)[2 * i] = f.lo;
+    reinterpret_cast<float4*>(dst)[2 * i + 1] = f.hi;
   }
 }
 
@@ -306,7 +316,8 @@ __global__ void __launch_bounds__(256) tree_recompute_range_kernel(TreeView tv, 
 // kPerDraw (global sampling): B counts the W*Bc global draws; draw b goes to rank b / Bc's slot (dst_base[b / Bc] plus
 // the slot offsets), column b % Bc, and draws with leaf[b] < 0 belong to another shard and are skipped.
 struct GatherParams {
-  const float *obs_rows, *act_rows, *rew_rows, *term_rows, *state_rows;
+  const float *obs_rows, *act_rows, *rew_rows, *term_rows;
+  const void* state_rows;   // float, or __half under kHalfStates
   const long long* leaf;
   float *obs, *act, *rew, *term, *states;
   int T, B, O, A, H;
@@ -333,23 +344,14 @@ __device__ __forceinline__ void warp_widen_row(const __half* __restrict__ src, f
     const uint4* s8 = reinterpret_cast<const uint4*>(src);
     float4* d4 = reinterpret_cast<float4*>(dst);
     for (int k = lane; k < (n >> 3); k += 32) {
-      const uint4 v = __ldg(s8 + k);
-      const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-      const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-      const float2 c = __half22float2(*reinterpret_cast<const __half2*>(&v.z));
-      const float2 d = __half22float2(*reinterpret_cast<const __half2*>(&v.w));
-      d4[2 * k] = make_float4(a.x, a.y, b.x, b.y);
-      d4[2 * k + 1] = make_float4(c.x, c.y, d.x, d.y);
+      const Float8 f = widen8(__ldg(s8 + k));
+      d4[2 * k] = f.lo;
+      d4[2 * k + 1] = f.hi;
     }
   } else if ((n & 3) == 0) {
     const uint2* s4 = reinterpret_cast<const uint2*>(src);
     float4* d4 = reinterpret_cast<float4*>(dst);
-    for (int k = lane; k < (n >> 2); k += 32) {
-      const uint2 v = __ldg(s4 + k);
-      const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-      const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-      d4[k] = make_float4(a.x, a.y, b.x, b.y);
-    }
+    for (int k = lane; k < (n >> 2); k += 32) d4[k] = widen4(__ldg(s4 + k));
   } else {
     for (int k = lane; k < n; k += 32) dst[k] = __half2float(src[k]);
   }
@@ -391,12 +393,6 @@ __device__ __forceinline__ void host_copy_row(const float* __restrict__ src, flo
   }
 }
 
-__device__ __forceinline__ float4 widen4(uint2 v) {
-  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&v.x));
-  const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&v.y));
-  return make_float4(a.x, a.y, b.x, b.y);
-}
-
 // warp_widen_row's three routes (16-byte, 8-byte, scalar by H % 8 and H % 4) with the loads of a chunk first
 __device__ __forceinline__ void host_widen_row(const __half* __restrict__ src, float* __restrict__ dst, int n, int lane) {
   if ((n & 7) == 0) {
@@ -409,8 +405,9 @@ __device__ __forceinline__ void host_widen_row(const __half* __restrict__ src, f
       for (int j = 0; j < kHostLoads; ++j) {
         const int k = k0 + j * 32 + lane;
         if (k < (n >> 3)) {
-          d4[2 * k] = widen4(make_uint2(v[j].x, v[j].y));
-          d4[2 * k + 1] = widen4(make_uint2(v[j].z, v[j].w));
+          const Float8 f = widen8(v[j]);
+          d4[2 * k] = f.lo;
+          d4[2 * k + 1] = f.hi;
         }
       }
     }
@@ -475,15 +472,17 @@ __device__ __forceinline__ void gather_batch(GatherParams g) {
       }
     } else if (kHostStates) {
       if (kHalfStates)
-        host_widen_row(reinterpret_cast<const __half*>(g.state_rows) + (leaf * 8 + t) * g.H,
+        host_widen_row(static_cast<const __half*>(g.state_rows) + (leaf * 8 + t) * g.H,
                        states + ((long long)t * ld + col) * g.H, g.H, lane);
       else
-        host_copy_row(g.state_rows + (leaf * 8 + t) * g.H, states + ((long long)t * ld + col) * g.H, g.H, lane);
+        host_copy_row(static_cast<const float*>(g.state_rows) + (leaf * 8 + t) * g.H,
+                      states + ((long long)t * ld + col) * g.H, g.H, lane);
     } else if (kHalfStates) {
-      warp_widen_row(reinterpret_cast<const __half*>(g.state_rows) + (leaf * 8 + (t - g.T)) * g.H,
+      warp_widen_row(static_cast<const __half*>(g.state_rows) + (leaf * 8 + (t - g.T)) * g.H,
                      states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
     } else {
-      warp_copy_row(g.state_rows + (leaf * 8 + (t - g.T)) * g.H, states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
+      warp_copy_row(static_cast<const float*>(g.state_rows) + (leaf * 8 + (t - g.T)) * g.H,
+                    states + ((long long)(t - g.T) * ld + col) * g.H, g.H, lane);
     }
     t += dt; b += db;
     if (b >= g.B) { b -= g.B; ++t; }
@@ -519,19 +518,19 @@ struct Episode {
 struct Replay {
   r2d2_replay_config cfg;
   int rows_per_window;
-  float *obs_rows = nullptr, *act_rows = nullptr, *rew_rows = nullptr, *term_rows = nullptr, *state_rows = nullptr;
-  // R2D2_STATE_F16: the states live in state_half (state_rows stays null), and ingest rounds them from a grow-only
-  // device staging block: [overflow count (16 B) | fp32 states of the largest call so far]
+  float *obs_rows = nullptr, *act_rows = nullptr, *rew_rows = nullptr, *term_rows = nullptr;
+  // The recurrent states [cap,4,2,H]: fp32, or __half under R2D2_STATE_F16 (half_states).  In HBM, or under
+  // R2D2_STATE_MEMORY_HOST (host_states) in mapped, page-locked host memory (host_alloc, freed with cudaFreeHost) that
+  // state_rows addresses through its device pointer.  Rows: state_row_bytes / state_row.
+  char* state_rows = nullptr;
   bool half_states = false;
-  __half* state_half = nullptr;
-  char* stage = nullptr;
-  size_t stage_bytes = 0;
-  size_t device_bytes = 0;   // every device allocation of the shard (rows, tree, staging)
-  // R2D2_STATE_MEMORY_HOST: state_rows / state_half point into mapped, page-locked host memory (host_alloc, freed with
-  // cudaFreeHost); ingest and restore stage the states in the device block first, so every write is stream-ordered
   bool host_states = false;
   void* host_alloc = nullptr;
   size_t host_bytes = 0;
+  // grow-only device staging block (stage_states): [count (16 B) | the packed states of the largest call so far]
+  char* stage = nullptr;
+  size_t stage_bytes = 0;
+  size_t device_bytes = 0;   // every device allocation of the shard (rows, tree, staging)
   std::vector<float*> level_alloc;
   TreeView tv;
   std::deque<Episode> episodes;
@@ -563,6 +562,13 @@ struct Replay {
   Import* import = nullptr;
 };
 
+// bytes of one [4,2,H] state row stored as fp16 (half) or fp32, or in the shard's type; the address of ring row i
+static size_t state_row_bytes(const Replay* r, bool half) {
+  return (half ? sizeof(__half) : sizeof(float)) * 8 * (size_t)r->cfg.hidden;
+}
+static size_t state_row_bytes(const Replay* r) { return state_row_bytes(r, r->half_states); }
+static char* state_row(const Replay* r, long long i) { return r->state_rows + i * state_row_bytes(r); }
+
 static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leaves, cudaStream_t stream) {
   long long lo = first_leaf, hi = first_leaf + n_leaves - 1;
   for (int l = 1; l < r->tv.levels; ++l) {
@@ -576,37 +582,37 @@ static int recompute_ancestors(Replay* r, long long first_leaf, long long n_leav
   return R2D2_OK;
 }
 
-int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage, int state_memory) {
+int replay_create(Replay** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options) {
   R2D2_REQUIRE(out && cfg, "null");
   R2D2_REQUIRE(cfg->obs_size > 0 && cfg->n_actions > 0 && cfg->hidden > 0, "sizes");
   R2D2_REQUIRE(cfg->capacity_rows > 0, "capacity_rows");
-  R2D2_REQUIRE(state_storage == R2D2_STATE_F32 || state_storage == R2D2_STATE_F16,
+  const r2d2_replay_options opt = options ? *options : r2d2_replay_options{};   // zeroed = fp32 states in HBM
+  R2D2_REQUIRE(opt.state_storage == R2D2_STATE_F32 || opt.state_storage == R2D2_STATE_F16,
                "state_storage is R2D2_STATE_F32 or R2D2_STATE_F16");
-  R2D2_REQUIRE(state_memory == R2D2_STATE_MEMORY_DEVICE || state_memory == R2D2_STATE_MEMORY_HOST,
+  R2D2_REQUIRE(opt.state_memory == R2D2_STATE_MEMORY_DEVICE || opt.state_memory == R2D2_STATE_MEMORY_HOST,
                "state_memory is R2D2_STATE_MEMORY_DEVICE or R2D2_STATE_MEMORY_HOST");
   Replay* r = new Replay();
   r->cfg = *cfg;
   r->rows_per_window = cfg->burn_in + cfg->learning + cfg->n_step;
-  r->half_states = state_storage == R2D2_STATE_F16;
-  r->host_states = state_memory == R2D2_STATE_MEMORY_HOST;
+  r->half_states = opt.state_storage == R2D2_STATE_F16;
+  r->host_states = opt.state_memory == R2D2_STATE_MEMORY_HOST;
   const long long cap = cfg->capacity_rows;
+  const size_t state_bytes = (size_t)cap * state_row_bytes(r);
   if (r->host_states) {   // first, so that a refusal leaves nothing allocated
-    const size_t bytes = (r->half_states ? sizeof(__half) : sizeof(float)) * (size_t)cap * 8 * cfg->hidden;
     void* dev = nullptr;
-    cudaError_t e = cudaHostAlloc(&r->host_alloc, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+    cudaError_t e = cudaHostAlloc(&r->host_alloc, state_bytes, cudaHostAllocMapped | cudaHostAllocPortable);
     if (e == cudaSuccess) e = cudaHostGetDevicePointer(&dev, r->host_alloc, 0);
     if (e != cudaSuccess) {
       cudaGetLastError();
       if (r->host_alloc) cudaFreeHost(r->host_alloc);
       delete r;
-      set_last_error("replay shard: " + std::to_string(bytes) + " bytes of mapped pinned host memory for the recurrent "
-                     "states could not be allocated (" + cudaGetErrorString(e) + ")");
+      set_last_error("replay shard: " + std::to_string(state_bytes) + " bytes of mapped pinned host memory for the "
+                     "recurrent states could not be allocated (" + cudaGetErrorString(e) + ")");
       return R2D2_ERR_CUDA;
     }
-    memset(r->host_alloc, 0, bytes);   // nothing can be in flight on a buffer that was just allocated
-    r->host_bytes = bytes;
-    if (r->half_states) r->state_half = static_cast<__half*>(dev);
-    else r->state_rows = static_cast<float*>(dev);
+    memset(r->host_alloc, 0, state_bytes);   // nothing can be in flight on a buffer that was just allocated
+    r->host_bytes = state_bytes;
+    r->state_rows = static_cast<char*>(dev);
   }
   auto dmalloc_bytes = [&](void** p, size_t bytes) -> int {
     R2D2_CUDA_TRY(cudaMalloc(p, bytes));
@@ -620,9 +626,7 @@ int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage
   int rc = R2D2_OK;
   if ((rc = dmalloc(&r->obs_rows, cap * cfg->obs_size)) || (rc = dmalloc(&r->act_rows, cap * cfg->n_actions)) ||
       (rc = dmalloc(&r->rew_rows, cap)) || (rc = dmalloc(&r->term_rows, cap)) ||
-      (!r->host_states &&
-       (rc = r->half_states ? dmalloc_bytes(reinterpret_cast<void**>(&r->state_half), sizeof(__half) * (size_t)cap * 8 * cfg->hidden)
-                            : dmalloc(&r->state_rows, cap * 8 * cfg->hidden)))) {
+      (!r->host_states && (rc = dmalloc_bytes(reinterpret_cast<void**>(&r->state_rows), state_bytes)))) {
     replay_destroy(r);
     return rc;
   }
@@ -667,14 +671,10 @@ static int raise_fresh_leaves(Replay* r, long long first, long long n, cudaStrea
   return R2D2_OK;
 }
 
-// fp16 state storage: the staging block starts with the overflow count, the fp32 states follow 16 bytes in (every
-// packed row of 8 H floats then starts 16-byte aligned, as states_to_f16_kernel needs)
+// The staging block starts with a count (fp16 overflow at ingest, bad leaves at restore); the packed states follow 16
+// bytes in, so every packed row of 8 H values starts 16-byte aligned, as the conversion kernels need.
 constexpr size_t kStageHead = 16;
-static float* staged_states(Replay* r) { return reinterpret_cast<float*>(r->stage + kStageHead); }
 
-// Copies the call's n packed fp32 states into the staging block (grown to fit) and counts the finite values that fp16
-// would round to +-inf.  Any such value refuses the whole call with R2D2_ERR_ARG before anything is placed, evicted or
-// committed.  Synchronises the stream (the count is read on the host).
 static int ensure_stage(Replay* r, size_t need) {
   if (need > r->stage_bytes) {
     R2D2_CUDA_TRY(cudaFree(r->stage));   // synchronises: no conversion of an earlier call still reads the old block
@@ -688,13 +688,36 @@ static int ensure_stage(Replay* r, size_t need) {
   return R2D2_OK;
 }
 
-static int stage_half_states(Replay* r, const float* states, size_t n, cudaStream_t stream) {
-  R2D2_TRY(ensure_stage(r, kStageHead + sizeof(float) * n));
+// The packed state rows of an ingest or restore call, as store_states reads them: the caller's host buffer, or the
+// staging block (which holds zeros past the caller's rows).
+struct StateSource {
+  const char* base;   // packed row 0
+  bool half;          // fp16 rows, else fp32
+  bool staged;
+};
+
+// The call's n_src packed state rows (fp16 or fp32, host memory) go through the staging block if and only if the shard
+// keeps its states in host memory - every write to the mapped rows is then stream-ordered device work - or in the other
+// type, whose conversion kernel reads device memory.  Staged, they are zero-padded to n_rows rows, and fp32 states
+// bound for fp16 rows are range-checked: a finite value that fp16 would round to +-inf refuses the whole call with
+// R2D2_ERR_ARG before anything is placed, evicted or committed (one stream synchronisation: the count is read on the
+// host).  Unstaged, the source is the caller's buffer.
+static int stage_states(Replay* r, const void* states, bool half, long long n_src, long long n_rows, cudaStream_t stream,
+                        StateSource* out) {
+  *out = {static_cast<const char*>(states), half, false};
+  if (!r->host_states && half == r->half_states) return R2D2_OK;
+  const size_t row = state_row_bytes(r, half);
+  R2D2_TRY(ensure_stage(r, kStageHead + row * (size_t)n_rows));
+  char* staged = r->stage + kStageHead;
+  *out = {staged, half, true};
+  if (n_src > 0) R2D2_CUDA_TRY(cudaMemcpyAsync(staged, states, row * (size_t)n_src, cudaMemcpyHostToDevice, stream));
+  if (n_rows > n_src) R2D2_CUDA_TRY(cudaMemsetAsync(staged + row * n_src, 0, row * (size_t)(n_rows - n_src), stream));
+  if (half || !r->half_states) return R2D2_OK;
+  const long long n = n_src * 8LL * r->cfg.hidden;
   unsigned long long* d_count = reinterpret_cast<unsigned long long*>(r->stage);
   R2D2_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(*d_count), stream));
   if (n > 0) {
-    R2D2_CUDA_TRY(cudaMemcpyAsync(staged_states(r), states, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    count_f16_overflow_kernel<<<grid_for((long long)n), 256, 0, stream>>>(staged_states(r), (long long)n, d_count);
+    count_f16_overflow_kernel<<<grid_for(n), 256, 0, stream>>>(reinterpret_cast<const float*>(staged), n, d_count);
     count_launch();
     R2D2_CUDA_TRY(cudaGetLastError());
   }
@@ -709,44 +732,51 @@ static int stage_half_states(Replay* r, const float* states, size_t n, cudaStrea
   return R2D2_OK;
 }
 
-// Rounds n_rows staged state rows (from packed row `first`) into ring rows [ring_row, ring_row + n_rows).
-static int convert_half_states(Replay* r, long long ring_row, long long first, long long n_rows, cudaStream_t stream) {
-  const long long w = 8LL * r->cfg.hidden, n = n_rows * w;
-  if (n == 0) return R2D2_OK;
-  states_to_f16_kernel<<<grid_for(n / 8), 256, 0, stream>>>(staged_states(r) + first * w, r->state_half + ring_row * w, n);
+// Packed rows [src_row, src_row + n_rows) of `src` into ring rows [ring_row, ring_row + n_rows): one copy when the types
+// match (cudaMemcpyDefault: either end may be host memory), else one rounding or widening kernel, which also stores
+// straight into mapped host rows.
+static int store_states(Replay* r, long long ring_row, const StateSource& src, long long src_row, long long n_rows,
+                        cudaStream_t stream) {
+  if (n_rows <= 0) return R2D2_OK;
+  const char* from = src.base + src_row * state_row_bytes(r, src.half);
+  char* to = state_row(r, ring_row);
+  if (src.half == r->half_states) {
+    R2D2_CUDA_TRY(cudaMemcpyAsync(to, from, state_row_bytes(r, src.half) * (size_t)n_rows, cudaMemcpyDefault, stream));
+    return R2D2_OK;
+  }
+  const long long n = n_rows * 8LL * r->cfg.hidden;
+  if (r->half_states)
+    states_to_f16_kernel<<<grid_for(n / 8), 256, 0, stream>>>(reinterpret_cast<const float*>(from),
+                                                              reinterpret_cast<__half*>(to), n);
+  else
+    states_from_f16_kernel<<<grid_for(n / 8), 256, 0, stream>>>(reinterpret_cast<const __half*>(from),
+                                                                reinterpret_cast<float*>(to), n);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
   return R2D2_OK;
 }
 
-// Host tier: the call's packed fp32 states (n values, then zeros up to n_total) in the staging block, so that they reach
-// the mapped host rows by stream-ordered work (store_staged_states).  fp16 storage stages through ingest's range check.
-static int stage_host_states(Replay* r, const float* states, size_t n, size_t n_total, cudaStream_t stream) {
-  R2D2_TRY(ensure_stage(r, kStageHead + sizeof(float) * n_total));
-  if (r->half_states)
-    R2D2_TRY(stage_half_states(r, states, n, stream));
-  else if (n > 0)
-    R2D2_CUDA_TRY(cudaMemcpyAsync(staged_states(r), states, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-  if (n_total > n) R2D2_CUDA_TRY(cudaMemsetAsync(staged_states(r) + n, 0, sizeof(float) * (n_total - n), stream));
-  return R2D2_OK;
-}
-
-// Host tier: staged rows [first, first + n_rows) into ring rows [ring_row, ring_row + n_rows).  fp16 storage rounds them
-// with states_to_f16_kernel, which stores into the mapped rows; fp32 storage is one device-to-host copy.
-static int store_staged_states(Replay* r, long long ring_row, long long first, long long n_rows, cudaStream_t stream) {
-  if (r->half_states) return convert_half_states(r, ring_row, first, n_rows, stream);
-  const long long w = 8LL * r->cfg.hidden;
-  if (n_rows > 0)
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + ring_row * w, staged_states(r) + first * w,
-                                  sizeof(float) * (size_t)(n_rows * w), cudaMemcpyDefault, stream));
-  return R2D2_OK;
+// Packed host rows [src_row, src_row + n_rows) of obs / act / rew / term into ring rows [ring_row, ring_row + n_rows),
+// and the first n_state_rows of them from the states of `src`.  The leaves stay with the callers.
+static int write_rows(Replay* r, long long ring_row, long long src_row, long long n_rows, const float* obs,
+                      const float* act, const float* rew, const float* term, const StateSource& src,
+                      long long n_state_rows, cudaStream_t stream) {
+  const size_t O = r->cfg.obs_size, A = r->cfg.n_actions, n = (size_t)n_rows;
+  R2D2_CUDA_TRY(cudaMemcpyAsync(r->obs_rows + ring_row * O, obs + src_row * O, sizeof(float) * n * O,
+                                cudaMemcpyHostToDevice, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + ring_row * A, act + src_row * A, sizeof(float) * n * A,
+                                cudaMemcpyHostToDevice, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + ring_row, rew + src_row, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + ring_row, term + src_row, sizeof(float) * n, cudaMemcpyHostToDevice,
+                                stream));
+  return store_states(r, ring_row, src, src_row, n_state_rows, stream);
 }
 
 int replay_destroy(Replay* r) {
   if (!r) return R2D2_OK;
   cudaFree(r->obs_rows); cudaFree(r->act_rows); cudaFree(r->rew_rows); cudaFree(r->term_rows);
   if (r->host_states) cudaFreeHost(r->host_alloc);
-  else { cudaFree(r->state_rows); cudaFree(r->state_half); }
+  else cudaFree(r->state_rows);
   cudaFree(r->stage);
   for (float* p : r->level_alloc) cudaFree(p);
   delete r->group;
@@ -819,6 +849,16 @@ static void commit_episode(Replay* r, long long start, int n_rows, int n_starts)
   r->sequence_counter += n_rows - (r->rows_per_window - 1);  // replay_memory.py:147
 }
 
+// The end of an ingest call: the cap's evictions (replay_memory.py:148-152), one refresh of every touched leaf range,
+// and the synchronisation after which the caller may release its host buffers.
+static int finish_ingest(Replay* r, RangeList& ranges, cudaStream_t stream) {
+  while (r->cfg.max_sequences > 0 && r->sequence_counter > r->cfg.max_sequences && !r->episodes.empty())
+    R2D2_TRY(evict_front(r, stream, &ranges));
+  R2D2_TRY(refresh_ranges(r, ranges, stream));
+  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
+  return R2D2_OK;
+}
+
 int replay_add_episode(Replay* r, const float* obs, const float* act, const float* rew, const float* term,
                        const float* states, int n_rows, int n_state_rows, const float* priority, int n_starts,
                        cudaStream_t stream) {
@@ -827,32 +867,16 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
   R2D2_REQUIRE(n_starts >= 0 && n_starts <= n_rows - r->rows_per_window + 1, "n_starts exceeds valid window starts");
   R2D2_REQUIRE(n_state_rows >= n_starts && n_state_rows <= n_rows, "state rows");
   R2D2_REQUIRE(n_starts == 0 || priority, "priority");
-  const int O = r->cfg.obs_size, A = r->cfg.n_actions, H = r->cfg.hidden;
-  if (r->host_states)
-    R2D2_TRY(stage_host_states(r, states, (size_t)n_state_rows * 8 * H, (size_t)n_rows * 8 * H, stream));
-  else if (r->half_states)
-    R2D2_TRY(stage_half_states(r, states, (size_t)n_state_rows * 8 * H, stream));
+  StateSource src;
+  R2D2_TRY(stage_states(r, states, false, n_state_rows, n_rows, stream, &src));
   RangeList ranges;
   long long start = 0;
   R2D2_TRY(place_episode(r, n_rows, stream, &ranges, &start));
-  R2D2_CUDA_TRY(cudaMemcpyAsync(r->obs_rows + start * O, obs, sizeof(float) * (size_t)n_rows * O, cudaMemcpyHostToDevice, stream));
-  R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + start * A, act, sizeof(float) * (size_t)n_rows * A, cudaMemcpyHostToDevice, stream));
-  R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + start, rew, sizeof(float) * (size_t)n_rows, cudaMemcpyHostToDevice, stream));
-  R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + start, term, sizeof(float) * (size_t)n_rows, cudaMemcpyHostToDevice, stream));
-  if (r->host_states) {
-    R2D2_TRY(store_staged_states(r, start, 0, n_rows, stream));   // the rows past n_state_rows were staged as zeros
-  } else if (r->half_states) {
-    R2D2_TRY(convert_half_states(r, start, 0, n_state_rows, stream));
-    if (n_state_rows < n_rows)
-      R2D2_CUDA_TRY(cudaMemsetAsync(r->state_half + (start + n_state_rows) * 8 * H, 0,
-                                    sizeof(__half) * (size_t)(n_rows - n_state_rows) * 8 * H, stream));
-  } else {
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + start * 8 * H, states, sizeof(float) * (size_t)n_state_rows * 8 * H,
-                                  cudaMemcpyHostToDevice, stream));
-    if (n_state_rows < n_rows)
-      R2D2_CUDA_TRY(cudaMemsetAsync(r->state_rows + (start + n_state_rows) * 8 * H, 0,
-                                    sizeof(float) * (size_t)(n_rows - n_state_rows) * 8 * H, stream));
-  }
+  // rows past n_state_rows get zero states: staged, the block holds them; from the caller's buffer, a memset
+  const long long n_stored = src.staged ? n_rows : n_state_rows;
+  R2D2_TRY(write_rows(r, start, 0, n_rows, obs, act, rew, term, src, n_stored, stream));
+  if (n_stored < n_rows)
+    R2D2_CUDA_TRY(cudaMemsetAsync(state_row(r, start + n_stored), 0, state_row_bytes(r) * (size_t)(n_rows - n_stored), stream));
   if (n_starts > 0) {
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + start, priority, sizeof(float) * (size_t)n_starts,
                                   cudaMemcpyHostToDevice, stream));
@@ -862,11 +886,7 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
     R2D2_CUDA_TRY(cudaMemsetAsync(r->tv.lvl[0] + start + n_starts, 0, sizeof(float) * (size_t)(n_rows - n_starts), stream));
   ranges.push_back({start, (long long)n_rows});
   commit_episode(r, start, n_rows, n_starts);
-  while (r->cfg.max_sequences > 0 && r->sequence_counter > r->cfg.max_sequences && !r->episodes.empty())
-    R2D2_TRY(evict_front(r, stream, &ranges));                               // replay_memory.py:148-152
-  R2D2_TRY(refresh_ranges(r, ranges, stream));
-  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));  // host buffers may be released by the caller
-  return R2D2_OK;
+  return finish_ingest(r, ranges, stream);
 }
 
 // One actor file at a time (LearnerReplayMemory.load, replay_memory.py:138-157): every episode of the file is appended,
@@ -880,40 +900,27 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
                         long long* sequence_counter_out, cudaStream_t stream) {
   R2D2_REQUIRE(r && n_episodes >= 0 && (n_episodes == 0 || (n_rows && n_starts && obs && act && rew && term && states && leaf_prio)),
                "null");
-  const int O = r->cfg.obs_size, A = r->cfg.n_actions, H = r->cfg.hidden;
+  long long R = 0;
   for (int e = 0; e < n_episodes; ++e) {
     R2D2_REQUIRE(n_rows[e] >= r->rows_per_window, "episode shorter than one window");
     R2D2_REQUIRE(n_starts[e] >= 0 && n_starts[e] <= n_rows[e] - r->rows_per_window + 1, "n_starts exceeds valid window starts");
     R2D2_REQUIRE(n_rows[e] <= r->cfg.capacity_rows, "episode larger than the ring");
+    R += n_rows[e];
   }
-  if ((r->half_states || r->host_states) && n_episodes > 0) {
-    long long R = 0;
-    for (int e = 0; e < n_episodes; ++e) R += n_rows[e];
-    if (r->host_states) R2D2_TRY(stage_host_states(r, states, (size_t)R * 8 * H, (size_t)R * 8 * H, stream));
-    else R2D2_TRY(stage_half_states(r, states, (size_t)R * 8 * H, stream));
-  }
+  StateSource src{};
+  if (n_episodes > 0) R2D2_TRY(stage_states(r, states, false, R, R, stream, &src));
   const long long evicted0 = r->evicted_total;
   RangeList ranges;
-  long long src = 0;                    // first packed row of the current run
+  long long first = 0;                  // first packed row of the current run
   long long run_start = -1, run_rows = 0;
   auto flush = [&]() -> int {
     if (run_rows == 0) return R2D2_OK;
-    const size_t n = (size_t)run_rows;
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->obs_rows + run_start * O, obs + src * O, sizeof(float) * n * O, cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + run_start * A, act + src * A, sizeof(float) * n * A, cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + run_start, rew + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + run_start, term + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
-    if (r->host_states)
-      R2D2_TRY(store_staged_states(r, run_start, src, run_rows, stream));
-    else if (r->half_states)
-      R2D2_TRY(convert_half_states(r, run_start, src, run_rows, stream));
-    else
-      R2D2_CUDA_TRY(cudaMemcpyAsync(r->state_rows + run_start * 8 * H, states + src * 8 * H, sizeof(float) * n * 8 * H,
-                                    cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + run_start, leaf_prio + src, sizeof(float) * n, cudaMemcpyHostToDevice, stream));
+    R2D2_TRY(write_rows(r, run_start, first, run_rows, obs, act, rew, term, src, run_rows, stream));
+    R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + run_start, leaf_prio + first, sizeof(float) * (size_t)run_rows,
+                                  cudaMemcpyHostToDevice, stream));
     R2D2_TRY(raise_fresh_leaves(r, run_start, run_rows, stream));
     ranges.push_back({run_start, run_rows});
-    src += run_rows;
+    first += run_rows;
     run_rows = 0;
     return R2D2_OK;
   };
@@ -930,19 +937,32 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     if (row_start_out) row_start_out[e] = start;
   }
   R2D2_TRY(flush());
-  while (r->cfg.max_sequences > 0 && r->sequence_counter > r->cfg.max_sequences && !r->episodes.empty())
-    R2D2_TRY(evict_front(r, stream, &ranges));                               // replay_memory.py:148-152
-  R2D2_TRY(refresh_ranges(r, ranges, stream));
-  R2D2_CUDA_TRY(cudaStreamSynchronize(stream));  // host buffers may be released by the caller
+  R2D2_TRY(finish_ingest(r, ranges, stream));
   if (n_evicted_out) *n_evicted_out = r->evicted_total - evicted0;
   if (sequence_counter_out) *sequence_counter_out = r->sequence_counter;
   return R2D2_OK;
 }
 
-// GatherParams keeps its fp32 state pointer (so that the fp32 gather compiles as before); the fp16 instantiations
-// read it as __half
-static const float* state_source(const Replay* r) {
-  return r->half_states ? reinterpret_cast<const float*>(r->state_half) : r->state_rows;
+// The ring side of a gather: the shard's rows and sizes.  The caller fills in the leaves and the destination.
+static GatherParams ring_gather_params(const Replay* r) {
+  GatherParams g{};
+  g.obs_rows = r->obs_rows; g.act_rows = r->act_rows; g.rew_rows = r->rew_rows; g.term_rows = r->term_rows;
+  g.state_rows = r->state_rows;
+  g.T = r->rows_per_window; g.O = r->cfg.obs_size; g.A = r->cfg.n_actions; g.H = r->cfg.hidden;
+  return g;
+}
+
+// The gather instantiation for the shard's state type and tier, one warp per task
+template <bool kPerDraw>
+static int launch_gather(const Replay* r, const GatherParams& g, long long tasks, cudaStream_t stream) {
+  const int grid = grid_for(tasks * 32);
+  if (r->host_states && r->half_states) gather_host_states_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
+  else if (r->host_states) gather_host_states_kernel<kPerDraw, false><<<grid, 256, 0, stream>>>(g);
+  else if (r->half_states) gather_batch_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
+  else gather_batch_kernel<kPerDraw, false><<<grid, 256, 0, stream>>>(g);
+  count_launch();
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return R2D2_OK;
 }
 
 int replay_device_bytes(Replay* r, size_t* out) {
@@ -960,26 +980,15 @@ int replay_host_bytes(Replay* r, size_t* out) {
 int replay_gather(Replay* r, const long long* leaf_idx, int batch, float* obs, float* act, float* rew, float* term,
                   float* states, cudaStream_t stream) {
   R2D2_REQUIRE(r && leaf_idx && batch > 0, "args");
-  const int T = r->rows_per_window, O = r->cfg.obs_size, A = r->cfg.n_actions, H = r->cfg.hidden;
-  if (obs || act || rew || term || states) {
-    GatherParams g;
-    g.obs_rows = r->obs_rows; g.act_rows = r->act_rows; g.rew_rows = r->rew_rows; g.term_rows = r->term_rows;
-    g.state_rows = state_source(r); g.leaf = leaf_idx;
-    g.obs = obs; g.act = act; g.rew = rew; g.term = term; g.states = states;
-    g.T = T; g.B = batch; g.O = O; g.A = A; g.H = H;
-    const long long tasks = (long long)T * batch + (states ? (long long)8 * batch : 0);
-    if (r->host_states && r->half_states)
-      gather_host_states_kernel<false, true><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
-    else if (r->host_states)
-      gather_host_states_kernel<false, false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
-    else if (r->half_states)
-      gather_batch_kernel<false, true><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
-    else
-      gather_batch_kernel<false, false><<<grid_for(tasks * 32), 256, 0, stream>>>(g);
-    count_launch();
+  if (!(obs || act || rew || term || states)) {
+    R2D2_CUDA_TRY(cudaGetLastError());
+    return R2D2_OK;
   }
-  R2D2_CUDA_TRY(cudaGetLastError());
-  return R2D2_OK;
+  GatherParams g = ring_gather_params(r);
+  g.leaf = leaf_idx;
+  g.obs = obs; g.act = act; g.rew = rew; g.term = term; g.states = states;
+  g.B = batch;
+  return launch_gather<false>(r, g, (long long)g.T * batch + (states ? (long long)8 * batch : 0), stream);
 }
 
 int replay_sample(Replay* r, const float* u, int batch, long long* leaf_idx, float* obs, float* act, float* rew,
@@ -1092,17 +1101,14 @@ int replay_export_rows(Replay* r, long long first, long long n, float* obs, floa
                        void* states, float* leaves, cudaStream_t stream) {
   R2D2_REQUIRE(r && obs && act && rew && term && states && leaves, "null");
   R2D2_REQUIRE(first >= 0 && n >= 0 && first + n <= r->cfg.capacity_rows, "row range outside the ring");
-  const size_t O = r->cfg.obs_size, A = r->cfg.n_actions, w = 8 * (size_t)r->cfg.hidden, k = (size_t)n;
+  const size_t O = r->cfg.obs_size, A = r->cfg.n_actions, k = (size_t)n;
   R2D2_CUDA_TRY(cudaMemcpyAsync(obs, r->obs_rows + first * O, sizeof(float) * k * O, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(act, r->act_rows + first * A, sizeof(float) * k * A, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(rew, r->rew_rows + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(term, r->term_rows + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
   // cudaMemcpyDefault: the host tier's rows are host memory.  Only ingest and restore write them, and both synchronise
   // the stream before they return, so no write to these rows is in flight here
-  if (r->half_states)
-    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_half + first * w, sizeof(__half) * k * w, cudaMemcpyDefault, stream));
-  else
-    R2D2_CUDA_TRY(cudaMemcpyAsync(states, r->state_rows + first * w, sizeof(float) * k * w, cudaMemcpyDefault, stream));
+  R2D2_CUDA_TRY(cudaMemcpyAsync(states, state_row(r, first), state_row_bytes(r) * k, cudaMemcpyDefault, stream));
   R2D2_CUDA_TRY(cudaMemcpyAsync(leaves, r->tv.lvl[0] + first, sizeof(float) * k, cudaMemcpyDeviceToHost, stream));
   R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
   return R2D2_OK;
@@ -1215,46 +1221,19 @@ int replay_import_rows(Replay* r, long long first, long long n, const float* obs
     return refuse_import(r, stream, "rows [" + std::to_string(first) + ", " + std::to_string(first + n) +
                                         ") do not continue the " + std::to_string(im.received) + " of " +
                                         std::to_string(im.packed_rows) + " rows received so far");
-  const long long O = r->cfg.obs_size, A = r->cfg.n_actions, w = 8LL * r->cfg.hidden;
-  const bool src_half = im.storage == R2D2_STATE_F16;
-  if (src_half && !r->half_states) {            // fp16 file, fp32 ring: the halves go through the staging block
-    R2D2_TRY(ensure_stage(r, kStageHead + sizeof(__half) * (size_t)(n * w)));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->stage + kStageHead, states, sizeof(__half) * (size_t)(n * w), cudaMemcpyHostToDevice,
-                                  stream));
-  } else if (!src_half && r->half_states) {     // fp32 file, fp16 ring: ingest's range check, then its rounding
-    const int rc = stage_half_states(r, static_cast<const float*>(states), (size_t)(n * w), stream);
-    if (rc != R2D2_OK) return refuse_import(r, stream, std::string(last_error()));
-  } else if (r->host_states) {                  // same type, host tier: staged, then device-to-host copies
-    const size_t b = (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(n * w);
-    R2D2_TRY(ensure_stage(r, kStageHead + b));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->stage + kStageHead, states, b, cudaMemcpyHostToDevice, stream));
-  }
-  R2D2_TRY(ensure_stage(r, kStageHead));
+  StateSource src;   // the file's states (in its type), staged as ingest stages them
+  const int rc = stage_states(r, states, im.storage == R2D2_STATE_F16, n, n, stream, &src);
+  if (rc == R2D2_ERR_ARG) return refuse_import(r, stream, std::string(last_error()));
+  R2D2_TRY(rc);
+  R2D2_TRY(ensure_stage(r, kStageHead));   // the bad-leaf count
   unsigned long long* d_count = reinterpret_cast<unsigned long long*>(r->stage);
   R2D2_CUDA_TRY(cudaMemsetAsync(d_count, 0, sizeof(*d_count), stream));
   for (const Replay::Import::Run& run : im.runs) {
     const long long lo = std::max(run.src, first), hi = std::min(run.src + run.n, first + n);
     if (lo >= hi) continue;
     const long long s = lo - first, d = run.dst + (lo - run.src), k = hi - lo;
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->obs_rows + d * O, obs + s * O, sizeof(float) * (size_t)(k * O), cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->act_rows + d * A, act + s * A, sizeof(float) * (size_t)(k * A), cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->rew_rows + d, rew + s, sizeof(float) * (size_t)k, cudaMemcpyHostToDevice, stream));
-    R2D2_CUDA_TRY(cudaMemcpyAsync(r->term_rows + d, term + s, sizeof(float) * (size_t)k, cudaMemcpyHostToDevice, stream));
+    R2D2_TRY(write_rows(r, d, s, k, obs, act, rew, term, src, k, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + d, leaves + s, sizeof(float) * (size_t)k, cudaMemcpyHostToDevice, stream));
-    if (src_half == r->half_states) {
-      const size_t b = (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(k * w);
-      void* to = src_half ? static_cast<void*>(r->state_half + d * w) : static_cast<void*>(r->state_rows + d * w);
-      const char* base = r->host_states ? r->stage + kStageHead : static_cast<const char*>(states);
-      const char* from = base + (src_half ? sizeof(__half) : sizeof(float)) * (size_t)(s * w);
-      R2D2_CUDA_TRY(cudaMemcpyAsync(to, from, b, cudaMemcpyDefault, stream));
-    } else if (src_half) {
-      const __half* staged = reinterpret_cast<const __half*>(r->stage + kStageHead) + s * w;
-      states_from_f16_kernel<<<grid_for(k * w / 8), 256, 0, stream>>>(staged, r->state_rows + d * w, k * w);
-      count_launch();
-      R2D2_CUDA_TRY(cudaGetLastError());
-    } else {
-      R2D2_TRY(convert_half_states(r, d, s, k, stream));
-    }
   }
   for (size_t e = 0; e < im.kept.size(); ++e) {   // every kept episode's piece of this chunk: its leaves checked
     const Episode& ep = im.kept[e];
@@ -1417,30 +1396,16 @@ int replay_global_draw(Replay* r, int stage, int slot, int weighted, float beta,
       global_draw_kernel<false><<<1, 1024, 0, stream>>>(r->tv, g.peers, g.lay, g.world, g.rank, g.batch, slot, g.draw_epoch);
     count_launch();
     R2D2_CUDA_TRY(cudaGetLastError());
-    GatherParams gp;
-    gp.obs_rows = r->obs_rows; gp.act_rows = r->act_rows; gp.rew_rows = r->rew_rows; gp.term_rows = r->term_rows;
-    gp.state_rows = state_source(r);
+    GatherParams gp = ring_gather_params(r);
     char* own = g.peers.base[g.rank];
     gp.leaf = reinterpret_cast<const long long*>(own + g.lay.off_draw_leaf);
-    gp.obs = gp.act = gp.rew = gp.term = nullptr;
     gp.states = reinterpret_cast<float*>(own + g.lay.slot(slot) + g.lay.off_states);   // non-null: state tasks run
-    gp.T = r->rows_per_window; gp.B = g.world * g.batch; gp.O = r->cfg.obs_size; gp.A = r->cfg.n_actions;
-    gp.H = r->cfg.hidden; gp.Bc = g.batch;
+    gp.B = g.world * g.batch; gp.Bc = g.batch;
     const size_t so = g.lay.slot(slot);
     gp.off_obs = so + g.lay.off_obs; gp.off_act = so + g.lay.off_act; gp.off_rew = so + g.lay.off_rew;
     gp.off_term = so + g.lay.off_term; gp.off_states = so + g.lay.off_states;
     gp.dst = g.peers;
-    const long long tasks = (long long)(gp.T + 8) * gp.B;
-    if (r->host_states && r->half_states)
-      gather_host_states_kernel<true, true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
-    else if (r->host_states)
-      gather_host_states_kernel<true, false><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
-    else if (r->half_states)
-      gather_batch_kernel<true, true><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
-    else
-      gather_batch_kernel<true, false><<<grid_for(tasks * 32), 256, 0, stream>>>(gp);
-    count_launch();
-    R2D2_CUDA_TRY(cudaGetLastError());
+    R2D2_TRY(launch_gather<true>(r, gp, (long long)(gp.T + 8) * gp.B, stream));
     R2D2_TRY(global_deliver(g.peers, g.world, g.rank, g.draw_epoch, stream));
     g.draw_stage = 2;
   }

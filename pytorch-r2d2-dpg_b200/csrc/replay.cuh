@@ -43,8 +43,7 @@ int global_receive(const GlobalPeers& p, const GlobalLayout& lay, int world, int
                    float beta, unsigned epoch, cudaStream_t st);
 
 struct Replay;
-int replay_create(Replay** out, const r2d2_replay_config* cfg, int state_storage = R2D2_STATE_F32,
-                  int state_memory = R2D2_STATE_MEMORY_DEVICE);
+int replay_create(Replay** out, const r2d2_replay_config* cfg, const r2d2_replay_options* options);   // null: defaults
 int replay_device_bytes(Replay* r, size_t* out);
 int replay_host_bytes(Replay* r, size_t* out);
 int replay_destroy(Replay* r);

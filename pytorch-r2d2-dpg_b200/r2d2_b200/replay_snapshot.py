@@ -89,8 +89,12 @@ class Header:
     def header_bytes(self) -> int:
         return _FIXED.size + len(self.rng_state)
 
+    def state_row_bytes(self) -> int:
+        """Bytes of one row's recurrent states [4, 2, H] in the stored type."""
+        return (2 if self.state_storage else 4) * 8 * self.hidden
+
     def row_bytes(self) -> int:
-        return 4 * (self.obs_size + self.n_actions + 3) + (2 if self.state_storage else 4) * 8 * self.hidden
+        return 4 * (self.obs_size + self.n_actions + 3) + self.state_row_bytes()
 
     def file_bytes(self) -> int:
         return self.header_bytes + self.n_episodes * _EPISODE.itemsize + self.rows_used * self.row_bytes()
@@ -137,9 +141,8 @@ def check_header(h: Header, path, sizes: tuple, alpha: float, world: int | None 
 
 def _chunk_layout(h: Header, c: int):
     """(offset, bytes) of obs, act, rew, term, states, leaves in a chunk of c rows."""
-    sb = (2 if h.state_storage else 4) * 8 * h.hidden
     parts, off = [], 0
-    for n in (4 * h.obs_size * c, 4 * h.n_actions * c, 4 * c, 4 * c, sb * c, 4 * c):
+    for n in (4 * h.obs_size * c, 4 * h.n_actions * c, 4 * c, 4 * c, h.state_row_bytes() * c, 4 * c):
         parts.append((off, n))
         off += n
     return parts
