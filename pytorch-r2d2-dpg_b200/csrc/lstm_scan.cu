@@ -23,8 +23,9 @@
 // Why no write-after-read hazard remains: CTA d writes step s+1's slice into my buffer b only after its own step-s
 // MMAs (forward) / pointwise (BPTT) consumed the slice I sent at step s, and I send that slice only after a
 // __syncthreads that follows my reads of buffer b at step s-1; a peer is therefore never more than one step ahead of
-// the buffer it writes.  The same chain shows that the next phase of bar[b][d] cannot complete before every thread
-// of mine has observed the current one, so parity waits are unambiguous.
+// the buffer it writes (BPTT: a peer sends its partials in m-tile groups, the first one right after its pointwise
+// phase, so the chain is the same).  The same chain shows that the next phase of bar[b][d] cannot complete before
+// every thread of mine has observed the current one, so parity waits are unambiguous.
 // BPTT activation stage.  None of the BPTT's per-step global inputs (gates[s], cs[s], dh_head) depends on the
 // recurrence, so each thread cp.asyncs step s-1's values for its own cells into stage[plane][n][unit] right after the
 // pointwise phase of step s, and waits for them (cp.async.wait_group 0, no barrier: no thread reads a stage element
@@ -325,6 +326,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
   constexpr int MT = (M_TILES + 7) / 8;  // m-tiles per warp
   constexpr int KS = ROWS_PER_CTA / 16;  // 8
   constexpr bool WS = w_hi_in_smem<H>();
+  // m-tiles per reduce-scatter group: at H = 512 each m-tile's partials leave as soon as they are final; below, a warp
+  // has at most two m-tiles and one group measured faster
+  constexpr int MG = WS ? 1 : MT;
   using SM = BwdSmem<H, NB>;
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
@@ -491,62 +495,67 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) lstm_scan_bwd_kernel(ScanBwdP
 
     if (s > 0) {
       prefetch(s - 1);
-      // ---- partial dh_{s-1}[j, n] over this CTA's 128 gate rows
-      float acc[MT][NT][4];
-#pragma unroll
-      for (int i = 0; i < MT; ++i)
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) acc[i][nt][e] = 0.f;
+      // ---- partial dh_{s-1}[j, n] over this CTA's 128 gate rows, MG m-tiles at a time: a group's partials leave by
+      // st.async as soon as its last k-step is done, so the reduce-scatter overlaps the next group's MMAs.  Every
+      // accumulator sees the same MMAs in the same k order as with one group; the dG fragments are re-read per group.
       const __nv_bfloat16* d_hi = dgs;
       const __nv_bfloat16* d_lo = dgs + NB * DG_LD;
-#pragma unroll
-      for (int ks = 0; ks < KS; ++ks) {
-        uint32_t bh[NT][2], bl[NT][2];
-#pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-          const int off = (nt * 8 + g) * DG_LD + ks * 16 + 2 * c;
-          bh[nt][0] = *reinterpret_cast<const uint32_t*>(d_hi + off);
-          bh[nt][1] = *reinterpret_cast<const uint32_t*>(d_hi + off + 8);
-          bl[nt][0] = *reinterpret_cast<const uint32_t*>(d_lo + off);
-          bl[nt][1] = *reinterpret_cast<const uint32_t*>(d_lo + off + 8);
-        }
-#pragma unroll
-        for (int i = 0; i < MT; ++i) {
-          uint32_t ah[4];
-          if constexpr (WS) {
-            const uint4 v = w_hi_s[((i * KS + ks) * 8 + w) * 32 + lane];
-            ah[0] = v.x; ah[1] = v.y; ah[2] = v.z; ah[3] = v.w;
-          } else {
-#pragma unroll
-            for (int f = 0; f < 4; ++f) ah[f] = a_hi[i][ks][f];
-          }
-#pragma unroll
-          for (int nt = 0; nt < NT; ++nt) {
-            mma_bf16_16816(acc[i][nt], a_lo[i][ks], bh[nt]);
-            mma_bf16_16816(acc[i][nt], ah, bl[nt]);
-            mma_bf16_16816(acc[i][nt], ah, bh[nt]);
-          }
-        }
-      }
-      // ---- reduce-scatter: partial rows j go to the CTA that owns unit j (slot = my rank), fp32 st.async into its
-      // shared memory, each store completing its bytes on the owner's bar[buf ^ 1][rank]
       const uint32_t slot_bar = sm90::smem_u32(bar + (buf ^ 1) * C + rank);
 #pragma unroll
-      for (int i = 0; i < MT; ++i) {
-        const int mi = w * MT + i;
-        if (mi < M_TILES) {
+      for (int i0 = 0; i0 < MT; i0 += MG) {
+        float acc[MG][NT][4];
 #pragma unroll
-          for (int h2 = 0; h2 < 2; ++h2) {
-            const int j = mi * 16 + g + h2 * 8;
-            const int owner = j >> 5, jl = j & 31;
-            const uint32_t slot = sm90::map_cluster(
-                sm90::smem_u32(ps + (((buf ^ 1) * C + rank) * UNITS_PER_CTA + jl) * SM::PS_LD), owner);
-            const uint32_t owner_bar = sm90::map_cluster(slot_bar, owner);
+        for (int i = 0; i < MG; ++i)
 #pragma unroll
-            for (int nt = 0; nt < NT; ++nt)
-              sm90::st_async_f2(slot + (nt * 8 + 2 * c) * 4, acc[i][nt][2 * h2], acc[i][nt][2 * h2 + 1], owner_bar);
+          for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) acc[i][nt][e] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          uint32_t bh[NT][2], bl[NT][2];
+#pragma unroll
+          for (int nt = 0; nt < NT; ++nt) {
+            const int off = (nt * 8 + g) * DG_LD + ks * 16 + 2 * c;
+            bh[nt][0] = *reinterpret_cast<const uint32_t*>(d_hi + off);
+            bh[nt][1] = *reinterpret_cast<const uint32_t*>(d_hi + off + 8);
+            bl[nt][0] = *reinterpret_cast<const uint32_t*>(d_lo + off);
+            bl[nt][1] = *reinterpret_cast<const uint32_t*>(d_lo + off + 8);
+          }
+#pragma unroll
+          for (int i = 0; i < MG; ++i) {
+            uint32_t ah[4];
+            if constexpr (WS) {
+              const uint4 v = w_hi_s[(((i0 + i) * KS + ks) * 8 + w) * 32 + lane];
+              ah[0] = v.x; ah[1] = v.y; ah[2] = v.z; ah[3] = v.w;
+            } else {
+#pragma unroll
+              for (int f = 0; f < 4; ++f) ah[f] = a_hi[i0 + i][ks][f];
+            }
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+              mma_bf16_16816(acc[i][nt], a_lo[i0 + i][ks], bh[nt]);
+              mma_bf16_16816(acc[i][nt], ah, bl[nt]);
+              mma_bf16_16816(acc[i][nt], ah, bh[nt]);
+            }
+          }
+        }
+        // ---- reduce-scatter: partial rows j go to the CTA that owns unit j (slot = my rank), fp32 st.async into its
+        // shared memory, each store completing its bytes on the owner's bar[buf ^ 1][rank]
+#pragma unroll
+        for (int i = 0; i < MG; ++i) {
+          const int mi = w * MT + i0 + i;
+          if (mi < M_TILES) {
+#pragma unroll
+            for (int h2 = 0; h2 < 2; ++h2) {
+              const int j = mi * 16 + g + h2 * 8;
+              const int owner = j >> 5, jl = j & 31;
+              const uint32_t slot = sm90::map_cluster(
+                  sm90::smem_u32(ps + (((buf ^ 1) * C + rank) * UNITS_PER_CTA + jl) * SM::PS_LD), owner);
+              const uint32_t owner_bar = sm90::map_cluster(slot_bar, owner);
+#pragma unroll
+              for (int nt = 0; nt < NT; ++nt)
+                sm90::st_async_f2(slot + (nt * 8 + 2 * c) * 4, acc[i][nt][2 * h2], acc[i][nt][2 * h2 + 1], owner_bar);
+            }
           }
         }
       }
