@@ -180,6 +180,31 @@ int r2d2_policy_step(const r2d2_net_shape* shape, const float* const params[4], 
                      const float* state_in, float* state_out, float* mu, int N, float* workspace,
                      r2d2_stream_t stream);
 
+/* r2d2_policy_step with an observation normaliser: obs_mean, obs_inv_std DEVICE [O] (both or neither; NULL is
+ * r2d2_policy_step), clip finite and > 0.  Phase 1 reads x_hat = clamp(fl(fl(x - mean) * inv_std), -clip, clip) (NaN
+ * passes through) in place of every obs value as it stages the obs rows - the bits r2d2_obs_normalize writes - so the
+ * step equals r2d2_policy_step on pre-normalised obs bit for bit; lane n's outputs stay independent of N.  Same five
+ * launches, the first one a separate kernel. */
+int r2d2_policy_step_ex(const r2d2_net_shape* shape, const float* const params[4], const float* obs,
+                        const float* state_in, float* state_out, float* mu, int N, float* workspace,
+                        const float* obs_mean, const float* obs_inv_std, float clip, r2d2_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Observation normalisation (off unless a caller attaches it).  Statistics are moment blocks of [1 + 2 O] doubles:
+ * count, mean [O], M2 [O] (the sum of squared deviations from the mean).  The fp32 pair every transform reads is
+ * mean_f = (float) mean, inv_std_f = (float)(1 / sqrt(M2 / n + 1e-8)), each rounded once from double, and the transform
+ * is x_hat = clamp(fl(fl(x - mean_f) * inv_std_f), -clip, clip) with NaN passing through (torch.clamp's behaviour).
+ * ---------------------------------------------------------------------------------------------- */
+/* Merge W blocks (DEVICE [W, 1 + 2 O]) into `running` (DEVICE [1 + 2 O]) in index order with Chan's parallel formula
+ * (n = na + nb, d = mb - ma, mean = ma + d nb / n, M2 = M2a + M2b + d^2 na nb / n; an empty side takes the other's values
+ * unchanged), then rewrite DEVICE mean_f, inv_std_f [O] from it; with n = 0 they become 0 and 1.  mean_f and inv_std_f
+ * may both be NULL (merge only).  One single-CTA launch, deterministic. */
+int r2d2_obs_norm_merge(double* running, const double* blocks, int W, int O, float* mean_f, float* inv_std_f,
+                        r2d2_stream_t stream);
+/* y [rows, O] = x_hat of x [rows, O] (DEVICE; y may be x).  One grid-stride launch. */
+int r2d2_obs_normalize(const float* x, float* y, long long rows, int O, const float* mean_f, const float* inv_std_f,
+                       float clip, r2d2_stream_t stream);
+
 /* torch.optim.Adam defaults (learner.py:50-53,114,128) on a flat buffer; grad is multiplied by grad_scale first. */
 int r2d2_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, int step,
                    float lr, float beta1, float beta2, float eps, float grad_scale, r2d2_stream_t stream);
@@ -261,6 +286,26 @@ int r2d2_replay_add_episodes(r2d2_replay_t* r, int n_episodes, const int* n_rows
                              const float* obs, const float* act, const float* rew, const float* term,
                              const float* states, const float* leaf_prio, long long* row_start_out,
                              long long* n_evicted_out, long long* sequence_counter_out, r2d2_stream_t stream);
+
+/* r2d2_replay_add_episodes plus the observation moments of the call.  obs_moments (DEVICE [1 + 2 O], or NULL for
+ * r2d2_replay_add_episodes) receives (count, mean, M2) of the call's rows that are no pad row (the last n_step rows of
+ * each episode, actor.py:173) and hold only finite obs values.  They are taken per ring run right after its copy -
+ * a call wider than the ring overwrites its own earlier rows - in two passes (mean, then squared deviations) with
+ * double partials over a fixed partition of the rows, added in a fixed order and merged run by run (Chan): the bits do
+ * not depend on the schedule.  n_nonfinite_out (host, optional): the non-pad rows left out for a NaN or +-inf value.
+ * Five more launches per ring run. */
+int r2d2_replay_add_episodes_ex(r2d2_replay_t* r, int n_episodes, const int* n_rows, const int* n_starts,
+                                const float* obs, const float* act, const float* rew, const float* term,
+                                const float* states, const float* leaf_prio, long long* row_start_out,
+                                long long* n_evicted_out, long long* sequence_counter_out, double* obs_moments,
+                                long long* n_nonfinite_out, r2d2_stream_t stream);
+
+/* Observation normaliser of every gather of this shard (r2d2_replay_sample, _sample_weighted, _gather and the global
+ * draw's owner-side gather): the batch's obs hold x_hat of the stored raw rows (see r2d2_obs_norm_merge).  DEVICE
+ * mean_f, inv_std_f [O], read at every gather (the caller keeps them alive and may rewrite them in stream order);
+ * 16-byte aligned when O is a multiple of 4.  clip finite and > 0.  Both NULL: raw obs again.  The stored rows, the
+ * snapshots and the export stay raw. */
+int r2d2_replay_set_obs_normalizer(r2d2_replay_t* r, const float* mean_f, const float* inv_std_f, float clip);
 
 /* Draw `batch` starts from DEVICE uniforms u[batch] in [0,1) and gather the time-major batch:
  * leaf_idx [batch] (int64, start row = tree leaf), obs [T',batch,O], act [T',batch,A], rew [T',batch],

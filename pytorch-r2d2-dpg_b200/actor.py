@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from models import ActorNet, CriticNet
+from r2d2_b200 import obs_norm as obs_norm_mod
 from r2d2_b200 import td_options
 from replay_memory import ReplayMemory
 from utils import calc_priority, get_obs, inverse_value_rescale, invertical_vf, value_rescale
@@ -89,6 +90,7 @@ class Actor:
         self.target_actor = deepcopy(self.actor)
         self.critic = CriticNet(self.obs_size, self.action_size, 0, hidden=self.hidden).to(self.device).eval()
         self.target_critic = deepcopy(self.critic)
+        self.obs_norm = None      # model.pt's `obs_norm` {mean_f, inv_std_f, clip} when the learner normalises obs
         self.load_model()
 
     def _nets(self):
@@ -105,9 +107,15 @@ class Actor:
                 model_dict = torch.load(path, map_location=self.device)
                 for name, net in self._nets():
                     net.load_state_dict(model_dict[name])
+                self.obs_norm = model_dict.get('obs_norm')
                 return
             except Exception:
                 sleep(np.random.rand() * 2 + 0.5)
+
+    def _obs(self, x):
+        """What the nets read: the raw observation, or its normalised form under the learner's statistics."""
+        n = self.obs_norm
+        return x if n is None else obs_norm_mod.normalize_torch(x, n['mean_f'], n['inv_std_f'], n['clip'])
 
     def calc_nstep_reward(self):
         """Overwrite rewards with their n-step discounted sums (actor.py:74-76)."""
@@ -126,11 +134,12 @@ class Actor:
         self.td_loss = deque(maxlen=self.learning_length)
         self.priority = []
         t = lambda a: torch.from_numpy(np.asarray(a, np.float32)).to(self.device).unsqueeze(0)  # noqa: E731
+        o = lambda a: self._obs(t(a))  # noqa: E731
         for i in range(self.n_step):
-            nxt = t(self.sequence[i][0])
+            nxt = o(self.sequence[i][0])
             self.target_critic(nxt, self.target_actor(nxt))
         for i in range(len(self.sequence) - self.n_step):
-            obs, action, nxt = t(self.sequence[i][0]), t(self.sequence[i][1]), t(self.sequence[i + self.n_step][0])
+            obs, action, nxt = o(self.sequence[i][0]), t(self.sequence[i][1]), o(self.sequence[i + self.n_step][0])
             q = self.critic(obs, action).cpu().numpy()
             q_next = self.target_critic(nxt, self.target_actor(nxt)).cpu().numpy()
             if i >= self.burn_in_length:
@@ -157,7 +166,7 @@ class Actor:
             while not time_step.last():
                 states = [net.get_state() for _, net in self._nets()]
                 with torch.no_grad():
-                    x = torch.from_numpy(obs).to(self.device)
+                    x = self._obs(torch.from_numpy(obs).to(self.device))
                     action = self.actor(x)
                     self.critic(x, action)
                     self.target_critic(x, self.target_actor(x))

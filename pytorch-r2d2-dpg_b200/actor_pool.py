@@ -43,10 +43,12 @@ class ModelsStepper(StateRing):
         super().__init__(obs_size, n_actions, hidden, n_lanes, device, max_episode_steps)
         self.nets = [cls(obs_size, n_actions, 0, hidden=hidden).to(self.device).eval()
                      for cls in (ActorNet, ActorNet, CriticNet, CriticNet)]
+        self.obs_norm = None
 
     def load(self, model_dict):
         for net, name in zip(self.nets, NETS):
             net.load_state_dict(model_dict[name])
+        self.obs_norm = model_dict.get("obs_norm")    # {mean_f, inv_std_f, clip}: the nets read normalised obs
 
     @torch.no_grad()
     def _step(self, obs, state_in, state_out):
@@ -54,6 +56,10 @@ class ModelsStepper(StateRing):
         for k, net in enumerate(self.nets):
             net.set_state(state_in[k, 0], state_in[k, 1])
         x = torch.as_tensor(np.asarray(obs, np.float32)).to(self.device)
+        if self.obs_norm is not None:
+            from r2d2_b200.obs_norm import normalize_torch
+            n = self.obs_norm
+            x = normalize_torch(x, n["mean_f"], n["inv_std_f"], n["clip"])
         mu = actor(x)
         critic(x, mu)
         target_critic(x, target_actor(x))
@@ -120,7 +126,8 @@ class ActorPool:
             model_dict["critic"], model_dict["target_actor"], model_dict["target_critic"], episodes,
             hidden=self.hidden, burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
             gamma=self.gamma, rewards_are_raw=True, device=self.device, rescaling=self.td_options.value_rescaling,
-            eps=self.td_options.rescaling_eps, priority_metric=self.td_options.priority_metric)
+            eps=self.td_options.rescaling_eps, priority_metric=self.td_options.priority_metric,
+            obs_norm=model_dict.get("obs_norm"))
 
     def load_model(self):
         """Follow the learner's model.pt (actor.py:50-72); retried while the file is being replaced."""

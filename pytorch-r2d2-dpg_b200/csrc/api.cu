@@ -8,6 +8,7 @@
 #include "learner.cuh"
 #include "lstm_scan.cuh"
 #include "net.cuh"
+#include "obs_norm.cuh"
 #include "policy.cuh"
 #include "replay.cuh"
 #include "td3.cuh"
@@ -223,6 +224,23 @@ int r2d2_policy_step(const r2d2_net_shape* shape, const float* const params[4], 
                      workspace, S(stream));
 }
 
+int r2d2_policy_step_ex(const r2d2_net_shape* shape, const float* const params[4], const float* obs,
+                        const float* state_in, float* state_out, float* mu, int N, float* workspace,
+                        const float* obs_mean, const float* obs_inv_std, float clip, r2d2_stream_t stream) {
+  R2D2_REQUIRE(shape, "null");
+  return policy_step(shape->obs_size, shape->n_actions, shape->hidden, params, obs, state_in, state_out, mu, N,
+                     workspace, S(stream), obs_mean, obs_inv_std, clip);
+}
+
+int r2d2_obs_norm_merge(double* running, const double* blocks, int W, int O, float* mean_f, float* inv_std_f,
+                        r2d2_stream_t stream) {
+  return obs_norm_merge(running, blocks, W, O, mean_f, inv_std_f, S(stream));
+}
+int r2d2_obs_normalize(const float* x, float* y, long long rows, int O, const float* mean_f, const float* inv_std_f,
+                       float clip, r2d2_stream_t stream) {
+  return obs_normalize(x, y, rows, O, mean_f, inv_std_f, clip, S(stream));
+}
+
 int r2d2_adam_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, long long n, int step,
                    float lr, float beta1, float beta2, float eps, float grad_scale, r2d2_stream_t stream) {
   return adam_step(params, grads, exp_avg, exp_avg_sq, n, step, lr, beta1, beta2, eps, grad_scale, S(stream));
@@ -257,6 +275,18 @@ int r2d2_replay_add_episodes(r2d2_replay_t* r, int n_episodes, const int* n_rows
                              long long* n_evicted_out, long long* sequence_counter_out, r2d2_stream_t stream) {
   return replay_add_episodes(reinterpret_cast<Replay*>(r), n_episodes, n_rows, n_starts, obs, act, rew, term, states,
                              leaf_prio, row_start_out, n_evicted_out, sequence_counter_out, S(stream));
+}
+int r2d2_replay_add_episodes_ex(r2d2_replay_t* r, int n_episodes, const int* n_rows, const int* n_starts,
+                                const float* obs, const float* act, const float* rew, const float* term,
+                                const float* states, const float* leaf_prio, long long* row_start_out,
+                                long long* n_evicted_out, long long* sequence_counter_out, double* obs_moments,
+                                long long* n_nonfinite_out, r2d2_stream_t stream) {
+  return replay_add_episodes(reinterpret_cast<Replay*>(r), n_episodes, n_rows, n_starts, obs, act, rew, term, states,
+                             leaf_prio, row_start_out, n_evicted_out, sequence_counter_out, S(stream), obs_moments,
+                             n_nonfinite_out);
+}
+int r2d2_replay_set_obs_normalizer(r2d2_replay_t* r, const float* mean_f, const float* inv_std_f, float clip) {
+  return replay_set_obs_normalizer(reinterpret_cast<Replay*>(r), mean_f, inv_std_f, clip);
 }
 int r2d2_replay_sample(r2d2_replay_t* r, const float* u, int batch, long long* leaf_idx, float* obs, float* act,
                        float* rew, float* term, float* states, r2d2_stream_t stream) {

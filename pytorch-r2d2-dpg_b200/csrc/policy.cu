@@ -25,6 +25,7 @@
 //
 // Each kernel issues L2 prefetches of its weight rows before griddepcontrol.wait, so they overlap the tail of the
 // phase before; every kernel executes the wait, which makes the chain transitive (phase 5 may read phase 1's G).
+#include "obs_norm.cuh"
 #include "policy.cuh"
 
 namespace r2d2 {
@@ -46,6 +47,8 @@ struct StepArgs {
   float* Z;                        // [4,N,H]  l1 outputs (critics: obs half until phase 4)
   float* mu_t;                     // [N,A]
   int N, O, A, H;
+  const float *obs_mean, *obs_inv_std;   // r2d2_policy_step_ex: phase 1 stages obs_norm_apply(obs) (the kNorm kernel)
+  float obs_clip;
 };
 
 struct NetView {
@@ -76,15 +79,18 @@ __device__ __forceinline__ void prefetch_rows(const float* const (&w)[4], int K)
       asm volatile("prefetch.global.L2 [%0];" ::"l"(w[r] + k));
 }
 
-// xs[k][n] = src[n*ld + k] (tanh'd if kTanh) for k < kc, n < nl; zero for nl <= n < NT
-template <bool kTanh>
-__device__ __forceinline__ void stage(float* xs, const float* src, long long ld, int kc, int nl) {
+// xs[k][n] = src[n*ld + k] (tanh'd if kTanh; kNorm: obs_norm_apply with mean[k], inv_std[k]) for k < kc, n < nl;
+// zero for nl <= n < NT
+template <bool kTanh, bool kNorm = false>
+__device__ __forceinline__ void stage(float* xs, const float* src, long long ld, int kc, int nl,
+                                      const float* mean = nullptr, const float* inv_std = nullptr, float clip = 0.f) {
   for (int i = threadIdx.x; i < NT * kc; i += THREADS) {
     const int n = i / kc, k = i - n * kc;
     float x = 0.0f;
     if (n < nl) {
       x = src[(long long)n * ld + k];
       if (kTanh) x = tanhf(x);
+      if (kNorm) x = obs_norm_apply(x, __ldg(mean + k), __ldg(inv_std + k), clip);
     }
     xs[k * XS + n] = x;
   }
@@ -106,9 +112,10 @@ __device__ __forceinline__ void reduce_round(float (&acc)[4 * NT], int lane) {
 
 // v[i] = sum_k w[r][k] * x[n][k] for (r, n) = (lane / 8, 2 * (lane % 8) + i), x = src[n*ld + k] over the tile's
 // nl lanes.  Block-uniform K and src: every warp of the block calls it.
-template <bool kTanh>
+template <bool kTanh, bool kNorm = false>
 __device__ __forceinline__ void rows_dot(float (&v)[2], const float* const (&w)[4], int K, const float* src,
-                                         long long ld, int nl, float* xs) {
+                                         long long ld, int nl, float* xs, const float* mean = nullptr,
+                                         const float* inv_std = nullptr, float clip = 0.f) {
   const int lane = threadIdx.x & 31;
   float acc[4 * NT];
 #pragma unroll
@@ -116,7 +123,8 @@ __device__ __forceinline__ void rows_dot(float (&v)[2], const float* const (&w)[
   for (int k0 = 0; k0 < K; k0 += KC) {
     const int kc = min(KC, K - k0);
     __syncthreads();                                   // the previous chunk is consumed
-    stage<kTanh>(xs, src + k0, ld, kc, nl);
+    if (kNorm) stage<kTanh, true>(xs, src + k0, ld, kc, nl, mean + k0, inv_std + k0, clip);
+    else stage<kTanh>(xs, src + k0, ld, kc, nl);
     __syncthreads();
 #pragma unroll 2
     for (int k = lane; k < kc; k += 32) {
@@ -176,8 +184,9 @@ __device__ __forceinline__ void cell_update(const float (&v)[2], const StepArgs&
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;"); }
 
-template <int PHASE>
-__global__ void __launch_bounds__(THREADS, 2) policy_phase_kernel(const StepArgs a) {
+// kNormObs (phase 1 only): the obs rows are normalised as they are staged
+template <int PHASE, bool kNormObs>
+__device__ __forceinline__ void policy_phase(const StepArgs& a) {
   __shared__ __align__(16) float xs[KC * XS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile0 = blockIdx.y * NT;
@@ -212,7 +221,10 @@ __global__ void __launch_bounds__(THREADS, 2) policy_phase_kernel(const StepArgs
       prefetch_rows(w, a.O);
       pdl_wait();
       pdl_launch_dependents();
-      rows_dot<false>(v, w, a.O, a.obs + (size_t)tile0 * a.O, a.O, nl, xs);
+      if (kNormObs)
+        rows_dot<false, true>(v, w, a.O, a.obs + (size_t)tile0 * a.O, a.O, nl, xs, a.obs_mean, a.obs_inv_std, a.obs_clip);
+      else
+        rows_dot<false>(v, w, a.O, a.obs + (size_t)tile0 * a.O, a.O, nl, xs);
       const int row = 4 * q + r_out;
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
@@ -272,7 +284,17 @@ __global__ void __launch_bounds__(THREADS, 2) policy_phase_kernel(const StepArgs
 }
 
 template <int PHASE>
-int launch_phase(dim3 grid, const StepArgs& a, cudaStream_t stream) {
+__global__ void __launch_bounds__(THREADS, 2) policy_phase_kernel(const StepArgs a) {
+  policy_phase<PHASE, false>(a);
+}
+
+// phase 1 of r2d2_policy_step_ex with an observation normaliser
+__global__ void __launch_bounds__(THREADS, 2) policy_obs_norm_phase1_kernel(const StepArgs a) {
+  policy_phase<1, true>(a);
+}
+
+template <typename Kernel>
+int launch_phase(Kernel kernel, dim3 grid, const StepArgs& a, cudaStream_t stream) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = dim3(THREADS);
@@ -283,7 +305,7 @@ int launch_phase(dim3 grid, const StepArgs& a, cudaStream_t stream) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  R2D2_CUDA_TRY(cudaLaunchKernelEx(&cfg, policy_phase_kernel<PHASE>, a));
+  R2D2_CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, a));
   count_launch();
   return R2D2_OK;
 }
@@ -296,10 +318,13 @@ size_t policy_workspace_floats(int O, int A, int H, int N) {
 }
 
 int policy_step(int O, int A, int H, const float* const params[4], const float* obs, const float* state_in,
-                float* state_out, float* mu, int N, float* workspace, cudaStream_t stream) {
+                float* state_out, float* mu, int N, float* workspace, cudaStream_t stream, const float* obs_mean,
+                const float* obs_inv_std, float obs_clip) {
   R2D2_REQUIRE(params && params[0] && params[1] && params[2] && params[3] && obs && state_in && state_out && mu &&
                    workspace, "null");
   R2D2_REQUIRE(state_in != state_out, "state_in and state_out must be different buffers");
+  R2D2_REQUIRE((obs_mean == nullptr) == (obs_inv_std == nullptr), "obs_mean and obs_inv_std are both given or both NULL");
+  R2D2_REQUIRE(!obs_mean || (obs_clip > 0.f && obs_clip <= 3.402823466e38f), "clip must be finite and > 0");
   if (N < 1 || N > kPolicyMaxLanes || H < 32 || H > kPolicyMaxHidden || H % 32 != 0 || A < 1 ||
       A > kPolicyMaxActions || O < 1) {
     set_last_error("r2d2_policy_step: unsupported shape N=" + std::to_string(N) + " O=" + std::to_string(O) +
@@ -315,13 +340,16 @@ int policy_step(int O, int A, int H, const float* const params[4], const float* 
   a.Z = a.G + (size_t)N * H * 16;
   a.mu_t = a.Z + (size_t)N * H * 4;
   a.N = N; a.O = O; a.A = A; a.H = H;
+  a.obs_mean = obs_mean; a.obs_inv_std = obs_inv_std; a.obs_clip = obs_clip;
   const unsigned tiles = (unsigned)ceil_div(N, NT);
   const unsigned head_blocks = (unsigned)ceil_div(ceil_div(A, 4), WARPS);
-  R2D2_TRY(launch_phase<1>(dim3(H / WARPS + H / (4 * WARPS), tiles, 4), a, stream));
-  R2D2_TRY(launch_phase<2>(dim3(H / WARPS, tiles, 2), a, stream));
-  R2D2_TRY(launch_phase<3>(dim3(head_blocks, tiles, 2), a, stream));
-  R2D2_TRY(launch_phase<4>(dim3(H / (4 * WARPS), tiles, 2), a, stream));
-  R2D2_TRY(launch_phase<5>(dim3(H / WARPS, tiles, 2), a, stream));
+  const dim3 grid1(H / WARPS + H / (4 * WARPS), tiles, 4);
+  if (obs_mean) R2D2_TRY(launch_phase(policy_obs_norm_phase1_kernel, grid1, a, stream));
+  else R2D2_TRY(launch_phase(policy_phase_kernel<1>, grid1, a, stream));
+  R2D2_TRY(launch_phase(policy_phase_kernel<2>, dim3(H / WARPS, tiles, 2), a, stream));
+  R2D2_TRY(launch_phase(policy_phase_kernel<3>, dim3(head_blocks, tiles, 2), a, stream));
+  R2D2_TRY(launch_phase(policy_phase_kernel<4>, dim3(H / (4 * WARPS), tiles, 2), a, stream));
+  R2D2_TRY(launch_phase(policy_phase_kernel<5>, dim3(H / WARPS, tiles, 2), a, stream));
   return R2D2_OK;
 }
 

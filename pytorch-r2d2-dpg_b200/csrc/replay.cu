@@ -21,6 +21,7 @@
 #include <map>
 #include <vector>
 
+#include "obs_norm.cuh"
 #include "peer_sync.cuh"
 #include "replay.cuh"
 
@@ -324,6 +325,8 @@ struct GatherParams {
   int Bc;
   size_t off_obs, off_act, off_rew, off_term, off_states;
   GlobalPeers dst;
+  const float *norm_mean, *norm_inv_std;   // kNormObs: the shard's observation normaliser (r2d2_replay_set_obs_normalizer)
+  float norm_clip;
 };
 
 __device__ __forceinline__ void warp_copy_row(const float* __restrict__ src, float* __restrict__ dst, int n, int lane) {
@@ -333,6 +336,26 @@ __device__ __forceinline__ void warp_copy_row(const float* __restrict__ src, flo
     for (int k = lane; k < (n >> 2); k += 32) d4[k] = __ldg(s4 + k);
   } else {
     for (int k = lane; k < n; k += 32) dst[k] = __ldg(src + k);
+  }
+}
+
+// warp_copy_row with the observation transform applied to every element (obs_norm_apply); feature k of the row reads
+// mean[k] and inv_std[k], vectorised as the copy is.
+__device__ __forceinline__ void warp_norm_row(const float* __restrict__ src, float* __restrict__ dst, int n, int lane,
+                                              const float* __restrict__ mean, const float* __restrict__ inv_std,
+                                              float clip) {
+  if ((n & 3) == 0) {
+    const float4* s4 = reinterpret_cast<const float4*>(src);
+    const float4* m4 = reinterpret_cast<const float4*>(mean);
+    const float4* i4 = reinterpret_cast<const float4*>(inv_std);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    for (int k = lane; k < (n >> 2); k += 32) {
+      const float4 x = __ldg(s4 + k), m = __ldg(m4 + k), s = __ldg(i4 + k);
+      d4[k] = make_float4(obs_norm_apply(x.x, m.x, s.x, clip), obs_norm_apply(x.y, m.y, s.y, clip),
+                          obs_norm_apply(x.z, m.z, s.z, clip), obs_norm_apply(x.w, m.w, s.w, clip));
+    }
+  } else {
+    for (int k = lane; k < n; k += 32) dst[k] = obs_norm_apply(__ldg(src + k), __ldg(mean + k), __ldg(inv_std + k), clip);
   }
 }
 
@@ -437,7 +460,8 @@ __device__ __forceinline__ void host_widen_row(const __half* __restrict__ src, f
 // nh * B + b; row task t * B + b follows at 8 B + t * B + b), so that every host read is in flight from the start of the
 // launch and overlaps the HBM row copies instead of adding a host round trip after them; the row tasks are unchanged.
 // The two tiers are separate kernels (gather_batch_kernel and gather_host_states_kernel) over this one body.
-template <bool kPerDraw, bool kHalfStates, bool kHostStates>
+// kNormObs: the obs rows go through the shard's observation normaliser (the *_norm_kernel instantiations).
+template <bool kPerDraw, bool kHalfStates, bool kHostStates, bool kNormObs>
 __device__ __forceinline__ void gather_batch(GatherParams g) {
   const int lane = threadIdx.x & 31;
   const long long warp0 = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
@@ -464,7 +488,10 @@ __device__ __forceinline__ void gather_batch(GatherParams g) {
     } else if (kHostStates ? t >= lead : task < row_tasks) {
       const long long r = leaf + (t - lead);
       const long long o = (long long)(t - lead) * ld + col;
-      if (obs) warp_copy_row(g.obs_rows + r * g.O, obs + o * g.O, g.O, lane);
+      if (obs) {
+        if (kNormObs) warp_norm_row(g.obs_rows + r * g.O, obs + o * g.O, g.O, lane, g.norm_mean, g.norm_inv_std, g.norm_clip);
+        else warp_copy_row(g.obs_rows + r * g.O, obs + o * g.O, g.O, lane);
+      }
       if (act) warp_copy_row(g.act_rows + r * g.A, act + o * g.A, g.A, lane);
       if (lane == 0) {
         if (rew) rew[o] = __ldg(g.rew_rows + r);
@@ -491,12 +518,116 @@ __device__ __forceinline__ void gather_batch(GatherParams g) {
 
 template <bool kPerDraw = false, bool kHalfStates = false>
 __global__ void __launch_bounds__(256) gather_batch_kernel(GatherParams g) {
-  gather_batch<kPerDraw, kHalfStates, false>(g);
+  gather_batch<kPerDraw, kHalfStates, false, false>(g);
 }
 
 template <bool kPerDraw = false, bool kHalfStates = false>
 __global__ void __launch_bounds__(256) gather_host_states_kernel(GatherParams g) {
-  gather_batch<kPerDraw, kHalfStates, true>(g);
+  gather_batch<kPerDraw, kHalfStates, true, false>(g);
+}
+
+template <bool kPerDraw = false, bool kHalfStates = false>
+__global__ void __launch_bounds__(256) gather_batch_norm_kernel(GatherParams g) {
+  gather_batch<kPerDraw, kHalfStates, false, true>(g);
+}
+
+template <bool kPerDraw = false, bool kHalfStates = false>
+__global__ void __launch_bounds__(256) gather_host_states_norm_kernel(GatherParams g) {
+  gather_batch<kPerDraw, kHalfStates, true, true>(g);
+}
+
+// ---- observation moments at ingest (r2d2_replay_add_episodes_ex) ----
+// Per ring run, right after its copy: a row counts when it is no pad row and all its O values are finite; then two
+// passes over a fixed partition of the run's rows into chunks of kMomChunk - the sums (mean), then the squared
+// deviations from that mean (M2) - with one double partial per (chunk, feature), added in chunk order by one CTA.  No
+// floating-point atomics: the bits do not depend on the schedule.
+constexpr int kMomChunk = 128;
+
+// valid[i] = keep[i] && every obs value of row i is finite, one warp per row, grid-stride over the rows (the grid is
+// capped: a run may have any number of rows); kept rows that are not finite are counted (integer atomics, one per row).
+__global__ void __launch_bounds__(256) obs_row_valid_kernel(const float* __restrict__ obs, const unsigned char* __restrict__ keep,
+                                                            long long n, int O, unsigned char* __restrict__ valid,
+                                                            unsigned long long* __restrict__ n_bad) {
+  const int lane = threadIdx.x & 31;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long row = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; row < n; row += n_warps) {   // warp-uniform
+    bool fin = true;
+    for (int k = lane; k < O; k += 32) fin = fin && isfinite(obs[row * O + k]);
+    fin = __all_sync(0xffffffffu, fin);
+    if (lane == 0) {
+      const bool kept = keep[row] != 0;
+      valid[row] = kept && fin;
+      if (kept && !fin) atomicAdd(n_bad, 1ull);
+    }
+  }
+}
+
+// grid (chunks, ceil(O / 32)), block (32, 8): thread (x, y) sums feature 32 by + x over rows y, y + 8, .. of chunk bx,
+// then the 8 row groups are added in order.  The chunk index is the x dimension, so a run of up to 2^31 - 1 chunks fits
+// one launch.  kSquares: (x - mean)^2 instead of x.  Pass 1 also counts the chunk's rows.
+template <bool kSquares>
+__global__ void __launch_bounds__(256) obs_moment_partial_kernel(const float* __restrict__ obs,
+                                                                 const unsigned char* __restrict__ valid, long long n,
+                                                                 int O, const double* __restrict__ mean,
+                                                                 double* __restrict__ part, int* __restrict__ count) {
+  __shared__ double s[8][33];
+  const int o = blockIdx.y * 32 + threadIdx.x;
+  const long long r0 = (long long)blockIdx.x * kMomChunk, r1 = min(n, r0 + kMomChunk);
+  double acc = 0.0;
+  if (o < O) {
+    const double m = kSquares ? mean[o] : 0.0;
+    for (long long r = r0 + threadIdx.y; r < r1; r += 8) {
+      if (!valid[r]) continue;
+      const double x = (double)obs[r * O + o];
+      if (kSquares) {
+        const double d = __dsub_rn(x, m);
+        acc = __dadd_rn(acc, __dmul_rn(d, d));
+      } else {
+        acc = __dadd_rn(acc, x);
+      }
+    }
+  }
+  s[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y == 0 && o < O) {
+    double t = s[0][threadIdx.x];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) t = __dadd_rn(t, s[k][threadIdx.x]);
+    part[blockIdx.x * (long long)O + o] = t;
+  }
+  if (!kSquares && blockIdx.y == 0 && threadIdx.x == 0 && threadIdx.y == 0) {
+    int c = 0;
+    for (long long r = r0; r < r1; ++r) c += valid[r];
+    count[blockIdx.x] = c;
+  }
+}
+
+// One CTA.  Pass 1: the run's count and mean into run[0], run[1 .. O].  Pass 2: the run's M2, and the run merged into
+// the call's block `acc` (Chan, chan_merge).
+template <bool kSquares>
+__global__ void __launch_bounds__(256) obs_moment_finish_kernel(const double* __restrict__ part,
+                                                                const int* __restrict__ count, int chunks, int O,
+                                                                double* __restrict__ run, double* __restrict__ acc) {
+  long long c = 0;
+  for (int k = 0; k < chunks; ++k) c += count[k];
+  const double nb = (double)c, na = kSquares ? acc[0] : 0.0;
+  for (int o = threadIdx.x; o < O; o += blockDim.x) {
+    double t = 0.0;
+    for (int k = 0; k < chunks; ++k) t = __dadd_rn(t, part[(long long)k * O + o]);
+    if (!kSquares) {
+      run[1 + o] = c ? __ddiv_rn(t, nb) : 0.0;
+    } else {
+      double m = acc[1 + o], m2 = acc[1 + O + o];
+      chan_merge(na, m, m2, nb, run[1 + o], t);
+      acc[1 + o] = m;
+      acc[1 + O + o] = m2;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (kSquares) acc[0] = __dadd_rn(na, nb);
+    else run[0] = nb;
+  }
 }
 
 int grid_for(long long total) {
@@ -530,7 +661,14 @@ struct Replay {
   // grow-only device staging block (stage_states): [count (16 B) | the packed states of the largest call so far]
   char* stage = nullptr;
   size_t stage_bytes = 0;
-  size_t device_bytes = 0;   // every device allocation of the shard (rows, tree, staging)
+  // grow-only device scratch of the ingest moments: [n_bad (16 B) | run block 1 + O | partials | counts | keep | valid]
+  char* mom = nullptr;
+  size_t mom_bytes = 0;
+  size_t device_bytes = 0;   // every device allocation of the shard (rows, tree, staging, moment scratch)
+  // observation normaliser of every gather (r2d2_replay_set_obs_normalizer): DEVICE [O] each, NULL = raw obs
+  const float* norm_mean = nullptr;
+  const float* norm_inv_std = nullptr;
+  float norm_clip = 0.f;
   std::vector<float*> level_alloc;
   TreeView tv;
   std::deque<Episode> episodes;
@@ -778,6 +916,7 @@ int replay_destroy(Replay* r) {
   if (r->host_states) cudaFreeHost(r->host_alloc);
   else cudaFree(r->state_rows);
   cudaFree(r->stage);
+  cudaFree(r->mom);
   for (float* p : r->level_alloc) cudaFree(p);
   delete r->group;
   delete r->import;
@@ -894,10 +1033,37 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
 // of all episodes arrive packed ([R, *] with R = sum of n_rows; recurrent states zero-padded to R rows, leaf
 // priorities already expanded to one value per row): contiguous runs in the ring are one copy per tensor, the sum tree
 // is refreshed once over the merged touched ranges, and there is one stream synchronisation per file.
+// The moments of ring rows [ring_row, ring_row + n) - packed rows [first, first + n) of the call - merged into the
+// call's block: kernels of the ingest moments above, reading the keep flags the caller staged in the scratch.
+struct MomentScratch {
+  unsigned long long* n_bad;
+  double *run, *part;
+  int* count;
+  unsigned char *keep, *valid;
+};
+
+static int run_moments(Replay* r, const MomentScratch& m, long long ring_row, long long first, long long n,
+                       double* acc, cudaStream_t stream) {
+  if (n <= 0) return R2D2_OK;
+  const int O = r->cfg.obs_size;
+  const float* obs = r->obs_rows + ring_row * O;
+  const int chunks = (int)((n + kMomChunk - 1) / kMomChunk);
+  obs_row_valid_kernel<<<grid_for(n * 32), 256, 0, stream>>>(obs, m.keep + first, n, O, m.valid, m.n_bad);
+  const dim3 grid((unsigned)chunks, (unsigned)ceil_div(O, 32)), block(32, 8);
+  obs_moment_partial_kernel<false><<<grid, block, 0, stream>>>(obs, m.valid, n, O, nullptr, m.part, m.count);
+  obs_moment_finish_kernel<false><<<1, 256, 0, stream>>>(m.part, m.count, chunks, O, m.run, acc);
+  obs_moment_partial_kernel<true><<<grid, block, 0, stream>>>(obs, m.valid, n, O, m.run + 1, m.part, m.count);
+  obs_moment_finish_kernel<true><<<1, 256, 0, stream>>>(m.part, m.count, chunks, O, m.run, acc);
+  count_launch(5);
+  R2D2_CUDA_TRY(cudaGetLastError());
+  return R2D2_OK;
+}
+
 int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int* n_starts, const float* obs,
                         const float* act, const float* rew, const float* term, const float* states,
                         const float* leaf_prio, long long* row_start_out, long long* n_evicted_out,
-                        long long* sequence_counter_out, cudaStream_t stream) {
+                        long long* sequence_counter_out, cudaStream_t stream, double* obs_moments,
+                        long long* n_nonfinite_out) {
   R2D2_REQUIRE(r && n_episodes >= 0 && (n_episodes == 0 || (n_rows && n_starts && obs && act && rew && term && states && leaf_prio)),
                "null");
   long long R = 0;
@@ -909,6 +1075,39 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
   }
   StateSource src{};
   if (n_episodes > 0) R2D2_TRY(stage_states(r, states, false, R, R, stream, &src));
+  // obs_moments: the keep flags of the call's rows (0 on each episode's last n_step rows, the actors' pad rows) are
+  // staged next to the moment scratch; the block starts empty and every ring run is merged into it after its copy
+  MomentScratch ms{};
+  std::vector<unsigned char> keep;
+  if (obs_moments) {
+    const int O = r->cfg.obs_size;
+    const long long chunks = (R + kMomChunk - 1) / kMomChunk;
+    auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+    const size_t o_run = 256, o_part = up(o_run + sizeof(double) * (1 + (size_t)O)),
+                 o_count = up(o_part + sizeof(double) * (size_t)chunks * O), o_keep = up(o_count + sizeof(int) * chunks),
+                 o_valid = up(o_keep + (size_t)R), need = up(o_valid + (size_t)R);
+    if (need > r->mom_bytes) {
+      R2D2_CUDA_TRY(cudaFree(r->mom));   // synchronises: no earlier call's moments still read the old block
+      r->mom = nullptr;
+      r->device_bytes -= r->mom_bytes;
+      r->mom_bytes = 0;
+      R2D2_CUDA_TRY(cudaMalloc(&r->mom, need));
+      r->mom_bytes = need;
+      r->device_bytes += need;
+    }
+    ms = {reinterpret_cast<unsigned long long*>(r->mom), reinterpret_cast<double*>(r->mom + o_run),
+          reinterpret_cast<double*>(r->mom + o_part), reinterpret_cast<int*>(r->mom + o_count),
+          reinterpret_cast<unsigned char*>(r->mom + o_keep), reinterpret_cast<unsigned char*>(r->mom + o_valid)};
+    keep.assign((size_t)R, 1);
+    long long off = 0;
+    for (int e = 0; e < n_episodes; ++e) {
+      for (int k = n_rows[e] - r->cfg.n_step; k < n_rows[e]; ++k) keep[(size_t)(off + k)] = 0;
+      off += n_rows[e];
+    }
+    R2D2_CUDA_TRY(cudaMemsetAsync(r->mom, 0, sizeof(unsigned long long), stream));
+    R2D2_CUDA_TRY(cudaMemsetAsync(obs_moments, 0, sizeof(double) * (1 + 2 * (size_t)O), stream));
+    if (R > 0) R2D2_CUDA_TRY(cudaMemcpyAsync(ms.keep, keep.data(), (size_t)R, cudaMemcpyHostToDevice, stream));
+  }
   const long long evicted0 = r->evicted_total;
   RangeList ranges;
   long long first = 0;                  // first packed row of the current run
@@ -916,6 +1115,8 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
   auto flush = [&]() -> int {
     if (run_rows == 0) return R2D2_OK;
     R2D2_TRY(write_rows(r, run_start, first, run_rows, obs, act, rew, term, src, run_rows, stream));
+    // a later run of the same call may overwrite these rows (a call wider than the ring): the moments are taken now
+    if (obs_moments) R2D2_TRY(run_moments(r, ms, run_start, first, run_rows, obs_moments, stream));
     R2D2_CUDA_TRY(cudaMemcpyAsync(r->tv.lvl[0] + run_start, leaf_prio + first, sizeof(float) * (size_t)run_rows,
                                   cudaMemcpyHostToDevice, stream));
     R2D2_TRY(raise_fresh_leaves(r, run_start, run_rows, stream));
@@ -937,7 +1138,10 @@ int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int*
     if (row_start_out) row_start_out[e] = start;
   }
   R2D2_TRY(flush());
+  unsigned long long n_bad = 0;
+  if (obs_moments) R2D2_CUDA_TRY(cudaMemcpyAsync(&n_bad, ms.n_bad, sizeof(n_bad), cudaMemcpyDeviceToHost, stream));
   R2D2_TRY(finish_ingest(r, ranges, stream));
+  if (n_nonfinite_out) *n_nonfinite_out = (long long)n_bad;
   if (n_evicted_out) *n_evicted_out = r->evicted_total - evicted0;
   if (sequence_counter_out) *sequence_counter_out = r->sequence_counter;
   return R2D2_OK;
@@ -949,6 +1153,7 @@ static GatherParams ring_gather_params(const Replay* r) {
   g.obs_rows = r->obs_rows; g.act_rows = r->act_rows; g.rew_rows = r->rew_rows; g.term_rows = r->term_rows;
   g.state_rows = r->state_rows;
   g.T = r->rows_per_window; g.O = r->cfg.obs_size; g.A = r->cfg.n_actions; g.H = r->cfg.hidden;
+  g.norm_mean = r->norm_mean; g.norm_inv_std = r->norm_inv_std; g.norm_clip = r->norm_clip;
   return g;
 }
 
@@ -956,12 +1161,30 @@ static GatherParams ring_gather_params(const Replay* r) {
 template <bool kPerDraw>
 static int launch_gather(const Replay* r, const GatherParams& g, long long tasks, cudaStream_t stream) {
   const int grid = grid_for(tasks * 32);
-  if (r->host_states && r->half_states) gather_host_states_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
+  if (r->norm_mean) {
+    if (r->host_states && r->half_states) gather_host_states_norm_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
+    else if (r->host_states) gather_host_states_norm_kernel<kPerDraw, false><<<grid, 256, 0, stream>>>(g);
+    else if (r->half_states) gather_batch_norm_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
+    else gather_batch_norm_kernel<kPerDraw, false><<<grid, 256, 0, stream>>>(g);
+  } else if (r->host_states && r->half_states) gather_host_states_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
   else if (r->host_states) gather_host_states_kernel<kPerDraw, false><<<grid, 256, 0, stream>>>(g);
   else if (r->half_states) gather_batch_kernel<kPerDraw, true><<<grid, 256, 0, stream>>>(g);
   else gather_batch_kernel<kPerDraw, false><<<grid, 256, 0, stream>>>(g);
   count_launch();
   R2D2_CUDA_TRY(cudaGetLastError());
+  return R2D2_OK;
+}
+
+int replay_set_obs_normalizer(Replay* r, const float* mean_f, const float* inv_std_f, float clip) {
+  R2D2_REQUIRE(r, "null");
+  R2D2_REQUIRE((mean_f == nullptr) == (inv_std_f == nullptr), "mean_f and inv_std_f are both given or both NULL");
+  R2D2_REQUIRE(!mean_f || (clip > 0.f && clip <= FLT_MAX), "clip must be finite and > 0");
+  R2D2_REQUIRE(!mean_f || (r->cfg.obs_size % 4 != 0 ||
+                           ((reinterpret_cast<uintptr_t>(mean_f) | reinterpret_cast<uintptr_t>(inv_std_f)) & 15) == 0),
+               "mean_f and inv_std_f must be 16-byte aligned when obs_size is a multiple of 4");
+  r->norm_mean = mean_f;
+  r->norm_inv_std = inv_std_f;
+  r->norm_clip = mean_f ? clip : 0.f;
   return R2D2_OK;
 }
 

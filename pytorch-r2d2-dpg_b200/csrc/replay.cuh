@@ -54,7 +54,9 @@ int replay_add_episode(Replay* r, const float* obs, const float* act, const floa
 int replay_add_episodes(Replay* r, int n_episodes, const int* n_rows, const int* n_starts, const float* obs,
                         const float* act, const float* rew, const float* term, const float* states,
                         const float* leaf_prio, long long* row_start_out, long long* n_evicted_out,
-                        long long* sequence_counter_out, cudaStream_t stream);
+                        long long* sequence_counter_out, cudaStream_t stream, double* obs_moments = nullptr,
+                        long long* n_nonfinite_out = nullptr);
+int replay_set_obs_normalizer(Replay* r, const float* mean_f, const float* inv_std_f, float clip);
 int replay_sample(Replay* r, const float* u, int batch, long long* leaf_idx, float* obs, float* act, float* rew,
                   float* term, float* states, cudaStream_t stream);
 int replay_sample_weighted(Replay* r, const float* u, int batch, float beta, long long* leaf_idx, float* is_weight,

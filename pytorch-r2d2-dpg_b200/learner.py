@@ -63,6 +63,16 @@ so that the run continues bit for bit as if it had not stopped, and the warm-up 
 shard holds enough sequences.  A snapshot written at another world size is refused (re-sharding is not supported).
 Without a complete snapshot the resume loads learner_state.pt alone and the replay starts empty, as before.  Actor files
 not yet ingested stay on disk and are ingested after the resume as usual.
+
+Observation normalisation (r2d2_b200.obs_norm): R2D2_OBS_NORM=0|1 (default 0) and R2D2_OBS_NORM_CLIP (default 5; finite
+and > 0, else it raises).  On, the learner keeps float64 running mean / variance statistics of every observation row it
+ingests (not the actors' n_step pad rows, nor rows holding NaN or +-inf), and every net reads
+clamp((obs - mean) / std, -clip, clip) in place of the raw observation: the replay gather writes it into the batch, and
+model.pt gains an `obs_norm` entry {mean_f, inv_std_f, clip} (next to its four reference keys, once a row was seen)
+from which the drop-in Actor and ActorPool normalise what they act on.  The replay and its snapshots keep raw rows.  The
+statistics change only right after the loop's ingests (and once before the first step), merged over the data-parallel
+ranks in rank order, so every rank holds the same bits.  The checkpoint records them; a resume across an on / off
+change, or across another clip, is refused.
 """
 import math
 import os
@@ -178,6 +188,8 @@ class Learner:
         from r2d2_b200 import td3_options, td_options
         self.td_options = td_options.from_environ()
         self.td3_options = td3_options.from_environ()
+        from r2d2_b200 import obs_norm
+        self.obs_norm, self.obs_norm_clip = obs_norm.from_environ()
         cfg = PathConfig(obs=self.obs_size, act=self.n_actions, hidden=self.hidden, batch=self.batch_size,
                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
                          gamma=self.gamma, actor_lr=self.actor_lr, critic_lr=self.critic_lr,
@@ -187,13 +199,15 @@ class Learner:
                          priority_metric=self.td_options.priority_metric, **self.td3_options,
                          global_sampling=self._global_sampling_from_environ(),
                          replay_state_dtype=self.replay_state_dtype,
-                         replay_state_memory="host" if self.replay_host_gb > 0 else "device")
+                         replay_state_memory="host" if self.replay_host_gb > 0 else "device",
+                         obs_norm=self.obs_norm, obs_norm_clip=self.obs_norm_clip)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
                                           obs_size=self.obs_size, n_actions=self.n_actions, hidden=self.hidden,
                                           device=self.engine.device, priority_exponent=self.priority_exponent,
                                           state_dtype=self.replay_state_dtype, host_gb=self.replay_host_gb)
+        self.memory.obs_norm = getattr(self.engine, "obs_norm", None)   # None unless R2D2_OBS_NORM=1
         self.state_path = self.model_path + 'learner_state.pt'
         self.snapshot_root = self.model_path + 'replay_snapshot/'
         if os.environ.get("R2D2_RESUME", "0") == "1":
@@ -297,6 +311,10 @@ class Learner:
         if not self.dist_env.is_main:
             return
         model_dict = {net: self._sd(net) for net in ('actor', 'target_actor', 'critic', 'target_critic')}
+        stats = getattr(self.engine, "obs_norm", None)
+        norm = stats.actor_key() if stats is not None else None
+        if norm is not None:
+            model_dict['obs_norm'] = norm
         tmp = self.model_path + 'model.pt.tmp{}'.format(os.getpid())
         torch.save(model_dict, tmp)
         os.replace(tmp, self.model_path + 'model.pt')
@@ -313,12 +331,13 @@ class Learner:
                 self.memory.load(i)
 
     def run(self, max_steps=None):
-        while self.memory.sequence_counter < self.batch_size * 100:   # warm-up gate, learner.py:69-75
-            self._ingest()
-            sleep(0.1)
+        from r2d2_b200.run_loop import run_learner_loop, warm_up
+
+        def report():
             if self.dist_env.is_main:
                 print('learner memory sequence size:', self.memory.sequence_counter)
-        from r2d2_b200.run_loop import run_learner_loop
+        warm_up(self._ingest, lambda: self.memory.sequence_counter >= self.batch_size * 100,   # learner.py:69-75
+                pause=lambda: sleep(0.1), report=report)
 
         def save():
             self.save_model()
@@ -344,6 +363,8 @@ class Learner:
         snap = {}
         if self.replay_snapshot_interval:
             snap = dict(snapshot=self.save_replay_snapshot, snapshot_every=self.replay_snapshot_interval)
+        if getattr(self.engine, "obs_norm", None) is not None:
+            snap["exchange"] = self.engine.obs_norm.exchange
         run_learner_loop(self.engine, self.memory._dev, max_steps=max_steps, ingest_every=self.memory_update_interval,
                          save_every=self.model_save_interval, ingest=ingest, save=save, log=log, **snap)
         torch.cuda.synchronize()

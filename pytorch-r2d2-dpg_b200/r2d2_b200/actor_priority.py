@@ -38,10 +38,11 @@ def nstep_rewards(raw_tb: torch.Tensor, n_rows: torch.Tensor, n_step: int, gamma
 
 def episode_priorities(critic, target_actor, target_critic, episodes, *, hidden, burn_in=20, learning=40, n_step=5,
                        gamma=0.997, eta=0.9, rewards_are_raw=False, device=None, rescaling="reference",
-                       eps=td_options.DEFAULT_EPS, priority_metric="squared"):
+                       eps=td_options.DEFAULT_EPS, priority_metric="squared", obs_norm=None):
     """episodes: list of (obs [N,O], act [N,A], rew [N], term [N]) host arrays, N = real rows + n_step pad rows
     (actor.py:173).  Weights: state_dicts (or dicts of arrays) with the reference's keys.  rescaling / eps /
-    priority_metric: r2d2_b200.td_options (the defaults are the reference's).  Returns
+    priority_metric: r2d2_b200.td_options (the defaults are the reference's).  obs_norm: model.pt's `obs_norm` entry
+    {mean_f, inv_std_f, clip} - the chains then read the normalised observations (r2d2_obs_normalize) - or None.  Returns
     (list of float32 arrays [N - n_step - burn_in - learning], list of n-step reward arrays [N])."""
     opts = td_options.TdOptions(rescaling, eps, priority_metric)
     if not torch.cuda.is_available():
@@ -64,6 +65,11 @@ def episode_priorities(critic, target_actor, target_critic, episodes, *, hidden,
         term[:n, b] = torch.as_tensor(np.asarray(d, np.float32).reshape(-1))
     obs, act, rew, term = (x.to(dev) for x in (obs, act, rew, term))
     n_rows = torch.tensor(lens, dtype=torch.int32, device=dev)
+    if obs_norm is not None:
+        mean_f = torch.as_tensor(obs_norm["mean_f"], dtype=torch.float32).to(dev).contiguous()
+        inv_std_f = torch.as_tensor(obs_norm["inv_std_f"], dtype=torch.float32).to(dev).contiguous()
+        nv.check(lib.r2d2_obs_normalize(nv.dptr(obs), nv.dptr(obs), T * B, O, nv.dptr(mean_f), nv.dptr(inv_std_f),
+                                        float(obs_norm["clip"]), nv.current_stream()))
     if rewards_are_raw:
         rew = nstep_rewards(rew, n_rows, n_step, gamma)
     st = nv.current_stream()

@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import native as nv
+from . import obs_norm as obs_norm_mod
 from . import td_options
 
 # PathConfig.replay_state_dtype -> r2d2_replay_options.state_storage
@@ -66,7 +67,13 @@ class PathConfig:
 
     `replay_state_memory` (replay shard): "device" (default) keeps those states in HBM; "host" keeps them in mapped,
     page-locked host memory while the rest of every row and the sum tree stay in HBM.  The gather then reads each drawn
-    sequence's start states over the host link; the batch is bit-identical to the device tier's."""
+    sequence's start states over the host link; the batch is bit-identical to the device tier's.
+
+    `obs_norm` (off by default, r2d2_b200.obs_norm): the engine keeps running float64 mean / variance statistics of the
+    ingested observation rows (DeviceReplay.add_episodes(obs_norm=...)), and every gather of an attached shard writes
+    x_hat = clamp((x - mean) / std, -c, c) into the batch, c = `obs_norm_clip` (> 0, default 5).  Actions, rewards,
+    terminals and stored states are not normalised; the replay keeps raw rows.  The statistics change only at
+    LearnerEngine.obs_norm.exchange(), which the training loop calls after its ingests (run_loop)."""
     obs: int
     act: int
     hidden: int = 128
@@ -93,6 +100,8 @@ class PathConfig:
     global_sampling: bool = False
     replay_state_dtype: str = "float32"
     replay_state_memory: str = "device"
+    obs_norm: bool = False
+    obs_norm_clip: float = obs_norm_mod.DEFAULT_CLIP
 
     def __post_init__(self):
         for name, least in (("burn_in", 0), ("learning", 2), ("n_step", 1)):
@@ -108,7 +117,8 @@ class PathConfig:
         if not isinstance(self.replay_state_memory, str) or self.replay_state_memory not in REPLAY_STATE_MEMORY:
             raise ValueError("replay_state_memory must be one of %s, got %r" % (", ".join(REPLAY_STATE_MEMORY),
                                                                                self.replay_state_memory))
-        for name in ("twin_critic", "global_sampling"):
+        obs_norm_mod.validate_clip(self.obs_norm_clip)
+        for name in ("twin_critic", "global_sampling", "obs_norm"):
             if not isinstance(getattr(self, name), bool):
                 raise ValueError("%s must be True or False, got %r" % (name, getattr(self, name)))
         for name, lo_ok in (("target_noise", lambda v: v >= 0.0), ("target_noise_clip", lambda v: v > 0.0)):
@@ -278,6 +288,8 @@ class LearnerEngine:
         # single rank; enable_data_parallel replaces it by symmetric memory); off, the slots stay in the library's arena
         self._global_buf = self._global_hdl = None
         self.global_peer_ptrs = None
+        # observation normalisation: the device statistics every attached replay shard's gathers read
+        self.obs_norm = obs_norm_mod.ObsNormStats(cfg.obs, cfg.obs_norm_clip, self.device) if cfg.obs_norm else None
         if cfg.global_sampling:
             lay = self.global_layout(1)
             self.use_global_slots(torch.zeros(int(lay.bytes) // 4, dtype=torch.float32, device=self.device), lay)
@@ -448,6 +460,8 @@ class LearnerEngine:
             self._sync = GradSync(dist, self.world)
             self._sync_actor = GradSync(dist, self.world)
             self._rank = dist.get_rank()             # the target noise is keyed on (seed, rank): ranks draw their own
+            if self.obs_norm is not None:
+                self.obs_norm.dist = dist
             if self.cfg.target_noise > 0:
                 self.set_target_smoothing()
             if self._dp_mode == "peer":
@@ -657,13 +671,26 @@ class LearnerEngine:
         c = self.cfg
         out.update(twin_critic=bool(c.twin_critic), target_noise=float(c.target_noise),
                    target_noise_clip=float(c.target_noise_clip), target_noise_seed=int(c.target_noise_seed))
+        if getattr(self, "obs_norm", None) is not None:
+            out["obs_norm"] = self.obs_norm.state()
         return out
 
     def load_training_state(self, st: dict):
         """Refuses a state saved under other target / priority options: a critic trained in one value space means nothing
         in the other.  A state without them was saved by a build that had only the reference's (reference, squared).
         Likewise a twin-critic state and a single-critic engine, or the other way round (a state without the key is
-        single-critic).  The target-noise settings of the state are informational: the engine keeps its own."""
+        single-critic).  The target-noise settings of the state are informational: the engine keeps its own.  Observation
+        normalisation on one side and off on the other is refused too, and so is another clip; otherwise the statistics
+        are restored."""
+        stats = getattr(self, "obs_norm", None)
+        saved_norm = bool((st.get("obs_norm") or {}).get("enabled", False))
+        if saved_norm != (stats is not None):
+            raise ValueError("training state was saved with obs_norm=%r; this engine runs obs_norm=%r: nets trained on "
+                             "normalised observations mean nothing on raw ones, and the other way round"
+                             % (saved_norm, stats is not None))
+        if stats is not None and np.float32(st["obs_norm"]["clip"]) != np.float32(stats.clip):
+            raise ValueError("training state was saved with obs_norm_clip=%r; this engine runs obs_norm_clip=%r: the nets "
+                             "were trained on differently clamped observations" % (st["obs_norm"]["clip"], stats.clip))
         saved_twin = bool(st.get("twin_critic", False))
         if saved_twin != bool(self.cfg.twin_critic):
             raise ValueError("training state was saved with twin_critic=%r; this engine runs twin_critic=%r"
@@ -688,6 +715,8 @@ class LearnerEngine:
                     for k, v in self.views(net, what).items():
                         v.copy_(torch.as_tensor(opt[what][k], dtype=torch.float32).to(self.device))
         nv.check(self.lib.r2d2_learner_set_step_count(self._h, int(st.get("step", 0))))
+        if stats is not None:
+            stats.load_state(st["obs_norm"])
 
     @property
     def launches_per_iteration(self) -> int:
@@ -712,6 +741,7 @@ class DeviceReplay:
         if cfg.priority_exponent != 1.0:   # leaves hold p^alpha; actors and write-backs keep passing raw priorities
             nv.check(self.lib.r2d2_replay_set_priority_exponent(self._h, float(cfg.priority_exponent)))
         self._group = None                 # the engine whose rank / world / buffers global sampling uses
+        self._obs_norm = None              # the ObsNormStats the gathers read (attach_obs_norm)
 
     def attach_group(self, eng: LearnerEngine):
         """Global sampling: this shard becomes rank eng's shard of the group of eng.world ranks; from then on
@@ -727,6 +757,18 @@ class DeviceReplay:
         arr = (c_void_p * eng.world)(*eng.global_peer_ptrs)
         nv.check(self.lib.r2d2_replay_attach_group(self._h, eng._rank, eng.world, ec.batch, arr, eng._global_bytes))
         self._group = eng
+
+    def attach_obs_norm(self, stats):
+        """Every gather of this shard (sample_into, the global draw, r2d2_replay_gather) normalises the batch's obs with
+        the fp32 pair of `stats` (an ObsNormStats, e.g. LearnerEngine.obs_norm), read at each gather; None detaches."""
+        if stats is None:
+            nv.check(self.lib.r2d2_replay_set_obs_normalizer(self._h, None, None, 0.0))
+        else:
+            if stats.O != self.cfg.obs:
+                raise nv.NativeError("obs normaliser of width %d for a shard of obs %d" % (stats.O, self.cfg.obs))
+            nv.check(self.lib.r2d2_replay_set_obs_normalizer(self._h, nv.dptr(stats.mean_f), nv.dptr(stats.inv_std_f),
+                                                             float(stats.clip)))
+        self._obs_norm = stats
 
     @property
     def group(self):
@@ -792,10 +834,11 @@ class DeviceReplay:
         nv.check(self.lib.r2d2_replay_add_episode(self._h, po, pa, pr, pt, ps, obs.shape[0], states.shape[0], pp,
                                                   priority.shape[0], nv.current_stream()))
 
-    def add_episodes(self, episodes):
+    def add_episodes(self, episodes, obs_norm=None):
         """One actor file in one native call (LearnerReplayMemory.load, replay_memory.py:138-157).  `episodes`: list of
         (obs [n,O], act [n,A], rew [n], term [n], states [n_real,4,2,H], priority [n_starts]) host arrays.  Returns
-        (row_start per episode, episodes evicted by the call, sequence counter)."""
+        (row_start per episode, episodes evicted by the call, sequence counter).  `obs_norm` (an ObsNormStats): the
+        call's observation moments (r2d2_replay_add_episodes_ex) are merged into its pending block."""
         if not episodes:
             return [], 0, None
         n_rows = np.asarray([e[0].shape[0] for e in episodes], np.int32)
@@ -821,9 +864,17 @@ class DeviceReplay:
         starts = np.zeros(len(episodes), np.int64)
         n_evicted, counter = c_longlong(0), c_longlong(0)
         P = lambda a: a.ctypes.data_as(c_void_p)  # noqa: E731
-        nv.check(self.lib.r2d2_replay_add_episodes(self._h, len(episodes), P(n_rows), P(n_starts), P(obs), P(act), P(rew),
-                                                   P(term), P(states), P(leaf), P(starts), byref(n_evicted), byref(counter),
-                                                   nv.current_stream()))
+        if obs_norm is None:
+            nv.check(self.lib.r2d2_replay_add_episodes(self._h, len(episodes), P(n_rows), P(n_starts), P(obs), P(act),
+                                                       P(rew), P(term), P(states), P(leaf), P(starts), byref(n_evicted),
+                                                       byref(counter), nv.current_stream()))
+        else:
+            bad = c_longlong(0)
+            nv.check(self.lib.r2d2_replay_add_episodes_ex(self._h, len(episodes), P(n_rows), P(n_starts), P(obs), P(act),
+                                                          P(rew), P(term), P(states), P(leaf), P(starts), byref(n_evicted),
+                                                          byref(counter), nv.dptr(obs_norm.ingest_block, torch.float64),
+                                                          byref(bad), nv.current_stream()))
+            obs_norm.add_ingest(int(bad.value))
         return starts.tolist(), int(n_evicted.value), int(counter.value)
 
     def sample_indices(self, u: torch.Tensor) -> torch.Tensor:

@@ -132,6 +132,10 @@ SIGNATURES = {
     "r2d2_policy_workspace_floats": (c_size_t, [POINTER(NetShape), c_int]),
     "r2d2_policy_step": (c_int, [POINTER(NetShape), POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                  c_void_p, c_void_p]),
+    "r2d2_policy_step_ex": (c_int, [POINTER(NetShape), POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                    c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
+    "r2d2_obs_norm_merge": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "r2d2_obs_normalize": (c_int, [c_void_p, c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_float, c_void_p]),
     "r2d2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_float, c_float, c_float,
                                c_float, c_float, c_void_p]),
     "r2d2_replay_create": (c_int, [POINTER(c_void_p), POINTER(ReplayConfig)]),
@@ -142,6 +146,10 @@ SIGNATURES = {
     "r2d2_replay_set_priority_exponent": (c_int, [c_void_p, c_float]),
     "r2d2_replay_add_episodes": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "r2d2_replay_add_episodes_ex": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p]),
+    "r2d2_replay_set_obs_normalizer": (c_int, [c_void_p, c_void_p, c_void_p, c_float]),
     "r2d2_replay_add_episode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                         c_void_p, c_int, c_void_p]),
     "r2d2_replay_sample": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

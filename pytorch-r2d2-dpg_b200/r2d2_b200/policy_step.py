@@ -20,9 +20,10 @@ from .actor_priority import _flat
 NETS = ("actor", "target_actor", "critic", "target_critic")   # the replay's state order (actor.py:149,166)
 
 
-def policy_step(params, obs, state_in, state_out, mu, workspace=None):
+def policy_step(params, obs, state_in, state_out, mu, workspace=None, obs_norm=None):
     """One step on CUDA tensors: params = 4 flat blocks (NETS order), obs [N,O], state_in / state_out [4,2,N,H],
-    mu [N,A] (written).  Launches on the current stream and does not synchronise."""
+    mu [N,A] (written).  obs_norm: (mean_f [O], inv_std_f [O] CUDA tensors, clip) - the nets read the normalised obs
+    (r2d2_policy_step_ex) - or None.  Launches on the current stream and does not synchronise."""
     N, O = obs.shape
     A, H = mu.shape[1], state_in.shape[3]
     lib = nv.lib()
@@ -30,8 +31,14 @@ def policy_step(params, obs, state_in, state_out, mu, workspace=None):
     if workspace is None:
         workspace = torch.empty(max(1, lib.r2d2_policy_workspace_floats(nv.byref(shape), N)), device=obs.device)
     ptrs = (c_void_p * 4)(*[nv.dptr(p).value for p in params])
-    nv.check(lib.r2d2_policy_step(nv.byref(shape), ptrs, nv.dptr(obs), nv.dptr(state_in), nv.dptr(state_out),
-                                  nv.dptr(mu), N, nv.dptr(workspace), nv.current_stream()))
+    if obs_norm is None:
+        nv.check(lib.r2d2_policy_step(nv.byref(shape), ptrs, nv.dptr(obs), nv.dptr(state_in), nv.dptr(state_out),
+                                      nv.dptr(mu), N, nv.dptr(workspace), nv.current_stream()))
+    else:
+        mean_f, inv_std_f, clip = obs_norm
+        nv.check(lib.r2d2_policy_step_ex(nv.byref(shape), ptrs, nv.dptr(obs), nv.dptr(state_in), nv.dptr(state_out),
+                                         nv.dptr(mu), N, nv.dptr(workspace), nv.dptr(mean_f), nv.dptr(inv_std_f),
+                                         float(clip), nv.current_stream()))
 
 
 class StateRing:
@@ -102,20 +109,26 @@ class PolicyStepper(StateRing):
         self.mu_host = torch.empty((n_lanes, n_actions), pin_memory=True)
         self.obs_dev = torch.empty((n_lanes, obs_size), device=dev)
         self.mu_dev = torch.empty((n_lanes, n_actions), device=dev)
+        self.obs_norm = None          # (mean_f, inv_std_f, clip) on the device from model.pt's `obs_norm`, or None
 
     def load(self, model_dict):
-        """model.pt dict {'actor', 'target_actor', 'critic', 'target_critic'} -> the four flat blocks (plain copies)."""
+        """model.pt dict {'actor', 'target_actor', 'critic', 'target_critic'} -> the four flat blocks (plain copies).
+        An `obs_norm` entry {mean_f, inv_std_f, clip} makes every later step read normalised obs; without it raw obs."""
         for p, name in zip(self.params, NETS):
             flat = _flat(model_dict[name], self.device)
             if flat.numel() != p.numel():
                 raise ValueError("%s: %d parameters, the stepper was built for %d" % (name, flat.numel(), p.numel()))
             p.copy_(flat)
+        n = model_dict.get("obs_norm")
+        self.obs_norm = None if n is None else (
+            torch.as_tensor(n["mean_f"], dtype=torch.float32).to(self.device).contiguous(),
+            torch.as_tensor(n["inv_std_f"], dtype=torch.float32).to(self.device).contiguous(), float(n["clip"]))
 
     def _step(self, obs, state_in, state_out):
         self.obs_host.numpy()[:] = obs
         with torch.cuda.device(self.device):
             self.obs_dev.copy_(self.obs_host, non_blocking=True)
-            policy_step(self.params, self.obs_dev, state_in, state_out, self.mu_dev, self.workspace)
+            policy_step(self.params, self.obs_dev, state_in, state_out, self.mu_dev, self.workspace, self.obs_norm)
             self.mu_host.copy_(self.mu_dev, non_blocking=True)
             torch.cuda.current_stream().synchronize()
         return self.mu_host.numpy().copy()

@@ -20,17 +20,39 @@ Replay snapshots (`snapshot`, every `snapshot_every` steps, a multiple of `inges
 ingest of their step.  That step ran sequentially, so no batch is prefetched and no write-back is pending: the shard,
 the nets and the RNG that draws the next batch are all at the same point.
 
+Observation normalisation (`exchange`, PathConfig.obs_norm): the statistics the gathers read change only at
+`exchange()`, a collective over the data-parallel ranks.  The loop calls it once before its first step and after every
+ingest (before that step's snapshot): every rank runs the same steps, so every rank makes the same number of calls, and
+since nothing is drawn ahead of an ingest, a pipelined, a sequential and a resumed run see the same statistics on every
+batch.  The warm-up ingests before the loop (`warm_up`) stay local: the warm-up gate is per rank and passes after a
+different number of ingests on each.
+
 No CUDA, no torch: `engine` needs step(prefetch=None) + leaf_idx / priority attributes, `replay` needs sample_into(engine)
 and update_priorities(leaf_idx, priority) - tests drive it with recording fakes (tests/test_cpu_host.py).
 """
 from __future__ import annotations
 
 
+def warm_up(ingest, ready, pause=None, report=None) -> int:
+    """The warm-up gate (learner.py:69-75): `ingest()` until `ready()`, with `pause()` and `report()` after each.  Makes
+    no collective call.  Returns the number of ingests."""
+    n = 0
+    while not ready():
+        ingest()
+        n += 1
+        if pause is not None:
+            pause()
+        if report is not None:
+            report()
+    return n
+
+
 def run_learner_loop(engine, replay, *, max_steps=None, ingest_every: int, save_every: int, ingest, save,
-                     log=None, log_every: int = 100, snapshot=None, snapshot_every: int = 0) -> int:
+                     log=None, log_every: int = 100, snapshot=None, snapshot_every: int = 0, exchange=None) -> int:
     """Returns the number of steps run.  `ingest()` / `save()` are called after the steps whose number is a multiple of
     `ingest_every` / `save_every` (learner.py:141-149), `log(step)` before every `log_every`-th step (learner.py:79-80),
-    and `snapshot()`, if given, after the ingest of every `snapshot_every`-th step."""
+    `snapshot()`, if given, after the ingest of every `snapshot_every`-th step, and `exchange()`, if given, before the
+    first step and right after every ingest."""
     if ingest_every < 1 or save_every < 1:
         raise ValueError("ingest_every and save_every must be >= 1")
     if snapshot is not None and (snapshot_every < 1 or snapshot_every % ingest_every):
@@ -43,6 +65,8 @@ def run_learner_loop(engine, replay, *, max_steps=None, ingest_every: int, save_
 
     step = 0
     have_batch = False
+    if exchange is not None:
+        exchange()
     while max_steps is None or step < max_steps:
         if log is not None and step % log_every == 0:
             log(step)
@@ -60,6 +84,8 @@ def run_learner_loop(engine, replay, *, max_steps=None, ingest_every: int, save_
             save()
         if step % ingest_every == 0:
             ingest()                                                # learner.py:144-149 without the sleep stall
+            if exchange is not None:
+                exchange()
             if snapshot is not None and step % snapshot_every == 0:
                 snapshot()
     return step

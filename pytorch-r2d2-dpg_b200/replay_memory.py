@@ -158,6 +158,7 @@ class LearnerReplayMemory:
         self._cfg()                                         # rejects an exponent outside [0, 1] before any ingest
         self._dev = None          # DeviceReplay, created when the row width is known
         self._episodes = deque()  # (row_start, n_rows, n_starts) in FIFO order, mirrors the native ring
+        self.obs_norm = None      # ObsNormStats (observation normalisation): ingests feed it, the shard's gathers read it
         self.priority = _PriorityTable(self)
         self.total_priority = _TotalPriority(self)
 
@@ -200,6 +201,8 @@ class LearnerReplayMemory:
             rows = self._capacity_rows or self._default_capacity_rows(obs_size, n_actions, hidden)
             self._dev = DeviceReplay(self._cfg(), capacity_rows=rows, max_sequences=self.memory_sequence_size,
                                      device=self._device)
+            if self.obs_norm is not None:
+                self._dev.attach_obs_norm(self.obs_norm)
         return self._dev
 
     def _default_capacity_rows(self, obs_size, n_actions, hidden):
@@ -282,7 +285,8 @@ class LearnerReplayMemory:
     def add_episode(self, rows, states, priority):
         obs, act, rew, term, st = pack_episode(rows, states, self._hidden)
         dev = self._ensure_device(obs.shape[1], act.shape[1], st.shape[3])
-        starts, n_evicted, counter = dev.add_episodes([(obs, act, rew, term, st, np.asarray(priority, np.float32))])
+        starts, n_evicted, counter = dev.add_episodes([(obs, act, rew, term, st, np.asarray(priority, np.float32))],
+                                                      obs_norm=self.obs_norm)
         self._register(starts, [obs.shape[0]], [len(priority)], n_evicted, counter)
 
     def get_weighted_sample_index(self):
@@ -353,6 +357,6 @@ class LearnerReplayMemory:
             episodes.append((obs, act, rew, term, st, np.asarray(prio, np.float32)))
         if episodes:
             dev = self._ensure_device(episodes[0][0].shape[1], episodes[0][1].shape[1], episodes[0][4].shape[3])
-            starts, n_evicted, counter = dev.add_episodes(episodes)
+            starts, n_evicted, counter = dev.add_episodes(episodes, obs_norm=self.obs_norm)
             self._register(starts, [e[0].shape[0] for e in episodes], [len(e[5]) for e in episodes], n_evicted, counter)
         os.remove(claimed)
