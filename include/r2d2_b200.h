@@ -528,7 +528,7 @@ int r2d2_learner_set_grad_clip(r2d2_learner_t* l, float max_norm);
 int r2d2_learner_set_value_rescaling(r2d2_learner_t* l, int mode, float eps);
 int r2d2_learner_set_priority_metric(r2d2_learner_t* l, int metric);
 /* DEVICE address of [critic N, actor N], the pre-clip norms of the last optimiser steps (written only while clipping
- * is on; 0 after create) */
+ * or metrics are on; 0 after create) */
 int r2d2_learner_grad_norms(r2d2_learner_t* l, float** out);
 int r2d2_learner_target_phase(r2d2_learner_t* l, int slot, r2d2_stream_t stream);
 /* forget a target phase that ran ahead: the caller is about to overwrite that slot's batch */
@@ -573,6 +573,46 @@ int r2d2_learner_peer_status(r2d2_learner_t* l, int* status, r2d2_stream_t strea
 int r2d2_learner_peer_counters(r2d2_learner_t* l, unsigned long long* out6, int reset, r2d2_stream_t stream);
 /* resume: completed iterations so far (drives Adam's bias correction and the target-update period, learner.py:82,131) */
 int r2d2_learner_set_step_count(r2d2_learner_t* l, int step);
+/* Learner metrics, off by default: one record of r2d2_metrics_field_count() doubles per learner iteration, reduced on
+ * the device in the learner's stream - no host synchronisation - into a caller-owned device ring of `slots` records.
+ * Iteration i (the step count at its critic phase, so a resumed run continues the numbering) writes record i % slots.
+ * Fields, in order (r2d2_metrics_field_name(k) gives each name):
+ *    0 iteration         i: marks which iteration owns the slot
+ *    1 t_ns              %globaltimer when the critic phase's metrics kernel runs (differences: the iteration period;
+ *                        held in a double, so in steps of 256 ns at today's epoch times)
+ *    2 critic_loss       losses[0]
+ *    3 critic2_loss      losses[2] with the twin critic, else NaN
+ *    4 actor_loss        losses[1]
+ *    5-7 q_mean, q_min, q_max                  over critic 1's q [L,B,A]
+ *    8-10 target_mean, target_min, target_max  over the TD target y [L,B,A]
+ *    11-12 td_abs_mean, td_abs_max             |q - y| formed in double
+ *    13-14 priority_mean, priority_max         the raw priorities written back [B]
+ *    15-16 is_weight_min, is_weight_mean       the importance weights [B]; both 1 with importance weighting off
+ *    17 q2_mean          critic 2's q with the twin critic, else NaN
+ *    18 mu_abs_mean      mean |mu| over the actor head's output [L,B,A]
+ *    19 mu_saturated     the fraction of mu with |mu| >= 0.99
+ *    20 critic_grad_norm the pre-clip L2 norm of the gradient the critic's Adam consumed (grad_scale applied: the rank
+ *                        mean in data-parallel runs), as r2d2_learner_grad_norms; twin: joint over both critics
+ *    21 actor_grad_norm  the same for the actor.  It exists only after the finish phase, which in data-parallel runs
+ *                        follows the next critic phase: the device record holds NaN, and the finish phase copies the
+ *                        float norm into float k of the side array behind the records (k = the iteration's slot)
+ *    22 nonfinite        count of NaN / +-inf in q, y, q2 and mu
+ * Means are sums in double over the element count; min / max skip NaN (they are counted in nonfinite).  Fields 0-3, 5-17
+ * and 22 are written at the end of the critic phase, 4 and 18-20 (and 22's mu count) in the actor phase.  Sums are
+ * added in a fixed order and no floating-point atomic is used: two seeded runs write the same bits.  A record is
+ * complete once its iteration's finish phase has run.
+ *
+ * Switching metrics on adds per iteration one kernel to the critic phase and one to the actor phase, and - without
+ * gradient-norm clipping - the norm kernel before each Adam (r2d2_learner_grad_norms is then written too): 4 launches,
+ * 2 with clipping on.  Training is unchanged bit for bit; off (the default) issues none of it.
+ *
+ * ring: r2d2_metrics_ring_bytes(slots) bytes of device memory, 8-byte aligned - slots * fields doubles of records
+ * followed by slots floats of actor norms - or NULL to switch metrics off.  slots >= 1, else R2D2_ERR_ARG.  Only before
+ * the learner's first critic phase, else R2D2_ERR_STATE. */
+size_t r2d2_metrics_ring_bytes(int slots);
+int r2d2_metrics_field_count(void);
+const char* r2d2_metrics_field_name(int field);   /* NULL outside [0, r2d2_metrics_field_count()) */
+int r2d2_learner_set_metrics(r2d2_learner_t* l, void* ring, int slots);
 /* number of kernels launched by the three phases of one iteration (bench.py's gpu_launches) */
 int r2d2_learner_launches_per_iteration(r2d2_learner_t* l);
 

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from models import ActorNet, CriticNet
+from r2d2_b200 import metrics
 from r2d2_b200 import obs_norm as obs_norm_mod
 from r2d2_b200 import td_options
 from replay_memory import ReplayMemory
@@ -91,6 +92,8 @@ class Actor:
         self.critic = CriticNet(self.obs_size, self.action_size, 0, hidden=self.hidden).to(self.device).eval()
         self.target_critic = deepcopy(self.critic)
         self.obs_norm = None      # model.pt's `obs_norm` {mean_f, inv_std_f, clip} when the learner normalises obs
+        # R2D2_METRICS=1: one row per finished episode (r2d2_b200.metrics.EPISODE_COLUMNS)
+        self.episode_log = metrics.episode_csv("actor", actor_id) if metrics.from_environ() else None
         self.load_model()
 
     def _nets(self):
@@ -187,6 +190,10 @@ class Actor:
                     self.load_model()
             if self.actor_id == 0:
                 print('episode:', episode, 'step:', step, 'reward:', reward_sum)
+            if self.episode_log is not None:
+                metrics.append_csv(self.episode_log, metrics.EPISODE_COLUMNS,
+                                   [(self.actor_id, episode, step, len(self.sequence), reward_sum,
+                                     len(self.sequence) >= self.sequence_length)])
             if len(self.sequence) >= self.sequence_length:
                 pad = (np.zeros(self.obs_size, np.float32), np.zeros(self.action_size, np.float32), [0.0], [1.0])
                 self.sequence.extend([(pad[0].copy(), pad[1].copy(), [0.0], [1.0]) for _ in range(self.n_step)])

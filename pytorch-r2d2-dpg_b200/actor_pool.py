@@ -10,7 +10,9 @@ lane steps its own environment on the host.  Lane by lane it does what `Actor.ru
     step), with the target / priority options of the environment (r2d2_b200.td_options, as the learner reads them);
   * each lane has its own ReplayMemory, saved to memory{actor_id}.pt once it holds more than 3 episodes (same file
     format and atomic rename);
-  * model.pt is reloaded every 500 pool steps; lane 0 prints its episode reward.
+  * model.pt is reloaded every 500 pool steps; lane 0 prints its episode reward;
+  * with R2D2_METRICS=1 every lane's finished episodes are appended to ./model_data/metrics/episodes_pool{first actor
+    id}.csv (r2d2_b200.metrics: actor id, episode, pool step, length, return, kept).
 
 Differences from separate Actor processes:
   * the lanes step in lock-step: a lane whose episode ends starts the next one on the next pool step;
@@ -107,6 +109,8 @@ class ActorPool:
         self.device = stepper.device
         from r2d2_b200 import td_options
         self.td_options = td_options.from_environ()
+        from r2d2_b200 import metrics
+        self.episode_log = metrics.episode_csv("pool", self.actor_ids[0]) if metrics.from_environ() else None
         self.priority_fn = priority_fn or self._gpu_priorities
         self.model_dict = initial_model_dict(self.obs_size, self.action_size, self.hidden)
         self.stepper.load(self.model_dict)
@@ -185,11 +189,13 @@ class ActorPool:
             self._finish_episodes(finished)
 
     def _finish_episodes(self, lanes):
-        kept = []
+        kept, log = [], []
         for lane in lanes:
             seq = self.sequence[lane]
             if lane == 0:
                 print('episode:', self.episode[0], 'step:', self.steps, 'reward:', self.reward_sum[0])
+            log.append((self.actor_ids[lane], self.episode[lane], self.steps, len(seq), self.reward_sum[lane],
+                        len(seq) >= self.sequence_length))
             if len(seq) < self.sequence_length:
                 continue
             start = int(self.stepper.start[lane])
@@ -206,6 +212,9 @@ class ActorPool:
                 rows = [(o, a, [float(rew[i])], d) for i, (o, a, _, d) in enumerate(seq)]
                 recurrent = [[[st[k, 0], st[k, 1]] for k in range(4)] for st in states]
                 self.memories[lane].add(rows, recurrent, list(prio))
+        if self.episode_log is not None:
+            from r2d2_b200 import metrics
+            metrics.append_csv(self.episode_log, metrics.EPISODE_COLUMNS, log)
         for lane in lanes:
             if len(self.memories[lane].memory) > self.memory_save_interval:
                 self.memories[lane].save(self.actor_ids[lane])

@@ -551,6 +551,14 @@ int r2d2_learner_set_step_count(r2d2_learner_t* l, int step) {
   reinterpret_cast<Learner*>(l)->critic_iters = step;   // the target noise's iteration index resumes with it
   return R2D2_OK;
 }
+size_t r2d2_metrics_ring_bytes(int slots) {
+  return slots >= 1 ? (size_t)slots * (kMetricsFields * sizeof(double) + sizeof(float)) : 0;
+}
+int r2d2_metrics_field_count(void) { return kMetricsFields; }
+const char* r2d2_metrics_field_name(int i) { return metrics_field_name(i); }
+int r2d2_learner_set_metrics(r2d2_learner_t* l, void* ring, int slots) {
+  return learner_set_metrics(reinterpret_cast<Learner*>(l), ring, slots);
+}
 int r2d2_learner_launches_per_iteration(r2d2_learner_t* lh) {
   if (!lh) return -1;
   Learner* l = reinterpret_cast<Learner*>(lh);

@@ -18,6 +18,10 @@
 // TD against the same y and its own BPTT into the second half of the critic gradient block.  Critic 1 keeps every other
 // role: the DPG loss of phase 2, the priorities, td_sq and the target written out.
 //
+// Learner metrics (off by default, metrics.cuh): with a ring set, one reduction kernel at the end of phase 1 and one after
+// the actor loss in phase 2 write the iteration's record, the norm kernel runs before each Adam even without clipping, and
+// phase 3 copies the actor's norm into the ring.  Off, none of it is issued.
+//
 // The actor burn-in of learner.py:92 is skipped: its state is discarded at learner.py:117 before any use.
 #include "learner.cuh"
 
@@ -132,6 +136,7 @@ int learner_destroy(Learner* l) {
   if (l->ev_c1_inputs) cudaEventDestroy(l->ev_c1_inputs);
   if (l->ev_a1_inputs) cudaEventDestroy(l->ev_a1_inputs);
   cudaFree(l->arena);
+  cudaFree(l->metrics_part);
   delete l->peer;
   delete l;
   return R2D2_OK;
@@ -276,8 +281,17 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
     R2D2_TRY(net_backward(l->critic_sh, Pc2, &Gc2, l->ws_c1_2, l->obs, l->act, l->dq2, Bn, Tc, B, 1, nullptr, nullptr,
                           st));
   }
-  l->critic_iters += 1;
   if (l->peer) R2D2_TRY(peer_signal(*l->peer, kPeerCritic, st));
+  l->critic_phase_ran = true;
+  l->metrics_iter = l->critic_iters;
+  if (l->metrics_ring) {
+    MetricsCriticParams mp;
+    mp.q = l->q; mp.target = l->target; mp.q2 = l->twin ? l->q2 : nullptr; mp.priority = l->priority;
+    mp.is_weight = l->importance_weighting ? l->is_weight : nullptr; mp.losses = l->losses;
+    mp.n = (long long)L * B * A; mp.B = B; mp.iter = l->metrics_iter; mp.rec = l->metrics_record(l->metrics_iter);
+    R2D2_TRY(metrics_critic(mp, l->metrics_part, l->metrics_ticket, st));
+  }
+  l->critic_iters += 1;
   l->launches_phase[0] = (int)(launch_count() - launches0);
   return R2D2_OK;
 }
@@ -315,16 +329,17 @@ static bool updates_targets(const Learner* l) {
 }
 
 // Adam of one net (learner.py:114,128) on the gradient block the optimiser reads - in data-parallel runs the rank sum
-// that peer_wait just completed - preceded by the norm kernel when clipping is on.  On an update iteration with
+// that peer_wait just completed - preceded by the norm kernel when clipping is on, or when metrics are on (the norm
+// alone: Adam keeps coef = nullptr, so its instantiation and bits do not change).  On an update iteration with
 // target_tau < 1 the net's target is blended in the same pass; target_tau = 1 keeps the finish phase's hard copy.
 static int optimiser_step(Learner* l, int block, float* params, float* exp_avg, float* exp_avg_sq, float* target,
                           long long n, float lr, float grad_scale, cudaStream_t st) {
   const float* grads = l->optimiser_grads(block);
   const float* coef = nullptr;
-  if (l->grad_clip > 0.0f) {
+  if (l->grad_clip > 0.0f || l->metrics_ring) {
     R2D2_TRY(grad_norm(grads, n, grad_scale, l->grad_clip, l->norm_part + (size_t)block * kGradNormBlocks,
                        l->norm_ticket + block, l->optim + block, l->optim + 2 + block, st));
-    coef = l->optim + 2 + block;
+    if (l->grad_clip > 0.0f) coef = l->optim + 2 + block;
   }
   const bool polyak = l->target_tau < 1.0f && updates_targets(l);
   return adam_step(params, grads, exp_avg, exp_avg_sq, n, l->step + 1, lr, 0.9f, 0.999f, 1e-8f, grad_scale, st, coef,
@@ -370,6 +385,12 @@ int learner_actor_phase(Learner* l, float grad_scale, cudaStream_t st) {
   R2D2_TRY(net_forward(l->critic_sh, Pc, l->ws_c2, obs_l, l->mu, nullptr, nullptr, L, B, 1, st));
   R2D2_TRY(net_head_forward(l->critic_sh, Pc, l->ws_c2, 0, L, B, 1, l->q_pi, A, st));
   R2D2_TRY(scaled_sum(l->q_pi, LBA, -1.0f / (float)LBA, l->losses + 1, st));
+  if (l->metrics_ring) {   // the critic's norm of this iteration's optimiser step exists by now
+    MetricsActorParams mp;
+    mp.mu = l->mu; mp.losses = l->losses; mp.critic_norm = l->optim + kPeerCritic; mp.n = LBA;
+    mp.rec = l->metrics_record(l->metrics_iter);
+    R2D2_TRY(metrics_actor(mp, l->metrics_part, l->metrics_ticket, st));
+  }
   R2D2_TRY(fill_f32(l->dq_pi, LBA, -1.0f / (float)LBA, st));
   // dgrad only through the critic (its weight grads are wasted work in the reference); d_pre(actor) = dQ/da * (1-mu^2)
   R2D2_TRY(net_backward(l->critic_sh, Pc, nullptr, l->ws_c2, obs_l, l->mu, l->dq_pi, 0, L, B, 1, l->dpre_actor,
@@ -387,6 +408,11 @@ int learner_finish_phase(Learner* l, float grad_scale, cudaStream_t st) {
   if (l->peer) R2D2_TRY(peer_wait(*l->peer, kPeerActor, st));   // runs the slice reduction first if no critic phase did
   R2D2_TRY(optimiser_step(l, kPeerActor, c.actor_params, c.actor_exp_avg, c.actor_exp_avg_sq, c.target_actor_params,
                           (long long)l->actor_sh.param_count(), c.actor_lr, grad_scale, st));     // learner.py:128
+  // the actor's norm of iteration `step` (which may already be behind the next critic phase): a copy into the ring's
+  // side array, no kernel - the host widens it when it reads the record
+  if (l->metrics_ring)
+    R2D2_CUDA_TRY(cudaMemcpyAsync(l->metrics_actor_norms() + l->step % l->metrics_slots, l->optim + kPeerActor,
+                                  sizeof(float), cudaMemcpyDeviceToDevice, st));
   l->step += 1;
   if (l->target_tau == 1.0f && c.target_update_interval > 0 && l->step % c.target_update_interval == 0) {  // :131-132
     R2D2_CUDA_TRY(cudaMemcpyAsync(c.target_actor_params, c.actor_params, sizeof(float) * l->actor_sh.param_count(),
@@ -395,6 +421,26 @@ int learner_finish_phase(Learner* l, float grad_scale, cudaStream_t st) {
                                   cudaMemcpyDeviceToDevice, st));
   }
   l->launches_phase[2] = (int)(launch_count() - launches0);
+  return R2D2_OK;
+}
+
+int learner_set_metrics(Learner* l, void* ring, int slots) {
+  R2D2_REQUIRE(l, "null");
+  R2D2_REQUIRE(!ring || slots >= 1, "slots >= 1");
+  R2D2_REQUIRE(((uintptr_t)ring & 7) == 0, "the ring holds doubles: 8-byte aligned");
+  if (l->critic_phase_ran) {
+    set_last_error("metrics are switched on or off before the first critic phase");
+    return R2D2_ERR_STATE;
+  }
+  if (ring && !l->metrics_part) {
+    const size_t n = (size_t)kMetricsBlocks * kMetricsPartials;
+    R2D2_CUDA_TRY(cudaMalloc(&l->metrics_part, n * sizeof(double) + 64));
+    R2D2_CUDA_TRY(cudaMemset(l->metrics_part, 0, n * sizeof(double) + 64));
+    R2D2_CUDA_TRY(cudaDeviceSynchronize());   // the ticket is zero before any stream's first metrics kernel
+    l->metrics_ticket = reinterpret_cast<unsigned int*>(l->metrics_part + n);
+  }
+  l->metrics_ring = static_cast<double*>(ring);
+  l->metrics_slots = ring ? slots : 0;
   return R2D2_OK;
 }
 

@@ -1,6 +1,7 @@
 #pragma once
 #include "common.cuh"
 #include "elementwise.cuh"
+#include "metrics.cuh"
 #include "net.cuh"
 #include "peer.cuh"
 
@@ -81,6 +82,20 @@ struct Learner {
   // data-parallel learner: gradient blocks live in a peer-mapped buffer and are summed by peer.cu's kernels in this
   // learner's own stream (null: single GPU, or the caller reduces cfg.*_grads itself between the phases)
   PeerExchange* peer = nullptr;
+  // learner metrics (metrics.cuh), off while metrics_ring is null: the caller's ring of metrics_slots records of
+  // kMetricsFields doubles followed by metrics_slots floats of actor gradient norms (r2d2_learner_set_metrics).  The
+  // kernels' partials and ticket live in metrics_part, the learner's own allocation made by the first set call, so that
+  // the arena and every offset in it stay as they are.  metrics_iter: the iteration of the last critic phase.
+  double* metrics_ring = nullptr;
+  int metrics_slots = 0;
+  double* metrics_part = nullptr;
+  unsigned int* metrics_ticket = nullptr;
+  long long metrics_iter = 0;
+  bool critic_phase_ran = false;
+  double* metrics_record(long long iter) const { return metrics_ring + (size_t)(iter % metrics_slots) * kMetricsFields; }
+  float* metrics_actor_norms() const {
+    return reinterpret_cast<float*>(metrics_ring + (size_t)metrics_slots * kMetricsFields);
+  }
   const float* optimiser_grads(int block) const {
     return peer ? peer->sums(block) : (block == kPeerCritic ? cfg.critic_grads : cfg.actor_grads);
   }
@@ -101,5 +116,7 @@ int learner_finish_phase(Learner* l, float grad_scale, cudaStream_t stream);
 // peer_bases[k] = rank k's exchange buffer (peer_layout(...).bytes, zeroed, mapped into this process); moves the
 // learner's gradient blocks into peer_bases[rank]
 int learner_attach_peers(Learner* l, int rank, int world, void* const* peer_bases);
+// ring: r2d2_metrics_ring_bytes(slots) of device memory (8-byte aligned), or null for off; before the first critic phase
+int learner_set_metrics(Learner* l, void* ring, int slots);
 
 }  // namespace r2d2

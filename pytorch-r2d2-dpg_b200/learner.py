@@ -73,6 +73,14 @@ from which the drop-in Actor and ActorPool normalise what they act on.  The repl
 statistics change only right after the loop's ingests (and once before the first step), merged over the data-parallel
 ranks in rank order, so every rank holds the same bits.  The checkpoint records them; a resume across an on / off
 change, or across another clip, is refused.
+
+Learner metrics (r2d2_b200.metrics): R2D2_METRICS=0|1 (default 0; any other value raises).  On, the library reduces one
+record per iteration on the device (losses, Q / target / |TD error| / priority / importance-weight statistics, actor
+saturation, both gradient norms, non-finite count; include/r2d2_b200.h), and at every log point (every 100 steps) and
+when run() returns each rank appends the iterations finished since its last read to
+./model_data/metrics/learner_rank{r}.csv (a header row when the file is new, then one row per iteration); rank 0 prints
+one summary line of the interval's means after `learning step: N`.  No collective is added: each rank logs its own
+batch, and the gradient norms, taken of the rank mean, are the same on every rank.  Training is bit-identical either way.
 """
 import math
 import os
@@ -190,6 +198,9 @@ class Learner:
         self.td3_options = td3_options.from_environ()
         from r2d2_b200 import obs_norm
         self.obs_norm, self.obs_norm_clip = obs_norm.from_environ()
+        from r2d2_b200 import metrics
+        self.metrics_on = metrics.from_environ()
+        self.metrics_path = self.model_path + 'metrics/learner_rank{}.csv'.format(self.dist_env.rank)
         cfg = PathConfig(obs=self.obs_size, act=self.n_actions, hidden=self.hidden, batch=self.batch_size,
                          burn_in=self.burn_in_length, learning=self.learning_length, n_step=self.n_step,
                          gamma=self.gamma, actor_lr=self.actor_lr, critic_lr=self.critic_lr,
@@ -200,7 +211,7 @@ class Learner:
                          global_sampling=self._global_sampling_from_environ(),
                          replay_state_dtype=self.replay_state_dtype,
                          replay_state_memory="host" if self.replay_host_gb > 0 else "device",
-                         obs_norm=self.obs_norm, obs_norm_clip=self.obs_norm_clip)
+                         obs_norm=self.obs_norm, obs_norm_clip=self.obs_norm_clip, metrics=self.metrics_on)
         self.engine = LearnerEngine(cfg, device=device)
         self.engine.enable_data_parallel()
         self.memory = LearnerReplayMemory(memory_sequence_size=self.memory_sequence_size, batch_size=self.batch_size,
@@ -325,6 +336,20 @@ class Learner:
         self.engine.flat['target_actor'].copy_(self.engine.flat['actor'])
         self.engine.flat['target_critic'].copy_(self.engine.flat['critic'])   # twin critic: the whole [1 | 2] block
 
+    def log_metrics(self):
+        """With R2D2_METRICS=1: append the iterations finished since the last call to this rank's CSV file; rank 0
+        prints their summary.  A deferred data-parallel finish phase is not forced: its iteration comes next time."""
+        m = getattr(self.engine, "metrics", None)
+        if m is None:
+            return
+        from r2d2_b200 import metrics
+        rec = m.read()
+        if not len(rec["iteration"]):
+            return
+        metrics.append_records(self.metrics_path, rec)
+        if self.dist_env.is_main:
+            print(metrics.summary_line(rec))
+
     def _ingest(self):
         for i in self.dist_env.owned_actors(self.n_actors):   # all of them in a single-process run (learner.py:70-73)
             if os.path.isfile(self.memory_path + '/memory{}.pt'.format(i)):
@@ -347,6 +372,7 @@ class Learner:
         def log(step):
             if self.dist_env.is_main:
                 print('learning step:', step)
+            self.log_metrics()
 
         ingest = self._ingest
         if self.engine.cfg.global_sampling:
@@ -367,4 +393,5 @@ class Learner:
             snap["exchange"] = self.engine.obs_norm.exchange
         run_learner_loop(self.engine, self.memory._dev, max_steps=max_steps, ingest_every=self.memory_update_interval,
                          save_every=self.model_save_interval, ingest=ingest, save=save, log=log, **snap)
+        self.log_metrics()
         torch.cuda.synchronize()

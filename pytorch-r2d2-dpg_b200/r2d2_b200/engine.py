@@ -19,6 +19,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
+from . import metrics as metrics_mod
 from . import native as nv
 from . import obs_norm as obs_norm_mod
 from . import td_options
@@ -73,7 +74,10 @@ class PathConfig:
     ingested observation rows (DeviceReplay.add_episodes(obs_norm=...)), and every gather of an attached shard writes
     x_hat = clamp((x - mean) / std, -c, c) into the batch, c = `obs_norm_clip` (> 0, default 5).  Actions, rewards,
     terminals and stored states are not normalised; the replay keeps raw rows.  The statistics change only at
-    LearnerEngine.obs_norm.exchange(), which the training loop calls after its ingests (run_loop)."""
+    LearnerEngine.obs_norm.exchange(), which the training loop calls after its ingests (run_loop).
+
+    `metrics` (off by default, r2d2_b200.metrics): the library reduces one record of training statistics per iteration
+    on the device into a ring that LearnerEngine.metrics.read() returns; training itself is bit-identical either way."""
     obs: int
     act: int
     hidden: int = 128
@@ -102,6 +106,7 @@ class PathConfig:
     replay_state_memory: str = "device"
     obs_norm: bool = False
     obs_norm_clip: float = obs_norm_mod.DEFAULT_CLIP
+    metrics: bool = False
 
     def __post_init__(self):
         for name, least in (("burn_in", 0), ("learning", 2), ("n_step", 1)):
@@ -118,7 +123,7 @@ class PathConfig:
             raise ValueError("replay_state_memory must be one of %s, got %r" % (", ".join(REPLAY_STATE_MEMORY),
                                                                                self.replay_state_memory))
         obs_norm_mod.validate_clip(self.obs_norm_clip)
-        for name in ("twin_critic", "global_sampling", "obs_norm"):
+        for name in ("twin_critic", "global_sampling", "obs_norm", "metrics"):
             if not isinstance(getattr(self, name), bool):
                 raise ValueError("%s must be True or False, got %r" % (name, getattr(self, name)))
         for name, lo_ok in (("target_noise", lambda v: v >= 0.0), ("target_noise_clip", lambda v: v > 0.0)):
@@ -278,6 +283,8 @@ class LearnerEngine:
         self.twin_added_bytes = int(tb.value)
         if cfg.target_noise > 0:
             self.set_target_smoothing()
+        # learner metrics: the ring the library's metrics kernels write and its reader (None when off)
+        self.metrics = metrics_mod.LearnerMetrics.attach(self) if cfg.metrics else None
         self.world = 1
         self._dist = None
         self._sync = None
@@ -715,6 +722,8 @@ class LearnerEngine:
                     for k, v in self.views(net, what).items():
                         v.copy_(torch.as_tensor(opt[what][k], dtype=torch.float32).to(self.device))
         nv.check(self.lib.r2d2_learner_set_step_count(self._h, int(st.get("step", 0))))
+        if getattr(self, "metrics", None) is not None:
+            self.metrics.next = int(st.get("step", 0))    # the ring's numbering continues from the resumed step
         if stats is not None:
             stats.load_state(st["obs_norm"])
 

@@ -208,6 +208,10 @@ SIGNATURES = {
     "r2d2_learner_peer_counters": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     "r2d2_learner_peer_status": (c_int, [c_void_p, POINTER(c_int), c_void_p]),
     "r2d2_learner_launches_per_iteration": (c_int, [c_void_p]),
+    "r2d2_metrics_ring_bytes": (c_size_t, [c_int]),
+    "r2d2_metrics_field_count": (c_int, []),
+    "r2d2_metrics_field_name": (c_char_p, [c_int]),
+    "r2d2_learner_set_metrics": (c_int, [c_void_p, c_void_p, c_int]),
 }
 
 _lib = None
