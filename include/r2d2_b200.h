@@ -189,6 +189,40 @@ int r2d2_policy_step_ex(const r2d2_net_shape* shape, const float* const params[4
                         const float* state_in, float* state_out, float* mu, int N, float* workspace,
                         const float* obs_mean, const float* obs_inv_std, float clip, r2d2_stream_t stream);
 
+/* Actor exploration noise drawn in the step (off unless a caller asks for it; the reference adds N(0, 0.3) on the host).
+ * For lane n and action a, z comes from the generator of r2d2_target_smoothing with key = (seed, actor_id[n]) and
+ * counter = (a >> 2, (uint32) step, step >> 32, 1) - words (x0, x1) serve a % 4 in {0, 1}, (x2, x3) serve {2, 3}, the
+ * same Box-Muller - so c3 = 1 keeps these streams apart from target smoothing's (c3 = 0), and lane n's noise depends
+ * on its actor id and the step only, never on N or on the lane's position.  In fp32, in this order:
+ *   R2D2_EXPLORATION_GAUSSIAN: noise = fl(sigma[n] z)
+ *   R2D2_EXPLORATION_OU:       x' = fl(fl(one_minus_theta x) + fl(sigma[n] z)), written back to x = ou_state[n, a];
+ *                              noise = x'
+ *   action[n, a] = min(max(fl(mu[n, a] + noise), -1), 1)
+ * mu stays the noise-free actor output, and the critics read it. */
+#define R2D2_EXPLORATION_GAUSSIAN 0
+#define R2D2_EXPLORATION_OU 1
+typedef struct {
+  int kind;                    /* R2D2_EXPLORATION_GAUSSIAN or R2D2_EXPLORATION_OU; anything else is R2D2_ERR_ARG */
+  unsigned int seed;           /* first key word of every lane's stream */
+  unsigned long long step;     /* the actors' 0-based env-step count: the counter's words 1 and 2 */
+  float one_minus_theta;       /* OU: fl32(1 - theta), theta in (0, 1] so in [0, 1); ignored for GAUSSIAN */
+  const unsigned int* actor_id;  /* DEVICE [N]: the second key word of lane n */
+  const float* sigma;          /* DEVICE [N]: lane n's noise scale, finite and >= 0 */
+  float* ou_state;             /* DEVICE [N, A], read and written: OU's x (zero it at a lane's episode start); NULL for
+                                  GAUSSIAN */
+} r2d2_exploration;
+/* r2d2_policy_step_ex (obs_mean NULL: the raw-obs path) that also writes action [N, A] (DEVICE; must not overlap mu)
+ * as defined above, from the actor head's registers; mu, the target actor's mu_t, the critics' inputs and every state
+ * are bitwise those of r2d2_policy_step_ex.  Same five launches: the head phase is a separate kernel.  Before any
+ * launch the call copies sigma [N] to the host and synchronises `stream` to check it; a sigma that is NaN, inf or
+ * negative, one_minus_theta outside [0, 1) under OU, a NULL pointer where one is needed, a non-NULL ou_state under
+ * GAUSSIAN, an unknown kind or overlapping action and mu is R2D2_ERR_ARG; unsupported shapes are R2D2_ERR_UNSUPPORTED
+ * as for r2d2_policy_step.  Nothing is launched on an error. */
+int r2d2_policy_step_explore(const r2d2_net_shape* shape, const float* const params[4], const float* obs,
+                             const float* state_in, float* state_out, float* mu, int N, float* workspace,
+                             const float* obs_mean, const float* obs_inv_std, float clip,
+                             const r2d2_exploration* exploration, float* action, r2d2_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Observation normalisation (off unless a caller attaches it).  Statistics are moment blocks of [1 + 2 O] doubles:
  * count, mean [O], M2 [O] (the sum of squared deviations from the mean).  The fp32 pair every transform reads is

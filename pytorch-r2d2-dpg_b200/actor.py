@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from models import ActorNet, CriticNet
+from r2d2_b200 import exploration
 from r2d2_b200 import metrics
 from r2d2_b200 import obs_norm as obs_norm_mod
 from r2d2_b200 import td_options
@@ -92,6 +93,10 @@ class Actor:
         self.critic = CriticNet(self.obs_size, self.action_size, 0, hidden=self.hidden).to(self.device).eval()
         self.target_critic = deepcopy(self.critic)
         self.obs_norm = None      # model.pt's `obs_norm` {mean_f, inv_std_f, clip} when the learner normalises obs
+        # R2D2_EXPLORATION=gaussian|ou: noise keyed on (seed, actor id, step), as ActorPool lanes and the GPU draw it
+        self.exploration = exploration.from_environ()
+        self.noise = None if self.exploration.mode == "reference" else \
+            exploration.HostNoise(self.exploration, [actor_id], self.action_size)
         # R2D2_METRICS=1: one row per finished episode (r2d2_b200.metrics.EPISODE_COLUMNS)
         self.episode_log = metrics.episode_csv("actor", actor_id) if metrics.from_environ() else None
         self.load_model()
@@ -163,6 +168,8 @@ class Actor:
             obs = get_obs(time_step.observation)
             for _, net in self._nets():
                 net.reset_state()
+            if self.noise is not None:
+                self.noise.reset([0])
             self.sequence, self.recurrent_state, self.priority = [], [], []
             episode += 1
             reward_sum = 0.0
@@ -173,7 +180,10 @@ class Actor:
                     action = self.actor(x)
                     self.critic(x, action)
                     self.target_critic(x, self.target_actor(x))
-                action = np.clip(action.cpu().numpy()[0] + np.random.normal(0, 0.3, self.action_size), -1, 1)
+                if self.noise is None:
+                    action = np.clip(action.cpu().numpy()[0] + np.random.normal(0, 0.3, self.action_size), -1, 1)
+                else:
+                    action = self.noise.actions(action.cpu().numpy(), step)[0]
                 reward = 0.0
                 for _ in range(4):                                        # action repeat, actor.py:152-157
                     time_step = self.env.step(action)

@@ -2,7 +2,9 @@
 recurrent nets of all lanes together on the GPU (r2d2_b200.policy_step.PolicyStepper -> r2d2_policy_step), while each
 lane steps its own environment on the host.  Lane by lane it does what `Actor.run` does (actor.py:138-179):
 
-  * env from `actor._make_env(actor_id)`, action repeat 4; action = clip(mu + N(0, noise_std), -1, 1);
+  * env from `actor._make_env(actor_id)`, action repeat 4; action = clip(mu + N(0, noise_std), -1, 1), or under
+    R2D2_EXPLORATION=gaussian|ou (r2d2_b200.exploration) the actions the stepper draws for each lane's actor id at
+    t = the pool step, the noise a drop-in Actor with that id draws at its own step t;
   * the recorded recurrent state of a step is the state BEFORE that step, nets in the order actor, target_actor,
     critic, target_critic (actor.py:149,166);
   * episodes shorter than burn_in + learning = 60 steps are dropped; kept ones get n_step pad rows, n-step rewards and
@@ -17,7 +19,8 @@ lane steps its own environment on the host.  Lane by lane it does what `Actor.ru
 Differences from separate Actor processes:
   * the lanes step in lock-step: a lane whose episode ends starts the next one on the next pool step;
   * all lanes share one initial weight set until model.pt exists (each Actor draws its own);
-  * exploration noise comes from one seeded generator per pool, not from each process's global numpy state.
+  * in the reference exploration mode, the noise comes from one seeded generator per pool, not from each process's
+    global numpy state (the gaussian and ou modes key it on the actor id and the step, as Actor does).
 
 `actor_pool_process(actor_ids)` is the process entry point (picklable under spawn); pool_launch.py starts pools next to
 the learner.  The stepper and the priority function are arguments so the host bookkeeping can run with
@@ -46,6 +49,19 @@ class ModelsStepper(StateRing):
         self.nets = [cls(obs_size, n_actions, 0, hidden=hidden).to(self.device).eval()
                      for cls in (ActorNet, ActorNet, CriticNet, CriticNet)]
         self.obs_norm = None
+        self.noise = None             # set_exploration: r2d2_b200.exploration.HostNoise, the kernel's noise on the host
+
+    def set_exploration(self, options, actor_ids):
+        from r2d2_b200.exploration import HostNoise
+        if len(actor_ids) != self.n_lanes:
+            raise ValueError("set_exploration: %d actor ids for %d lanes" % (len(actor_ids), self.n_lanes))
+        self.noise = HostNoise(options, actor_ids, self.n_actions)
+
+    def reset(self, lanes):
+        lanes = list(lanes)
+        super().reset(lanes)
+        if self.noise is not None:
+            self.noise.reset(lanes)
 
     def load(self, model_dict):
         for net, name in zip(self.nets, NETS):
@@ -67,7 +83,10 @@ class ModelsStepper(StateRing):
         target_critic(x, target_actor(x))
         for k, net in enumerate(self.nets):
             state_out[k, 0], state_out[k, 1] = net.hx, net.cx
-        return mu.cpu().numpy()
+        mu = mu.cpu().numpy()
+        if self.noise is not None:
+            self.actions = self.noise.actions(mu, self.t)
+        return mu
 
 
 def initial_model_dict(obs_size, n_actions, hidden):
@@ -107,8 +126,11 @@ class ActorPool:
                                     max_episode_steps=max_episode_steps)
         self.stepper = stepper
         self.device = stepper.device
-        from r2d2_b200 import td_options
+        from r2d2_b200 import exploration, td_options
         self.td_options = td_options.from_environ()
+        self.exploration = exploration.from_environ()
+        if self.exploration.mode != "reference":
+            self.stepper.set_exploration(self.exploration, self.actor_ids)
         from r2d2_b200 import metrics
         self.episode_log = metrics.episode_csv("pool", self.actor_ids[0]) if metrics.from_environ() else None
         self.priority_fn = priority_fn or self._gpu_priorities
@@ -162,8 +184,11 @@ class ActorPool:
         mu = self.stepper.step(self.obs)
         t1 = perf_counter()
         self.last_mu = mu
-        actions = mu + self.rng.normal(0.0, self.noise_std, mu.shape) if self.noise_std else mu
-        actions = np.clip(actions, -1, 1)
+        if self.exploration.mode == "reference":
+            actions = mu + self.rng.normal(0.0, self.noise_std, mu.shape) if self.noise_std else mu
+            actions = np.clip(actions, -1, 1)
+        else:
+            actions = self.stepper.actions
         finished = []
         for lane, env in enumerate(self.envs):
             action = actions[lane]

@@ -232,6 +232,15 @@ int r2d2_policy_step_ex(const r2d2_net_shape* shape, const float* const params[4
                      workspace, S(stream), obs_mean, obs_inv_std, clip);
 }
 
+int r2d2_policy_step_explore(const r2d2_net_shape* shape, const float* const params[4], const float* obs,
+                             const float* state_in, float* state_out, float* mu, int N, float* workspace,
+                             const float* obs_mean, const float* obs_inv_std, float clip,
+                             const r2d2_exploration* exploration, float* action, r2d2_stream_t stream) {
+  R2D2_REQUIRE(shape && exploration, "null");
+  return policy_step(shape->obs_size, shape->n_actions, shape->hidden, params, obs, state_in, state_out, mu, N,
+                     workspace, S(stream), obs_mean, obs_inv_std, clip, exploration, action);
+}
+
 int r2d2_obs_norm_merge(double* running, const double* blocks, int W, int O, float* mean_f, float* inv_std_f,
                         r2d2_stream_t stream) {
   return obs_norm_merge(running, blocks, W, O, mean_f, inv_std_f, S(stream));

@@ -23,9 +23,17 @@
 // (per thread k ascending, then the same butterfly tree), with no atomics, so lane n's bits do not depend on the
 // other lanes.
 //
+// Exploration (r2d2_policy_step_explore): phase 3 runs as policy_explore_head_kernel, which also turns each of the
+// actor's mu elements into its noisy action from the same registers (explore_action).  The other four phases and mu
+// itself are unchanged.
+//
 // Each kernel issues L2 prefetches of its weight rows before griddepcontrol.wait, so they overlap the tail of the
 // phase before; every kernel executes the wait, which makes the chain transitive (phase 5 may read phase 1's G).
+#include <cmath>
+#include <vector>
+
 #include "obs_norm.cuh"
+#include "philox.cuh"
 #include "policy.cuh"
 
 namespace r2d2 {
@@ -50,6 +58,18 @@ struct StepArgs {
   const float *obs_mean, *obs_inv_std;   // r2d2_policy_step_ex: phase 1 stages obs_norm_apply(obs) (the kNorm kernel)
   float obs_clip;
 };
+
+// r2d2_exploration as the head kernel reads it
+struct ExploreArgs {
+  const unsigned int* actor_id;    // [N]
+  const float* sigma;              // [N]
+  float* ou_state;                 // [N,A] (OU)
+  float* action;                   // [N,A]
+  uint32_t seed, step_lo, step_hi;
+  float one_minus_theta;
+};
+
+constexpr int kNoNoise = 0, kGaussian = 1, kOU = 2;
 
 struct NetView {
   const float *w1, *b1, *wih, *whh, *bih, *bhh, *w3, *b3;
@@ -181,12 +201,30 @@ __device__ __forceinline__ void cell_update(const float (&v)[2], const StepArgs&
   a.state_out[((size_t)(net * 2) * N + n) * H + j] = go * tanhf(c2);
 }
 
+// lane n's action a from its noise-free mu m (include/r2d2_b200.h r2d2_exploration); under OU x is updated in place
+template <int kNoise>
+__device__ __forceinline__ float explore_action(const ExploreArgs& e, float m, int n, int a, int A) {
+  const Philox4 r = philox4x32_10((uint32_t)(a >> 2), e.step_lo, e.step_hi, 1u, e.seed, __ldg(e.actor_id + n));
+  const bool upper = (a & 2) != 0;                    // words (x2, x3) serve a % 4 in {2, 3}
+  float rad, s, c;
+  box_muller(upper ? r.x[2] : r.x[0], upper ? r.x[3] : r.x[1], rad, s, c);
+  const float z = __fmul_rn(rad, (a & 1) ? s : c);
+  float noise = __fmul_rn(__ldg(e.sigma + n), z);
+  if (kNoise == kOU) {
+    float* x = e.ou_state + (size_t)n * A + a;
+    noise = __fadd_rn(__fmul_rn(e.one_minus_theta, *x), noise);
+    *x = noise;
+  }
+  return fminf(fmaxf(__fadd_rn(m, noise), -1.0f), 1.0f);
+}
+
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;"); }
 
-// kNormObs (phase 1 only): the obs rows are normalised as they are staged
-template <int PHASE, bool kNormObs>
-__device__ __forceinline__ void policy_phase(const StepArgs& a) {
+// kNormObs (phase 1 only): the obs rows are normalised as they are staged.  kNoise (phase 3 only): the actor head
+// also writes e.action.
+template <int PHASE, bool kNormObs, int kNoise = kNoNoise>
+__device__ __forceinline__ void policy_phase(const StepArgs& a, const ExploreArgs& e = ExploreArgs{}) {
   __shared__ __align__(16) float xs[KC * XS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile0 = blockIdx.y * NT;
@@ -259,7 +297,12 @@ __device__ __forceinline__ void policy_phase(const StepArgs& a) {
     if (row < a.A) {
 #pragma unroll
       for (int i = 0; i < 2; ++i)
-        if (n_out + i < N) out[(size_t)(n_out + i) * a.A + row] = tanhf(v[i] + P.b3[row]);
+        if (n_out + i < N) {
+          const float m = tanhf(v[i] + P.b3[row]);
+          out[(size_t)(n_out + i) * a.A + row] = m;
+          if (kNoise != kNoNoise && net == 0)
+            e.action[(size_t)(n_out + i) * a.A + row] = explore_action<kNoise>(e, m, n_out + i, row, a.A);
+        }
     }
   } else {                                            // PHASE 4: critics' action columns of l1, then tanh
     const int net = 2 + blockIdx.z;
@@ -293,8 +336,14 @@ __global__ void __launch_bounds__(THREADS, 2) policy_obs_norm_phase1_kernel(cons
   policy_phase<1, true>(a);
 }
 
-template <typename Kernel>
-int launch_phase(Kernel kernel, dim3 grid, const StepArgs& a, cudaStream_t stream) {
+// phase 3 of r2d2_policy_step_explore (kNoise: kGaussian or kOU)
+template <int kNoise>
+__global__ void __launch_bounds__(THREADS, 2) policy_explore_head_kernel(const StepArgs a, const ExploreArgs e) {
+  policy_phase<3, false, kNoise>(a, e);
+}
+
+template <typename Kernel, typename... Extra>
+int launch_phase(Kernel kernel, dim3 grid, const StepArgs& a, cudaStream_t stream, const Extra&... extra) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = dim3(THREADS);
@@ -305,7 +354,7 @@ int launch_phase(Kernel kernel, dim3 grid, const StepArgs& a, cudaStream_t strea
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  R2D2_CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, a));
+  R2D2_CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, a, extra...));
   count_launch();
   return R2D2_OK;
 }
@@ -319,7 +368,7 @@ size_t policy_workspace_floats(int O, int A, int H, int N) {
 
 int policy_step(int O, int A, int H, const float* const params[4], const float* obs, const float* state_in,
                 float* state_out, float* mu, int N, float* workspace, cudaStream_t stream, const float* obs_mean,
-                const float* obs_inv_std, float obs_clip) {
+                const float* obs_inv_std, float obs_clip, const r2d2_exploration* explore, float* action) {
   R2D2_REQUIRE(params && params[0] && params[1] && params[2] && params[3] && obs && state_in && state_out && mu &&
                    workspace, "null");
   R2D2_REQUIRE(state_in != state_out, "state_in and state_out must be different buffers");
@@ -332,6 +381,30 @@ int policy_step(int O, int A, int H, const float* const params[4], const float* 
                    std::to_string(kPolicyMaxLanes) + ", H a multiple of 32 up to " + std::to_string(kPolicyMaxHidden) +
                    ", 1 <= A <= " + std::to_string(kPolicyMaxActions) + ", O >= 1)");
     return R2D2_ERR_UNSUPPORTED;
+  }
+  ExploreArgs e = {};
+  if (explore) {
+    const bool ou = explore->kind == R2D2_EXPLORATION_OU;
+    R2D2_REQUIRE(ou || explore->kind == R2D2_EXPLORATION_GAUSSIAN,
+                 "kind is R2D2_EXPLORATION_GAUSSIAN or R2D2_EXPLORATION_OU");
+    R2D2_REQUIRE(explore->actor_id && explore->sigma && action, "null");
+    R2D2_REQUIRE(ou == (explore->ou_state != nullptr), "ou_state is given under OU and NULL under GAUSSIAN");
+    R2D2_REQUIRE(!ou || (explore->one_minus_theta >= 0.0f && explore->one_minus_theta < 1.0f),
+                 "one_minus_theta = 1 - theta with theta in (0, 1]");
+    const size_t NA = (size_t)N * A;
+    R2D2_REQUIRE(action + NA <= mu || mu + NA <= action, "action must not overlap mu");
+    std::vector<float> sigma(N);
+    R2D2_CUDA_TRY(cudaMemcpyAsync(sigma.data(), explore->sigma, sizeof(float) * N, cudaMemcpyDeviceToHost, stream));
+    R2D2_CUDA_TRY(cudaStreamSynchronize(stream));
+    for (int n = 0; n < N; ++n)
+      if (!(sigma[n] >= 0.0f && std::isfinite(sigma[n]))) {
+        set_last_error("r2d2_policy_step_explore: sigma[" + std::to_string(n) + "] = " + std::to_string(sigma[n]) +
+                       " (allowed: finite and >= 0)");
+        return R2D2_ERR_ARG;
+      }
+    e.actor_id = explore->actor_id; e.sigma = explore->sigma; e.ou_state = explore->ou_state; e.action = action;
+    e.seed = explore->seed; e.step_lo = (uint32_t)explore->step; e.step_hi = (uint32_t)(explore->step >> 32);
+    e.one_minus_theta = explore->one_minus_theta;
   }
   StepArgs a;
   a.p0 = params[0]; a.p1 = params[1]; a.p2 = params[2]; a.p3 = params[3];
@@ -347,7 +420,12 @@ int policy_step(int O, int A, int H, const float* const params[4], const float* 
   if (obs_mean) R2D2_TRY(launch_phase(policy_obs_norm_phase1_kernel, grid1, a, stream));
   else R2D2_TRY(launch_phase(policy_phase_kernel<1>, grid1, a, stream));
   R2D2_TRY(launch_phase(policy_phase_kernel<2>, dim3(H / WARPS, tiles, 2), a, stream));
-  R2D2_TRY(launch_phase(policy_phase_kernel<3>, dim3(head_blocks, tiles, 2), a, stream));
+  const dim3 grid3(head_blocks, tiles, 2);
+  if (!explore) R2D2_TRY(launch_phase(policy_phase_kernel<3>, grid3, a, stream));
+  else if (explore->kind == R2D2_EXPLORATION_OU)
+    R2D2_TRY(launch_phase(policy_explore_head_kernel<kOU>, grid3, a, stream, e));
+  else
+    R2D2_TRY(launch_phase(policy_explore_head_kernel<kGaussian>, grid3, a, stream, e));
   R2D2_TRY(launch_phase(policy_phase_kernel<4>, dim3(H / (4 * WARPS), tiles, 2), a, stream));
   R2D2_TRY(launch_phase(policy_phase_kernel<5>, dim3(H / WARPS, tiles, 2), a, stream));
   return R2D2_OK;

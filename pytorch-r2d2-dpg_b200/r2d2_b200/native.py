@@ -71,6 +71,15 @@ class ReplaySnapshotInfo(Structure):
                                   "next_serial", "evicted_total", "rows_used")]
 
 
+class Exploration(Structure):
+    """r2d2_exploration: actor_id, sigma, ou_state are device addresses (ou_state None under GAUSSIAN)."""
+    _fields_ = [("kind", c_int), ("seed", c_uint), ("step", c_ulonglong), ("one_minus_theta", c_float),
+                ("actor_id", c_void_p), ("sigma", c_void_p), ("ou_state", c_void_p)]
+
+
+EXPLORATION_GAUSSIAN, EXPLORATION_OU = 0, 1   # Exploration.kind (R2D2_EXPLORATION_GAUSSIAN / _OU)
+
+
 class LearnerOptions(Structure):
     _fields_ = [("twin_critic", c_int)]
 
@@ -134,6 +143,9 @@ SIGNATURES = {
                                  c_void_p, c_void_p]),
     "r2d2_policy_step_ex": (c_int, [POINTER(NetShape), POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                     c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
+    "r2d2_policy_step_explore": (c_int, [POINTER(NetShape), POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_int, c_void_p, c_void_p, c_void_p, c_float, POINTER(Exploration), c_void_p,
+                                         c_void_p]),
     "r2d2_obs_norm_merge": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "r2d2_obs_normalize": (c_int, [c_void_p, c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_float, c_void_p]),
     "r2d2_adam_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_float, c_float, c_float,
@@ -275,4 +287,4 @@ def host_f32(a):
 
 
 __all__ = ["lib", "check", "dptr", "current_stream", "NativeError", "NetShape", "ReplayConfig", "ReplayStats",
-           "ReplayOptions", "ReplaySnapshotInfo", "STATE_F32", "STATE_F16", "STATE_MEMORY_DEVICE", "STATE_MEMORY_HOST", "LearnerConfig", "LearnerOptions", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
+           "ReplayOptions", "ReplaySnapshotInfo", "STATE_F32", "STATE_F16", "STATE_MEMORY_DEVICE", "STATE_MEMORY_HOST", "LearnerConfig", "LearnerOptions", "Exploration", "EXPLORATION_GAUSSIAN", "EXPLORATION_OU", "GlobalLayout", "LearnerBuffers", "TdOptions", "SIGNATURES", "view_f32", "view_i64", "host_f32", "byref"]
