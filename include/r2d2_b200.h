@@ -568,11 +568,16 @@ int r2d2_learner_target_phase(r2d2_learner_t* l, int slot, r2d2_stream_t stream)
 /* forget a target phase that ran ahead: the caller is about to overwrite that slot's batch */
 int r2d2_learner_discard_prefetch(r2d2_learner_t* l, r2d2_stream_t stream);
 /* phase 1: target chains (unless r2d2_learner_target_phase already ran for the selected slot), online critic chain,
- * TD/priority kernel, critic BPTT -> critic_grads */
+ * TD/priority kernel, critic BPTT -> critic_grads.  On one GPU (no peers attached, actor-input overlap on) and unless
+ * R2D2_OVERLAP_INPUTS=0, whole chains run on a second stream the learner owns: the actor's forward chain from the start
+ * of this call, and everything after the TD kernels (critic BPTT, the twin's chain, TD and BPTT, the metrics record).
+ * The priorities, q, target and losses[0] are ordered on `stream` when this call returns; critic_grads, losses[2] and the
+ * metrics record only after r2d2_learner_actor_phase (or r2d2_learner_discard_prefetch) on that stream. */
 int r2d2_learner_critic_phase(r2d2_learner_t* l, r2d2_stream_t stream);
 /* optional, between phase 1 and phase 2: the actor's forward chain of the DPG update (learner.py:117,120-123; zero
  * state, 2 cell steps per row).  It does not read the critic, so a data-parallel caller issues it while the
- * all-reduce of critic_grads is in flight; phase 2 then skips it.  Without this call phase 2 runs it itself. */
+ * all-reduce of critic_grads is in flight; phase 2 then skips it.  Without this call phase 2 runs it itself.  A no-op
+ * when it already ran for the iteration (phase 1 issues it on the second stream, see above). */
 int r2d2_learner_actor_forward(r2d2_learner_t* l, r2d2_stream_t stream);
 /* phase 2: critic Adam (grads * grad_scale; norm kernel first when clipping, Polyak update of the critic's target on
  * update iterations when target_tau < 1), actor chain unless r2d2_learner_actor_forward already ran, critic on actor

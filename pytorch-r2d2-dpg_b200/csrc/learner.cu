@@ -22,6 +22,10 @@
 // the actor loss in phase 2 write the iteration's record, the norm kernel runs before each Adam even without clipping, and
 // phase 3 copies the actor's norm into the ring.  Off, none of it is issued.
 //
+// Concurrent chains (one GPU, R2D2_OVERLAP_INPUTS not 0): phase 1 runs the actor's forward chain of phase 2, and its own
+// work after the TD kernels, on a second learner-owned stream (aux) beside the learner stream's chains; phase 2 joins
+// it before the critic's Adam.  Same kernels, same bits; learner_critic_phase lists the shared buffers.
+//
 // The actor burn-in of learner.py:92 is skipped: its state is discarded at learner.py:117 before any use.
 #include "learner.cuh"
 
@@ -113,16 +117,19 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg, bool twin_crit
   }
   R2D2_CUDA_TRY(cudaStreamSynchronize(0));
   learner_select_batch(l, 0);
-  {   // R2D2_OVERLAP_INPUTS=0 disables the side stream (A/B)
+  {   // R2D2_OVERLAP_INPUTS=0 disables the side and aux streams: the fully serial order (A/B)
     const char* e = getenv("R2D2_OVERLAP_INPUTS");
     l->overlap_inputs = !(e && e[0] == '0');
     if (l->overlap_inputs) {
       int lo = 0, hi = 0;
       R2D2_CUDA_TRY(cudaDeviceGetStreamPriorityRange(&lo, &hi));
       R2D2_CUDA_TRY(cudaStreamCreateWithPriority(&l->side, cudaStreamNonBlocking, lo));   // lowest priority: leftovers only
-      R2D2_CUDA_TRY(cudaEventCreateWithFlags(&l->ev_fork, cudaEventDisableTiming));
-      R2D2_CUDA_TRY(cudaEventCreateWithFlags(&l->ev_c1_inputs, cudaEventDisableTiming));
-      R2D2_CUDA_TRY(cudaEventCreateWithFlags(&l->ev_a1_inputs, cudaEventDisableTiming));
+      // aux at the lowest priority too, a caller's default stream's: a cfg-3 iteration measured 1.2 ms faster than
+      // with aux at the highest (DESIGN.md §7)
+      R2D2_CUDA_TRY(cudaStreamCreateWithPriority(&l->aux, cudaStreamNonBlocking, lo));
+      for (cudaEvent_t* ev : {&l->ev_fork, &l->ev_c1_inputs, &l->ev_a1_inputs, &l->ev_aux_fork, &l->ev_aux_done,
+                              &l->ev_q_next_read})
+        R2D2_CUDA_TRY(cudaEventCreateWithFlags(ev, cudaEventDisableTiming));
     }
   }
   *out = l;
@@ -132,9 +139,9 @@ int learner_create(Learner** out, const r2d2_learner_config* cfg, bool twin_crit
 int learner_destroy(Learner* l) {
   if (!l) return R2D2_OK;
   if (l->side) { cudaStreamSynchronize(l->side); cudaStreamDestroy(l->side); }
-  if (l->ev_fork) cudaEventDestroy(l->ev_fork);
-  if (l->ev_c1_inputs) cudaEventDestroy(l->ev_c1_inputs);
-  if (l->ev_a1_inputs) cudaEventDestroy(l->ev_a1_inputs);
+  if (l->aux) { cudaStreamSynchronize(l->aux); cudaStreamDestroy(l->aux); }
+  for (cudaEvent_t ev : {l->ev_fork, l->ev_c1_inputs, l->ev_a1_inputs, l->ev_aux_fork, l->ev_aux_done, l->ev_q_next_read})
+    if (ev) cudaEventDestroy(ev);
   cudaFree(l->arena);
   cudaFree(l->metrics_part);
   delete l->peer;
@@ -155,6 +162,8 @@ int learner_discard_prefetch(Learner* l, cudaStream_t st) {
   R2D2_REQUIRE(l, "null");
   // whatever the side stream still writes into the online critic's workspace for the dropped batch goes first
   if (l->c1_inputs_slot >= 0 && l->side) R2D2_CUDA_TRY(cudaStreamWaitEvent(st, l->ev_c1_inputs, 0));
+  // and whatever the aux stream still reads of the batch in flight (a caller may overwrite either slot next)
+  if (l->aux_pending) R2D2_CUDA_TRY(cudaStreamWaitEvent(st, l->ev_aux_done, 0));
   l->c1_inputs_slot = -1;
   l->targets_slot = -1;
   return R2D2_OK;
@@ -222,6 +231,10 @@ int learner_target_phase(Learner* l, int slot, cudaStream_t st) {
                               l->noise_seed, l->noise_rank, (unsigned long long)l->critic_iters, st));
   // target critic: stored actions while burning in, target-actor actions afterwards (learner.py:95,106)
   R2D2_TRY(net_forward(l->critic_sh, Pc_t, l->ws_tc, b.obs, l->act_tc, st_tc, st_tc + BH, Tt, B, 1, st));
+  if (l->q_next_pending) {   // the twin's TD of the batch in flight, on aux, reads q_next until here
+    R2D2_CUDA_TRY(cudaStreamWaitEvent(st, l->ev_q_next_read, 0));
+    l->q_next_pending = false;
+  }
   R2D2_TRY(net_head_forward(l->critic_sh, Pc_t, l->ws_tc, Bn + n, Tt, B, 1, l->q_next, A, st));
   if (l->twin) {   // target critic 2 from the zero state on the same actions, then q_next = min(q'_1, q'_2)
     const NetParams Pc_t2 = NetParams::from_flat(c.target_critic_params + l->critic_stride(), l->critic_sh);
@@ -243,7 +256,21 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
   const NetParams Gc = NetParams::from_flat(c.critic_grads, l->critic_sh);
   const size_t BH = (size_t)B * H;
   const float* st_c = l->states + 4 * BH;    // states[2] = critic
+  const bool concurrent = l->concurrent_chains();
+  auto fork_aux = [&]() -> int {
+    R2D2_CUDA_TRY(cudaEventRecord(l->ev_aux_fork, st));
+    R2D2_CUDA_TRY(cudaStreamWaitEvent(l->aux, l->ev_aux_fork, 0));
+    return R2D2_OK;
+  };
 
+  // The actor's forward chain reads batch i and the actor weights, which the finish phase of i-1 wrote before this
+  // call: on aux it runs beside the target and online critic chains below (the actor phase skips it)
+  int actor_launches = 0;
+  if (concurrent && !l->actor_forward_done) {
+    R2D2_TRY(fork_aux());
+    R2D2_TRY(learner_actor_forward(l, l->aux));
+    actor_launches = l->launches_actor_forward;
+  }
   l->target_phase_standalone = l->targets_slot == l->cur_slot;
   if (!l->target_phase_standalone) R2D2_TRY(learner_target_phase(l, l->cur_slot, st));
   // online critic over rows [0, Bn+L) with stored actions (learner.py:93,105); burn-in stays on the tape (Q4)
@@ -264,22 +291,47 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
   tp.is_weight = l->importance_weighting ? l->is_weight : nullptr;
   R2D2_TRY(td_priority(tp, st, TdOptions{l->rescaling, l->rescaling_eps, l->priority_metric}));
 
-  R2D2_CUDA_TRY(cudaMemsetAsync(c.critic_grads, 0, sizeof(float) * l->critic_block(), st));
-  R2D2_TRY(net_backward(l->critic_sh, Pc, &Gc, l->ws_c1, l->obs, l->act, l->dq, Bn, Tc, B, 1, nullptr, nullptr, st));
+  // The priorities exist.  Concurrent chains: the rest of the phase forks onto aux, and the learner stream goes on to
+  // the caller's hook and the next batch's target chains; the actor phase joins aux (ev_aux_done) before the critic's
+  // Adam.  What the forked work shares with the learner stream until that join, and why each is ordered:
+  //   slot i (obs, act, rew, term, is_weight)   read only; the hook writes the other slot
+  //   ws_c1 (z1, dG, hs, ...), dq               only the critic phase of i+1 and the side-stream input projection of
+  //                                             batch i+1 write them, both issued after the join (the actor phase forks
+  //                                             that projection after the critic's Adam)
+  //   q, target, priority, losses[0]            written above; the hook only reads the priorities
+  //   q_next                                    the twin's TD reads it; the next target phase writes it after waiting
+  //                                             for ev_q_next_read
+  //   critic_grads, ws_c1_2, q2, dq2, td_sq2, losses[2], metrics partials: aux only until the join
+  //   ws_a1, mu (actor forward above)          the actor phase reads them after the join
+  //   GEMM operand images, split-K and TD partials: per (device, stream) scratch, aux has its own
+  //   act_tc, ws_ta, ws_tc, ws_tc_2, q_next2   the target phase's alone; no forked kernel reads them
+  // Data parallel keeps the serial order: a slice-sum kernel spins on SMs that a forked BPTT would need, and the NCCL
+  // mode all-reduces the gradients on a stream ordered behind the learner stream only.
+  cudaStream_t bs = st;
+  if (concurrent) {
+    R2D2_TRY(fork_aux());
+    bs = l->aux;
+  }
+  R2D2_CUDA_TRY(cudaMemsetAsync(c.critic_grads, 0, sizeof(float) * l->critic_block(), bs));
+  R2D2_TRY(net_backward(l->critic_sh, Pc, &Gc, l->ws_c1, l->obs, l->act, l->dq, Bn, Tc, B, 1, nullptr, nullptr, bs));
   if (l->twin) {
     // critic 2 from the zero state over the same rows with the stored actions, its TD against the same y (q_next is
     // already the minimum; target / priority stay critic 1's), its loss into losses[2], its BPTT into the second half
     const size_t off = l->critic_stride();
     const NetParams Pc2 = NetParams::from_flat(c.critic_params + off, l->critic_sh);
     const NetParams Gc2 = NetParams::from_flat(c.critic_grads + off, l->critic_sh);
-    R2D2_TRY(net_forward(l->critic_sh, Pc2, l->ws_c1_2, l->obs, l->act, nullptr, nullptr, Tc, B, 1, st));
-    R2D2_TRY(net_head_forward(l->critic_sh, Pc2, l->ws_c1_2, Bn, Tc, B, 1, l->q2, A, st));
+    R2D2_TRY(net_forward(l->critic_sh, Pc2, l->ws_c1_2, l->obs, l->act, nullptr, nullptr, Tc, B, 1, bs));
+    R2D2_TRY(net_head_forward(l->critic_sh, Pc2, l->ws_c1_2, Bn, Tc, B, 1, l->q2, A, bs));
     TdPriorityParams tp2 = tp;
     tp2.q = l->q2; tp2.target = nullptr; tp2.dq = l->dq2; tp2.td_sq = l->td_sq2; tp2.priority = nullptr;
     tp2.loss_sum = l->losses + 2;
-    R2D2_TRY(td_priority(tp2, st, TdOptions{l->rescaling, l->rescaling_eps, l->priority_metric}));
+    R2D2_TRY(td_priority(tp2, bs, TdOptions{l->rescaling, l->rescaling_eps, l->priority_metric}));
+    if (concurrent) {
+      R2D2_CUDA_TRY(cudaEventRecord(l->ev_q_next_read, bs));
+      l->q_next_pending = true;
+    }
     R2D2_TRY(net_backward(l->critic_sh, Pc2, &Gc2, l->ws_c1_2, l->obs, l->act, l->dq2, Bn, Tc, B, 1, nullptr, nullptr,
-                          st));
+                          bs));
   }
   if (l->peer) R2D2_TRY(peer_signal(*l->peer, kPeerCritic, st));
   l->critic_phase_ran = true;
@@ -289,17 +341,23 @@ int learner_critic_phase(Learner* l, cudaStream_t st) {
     mp.q = l->q; mp.target = l->target; mp.q2 = l->twin ? l->q2 : nullptr; mp.priority = l->priority;
     mp.is_weight = l->importance_weighting ? l->is_weight : nullptr; mp.losses = l->losses;
     mp.n = (long long)L * B * A; mp.B = B; mp.iter = l->metrics_iter; mp.rec = l->metrics_record(l->metrics_iter);
-    R2D2_TRY(metrics_critic(mp, l->metrics_part, l->metrics_ticket, st));
+    R2D2_TRY(metrics_critic(mp, l->metrics_part, l->metrics_ticket, bs));
+  }
+  if (concurrent) {
+    R2D2_CUDA_TRY(cudaEventRecord(l->ev_aux_done, l->aux));
+    l->aux_pending = true;
   }
   l->critic_iters += 1;
-  l->launches_phase[0] = (int)(launch_count() - launches0);
+  l->launches_phase[0] = (int)(launch_count() - launches0) - actor_launches;   // the actor phase counts those
   return R2D2_OK;
 }
 
 // The actor's forward chain of the DPG update (learner.py:117,120-123 without the critic call): it reads the actor's
 // weights and the observations only - NOT the critic - so a data-parallel caller runs it while the all-reduce of the
-// critic gradients is in flight (r2d2_learner_actor_forward), before the critic's optimiser step.
+// critic gradients is in flight (r2d2_learner_actor_forward), before the critic's optimiser step.  A no-op when it already
+// ran for this iteration (with concurrent chains the critic phase issues it on aux).
 int learner_actor_forward(Learner* l, cudaStream_t st) {
+  if (l->actor_forward_done) return R2D2_OK;
   const r2d2_learner_config& c = l->cfg;
   const int B = c.batch, Bn = c.burn_in, L = c.learning, A = c.n_actions, O = c.obs_size;
   const long long launches0 = launch_count();
@@ -355,6 +413,10 @@ int learner_actor_phase(Learner* l, float grad_scale, cudaStream_t st) {
   const NetParams Pc = NetParams::from_flat(c.critic_params, l->critic_sh);
   const long long LBA = (long long)L * B * A;
 
+  if (l->aux_pending) {   // the critic gradients, and the actor's forward chain when the critic phase issued it on aux
+    R2D2_CUDA_TRY(cudaStreamWaitEvent(st, l->ev_aux_done, 0));
+    l->aux_pending = false;
+  }
   int extra = 0;
   if (!l->actor_forward_done) R2D2_TRY(learner_actor_forward(l, st));   // single-GPU order: same kernels, same results
   else extra = l->launches_actor_forward;

@@ -22,6 +22,15 @@ struct Learner {
   bool a1_inputs_pending = false;    // a1's input projection of this iteration was issued on the side stream
   bool actor_forward_done = false;   // learner_actor_forward already ran for the current iteration
   int launches_actor_forward = 0;
+  // second learner-owned stream for whole chains that run beside the learner stream's (single GPU,
+  // overlap_inputs on; learner.cu, learner_critic_phase): the actor's forward chain under the online critic's, the
+  // critic BPTT under the next batch's target chains.  ev_aux_done: the last aux work issued; the actor phase joins it.
+  // ev_q_next_read: the twin's TD on aux has read q_next, which the next target phase overwrites.
+  cudaStream_t aux = nullptr;
+  cudaEvent_t ev_aux_fork = nullptr, ev_aux_done = nullptr, ev_q_next_read = nullptr;
+  bool aux_pending = false;          // ev_aux_done is recorded and the actor phase has not joined it yet
+  bool q_next_pending = false;       // ev_q_next_read is recorded and no target phase has waited for it yet
+  bool concurrent_chains() const { return aux && overlap_actor_inputs && !peer; }
   float* arena = nullptr;
   size_t arena_floats = 0;
   // batch (filled by replay_sample or by the caller).  Two slots: while the phases of iteration i still read slot s, the

@@ -598,7 +598,9 @@ class LearnerEngine:
         one GPU the input projections hide under their scans as before).  On iterations that update the target nets
         (hard copy, or the Polyak blend of `target_tau` < 1, which starts at the critic's optimiser step) it is called at
         the end of the step instead, and a deferred data-parallel phase 3 is completed before the next critic phase.
-        At `target_interval` 1 that is every iteration: the next batch's target chains never run ahead.
+        At `target_interval` 1 that is every iteration: the next batch's target chains never run ahead.  On one GPU the
+        critic BPTT (and the twin's chain) may still run on the library's second stream while the hook runs: the hook
+        may read `used.priority` and `used.losses[0]`, the rest of `used.losses` is complete when step() returns.
 
         Data parallel, mode "peer" (default): the gradient blocks are summed by the library's own kernels over NVLink
         peer memory inside the phases (csrc/peer.cuh); the actor's optimiser step of iteration i runs after the critic
