@@ -13,10 +13,16 @@ What the reference does, per finished episode of E real rows + n pad rows (actor
     a deque of the last `learning` td values; for i >= burn_in + learning the priority
     0.9 max + 0.1 mean of td^2 over the deque, i.e. priority k covers steps k+burn_in+1 .. k+burn_in+learning
     (one step later than the window the learner trains on - the reference's off-by-one, kept).
+
+And the actor's policy step in float64 (reference actor.py `Actor.run`: actor, target actor, critic on the actor's mu,
+target critic on the target actor's mu, each net one step from its own recurrent state), with the four-net weights the
+policy-step tests draw.
 """
 import numpy as np
 
 from oracle import learner_oracle as lo
+
+NETS = ("actor", "target_actor", "critic", "target_critic")
 
 
 def nstep_rewards(raw, n_step, gamma):
@@ -61,3 +67,32 @@ def window_priorities(q, q_t, rew, term, *, burn_in, learning, n_step, gamma, et
         w = np.abs(w) if metric == "abs" else w ** 2
         out.append(eta * w.max() + (1 - eta) * w.mean())
     return np.asarray(out, np.float64)
+
+
+def policy_params(O, A, H, seed):
+    """{net: state dict} of the four nets in NETS, float32, uniform in +-1 / sqrt(fan-in)."""
+    rng = np.random.default_rng(seed)
+    out = {}
+    for k, name in enumerate(NETS):
+        I = O + (A if k >= 2 else 0)
+        u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.sqrt(fan)  # noqa: E731
+        out[name] = {"l1.weight": u((H, I), I), "l1.bias": u(H, I), "l2.weight_ih": u((4 * H, H), H),
+                     "l2.weight_hh": u((4 * H, H), H), "l2.bias_ih": u(4 * H, H), "l2.bias_hh": u(4 * H, H),
+                     "l3.weight": u((A, H), H), "l3.bias": u(A, H)}
+    return out
+
+
+def policy_step(P, obs, state):
+    """Actor.run's step in float64 (P: {net: float64 weights}): obs [N,O], state [4,2,N,H] before -> (mu, state
+    after)."""
+    new = np.empty_like(state)
+
+    def run(k, x, critic):
+        sv = lo.net_forward(P[NETS[k]], x[None], state[k, 0], state[k, 1], critic=critic)
+        new[k, 0], new[k, 1] = sv["hs"][1], sv["cs"][1]
+        return sv["out"][0]
+    mu = run(0, obs, False)
+    mu_t = run(1, obs, False)
+    run(2, np.concatenate((obs, mu), 1), True)
+    run(3, np.concatenate((obs, mu_t), 1), True)
+    return mu, new

@@ -94,15 +94,18 @@ def port_case(kw, seed=1, n_batches=3, batch_seed=6):
     return sd(port.actor), sd(port.critic), [ref_port.synthetic_batch(pc, seed=batch_seed + i) for i in range(n_batches)]
 
 
-def episode(rng, cfg, E, p_lo=0.01):
-    """One actor episode of E rows plus n_step terminal pad rows, as DeviceReplay.add_episodes takes it."""
+def episode(rng, cfg, E, p_lo=0.01, zero_pad=False):
+    """One actor episode of E rows plus n_step terminal pad rows, as DeviceReplay.add_episodes takes it; zero_pad: obs,
+    act and rew of the pad rows zeroed (the same draws either way)."""
     n_rows = E + cfg.n_step
     term = np.zeros(n_rows, np.float32)
     term[E:] = 1
-    return (rng.standard_normal((n_rows, cfg.obs)).astype(np.float32),
-            rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32),
-            rng.standard_normal(n_rows).astype(np.float32), term,
-            (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32),
+    obs = rng.standard_normal((n_rows, cfg.obs)).astype(np.float32)
+    act = rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32)
+    rew = rng.standard_normal(n_rows).astype(np.float32)
+    if zero_pad:
+        obs[E:], act[E:], rew[E:] = 0, 0, 0
+    return (obs, act, rew, term, (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32),
             rng.uniform(p_lo, 1.0, E - (cfg.burn_in + cfg.learning)).astype(np.float32))
 
 

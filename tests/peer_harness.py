@@ -30,6 +30,8 @@ from ctypes import byref, c_int, c_void_p  # noqa: E402
 
 import numpy as np  # noqa: E402
 
+from kernel_harness import scan_status  # noqa: E402
+
 # one rank's calls: ("select_batch", slot), ("critic_phase",), ("finish_phase",), ("prefetch",), ("target_phase", slot),
 # ("actor_forward",), ("actor_phase",)
 
@@ -246,9 +248,7 @@ class PeerGroup:
 
     def scan_status(self):
         """The scans' device-wide flag (sticky until read): 1 when a bounded hand-off wait of any scan expired."""
-        st = c_int(0)
-        self.nv.check(self.lib.r2d2_scan_status(byref(st), c_void_p(self.streams[0].cuda_stream)))
-        return int(st.value)
+        return scan_status(self.nv, c_void_p(self.streams[0].cuda_stream))
 
     def check_status(self):
         peer, scan = self.peer_status(), self.scan_status()

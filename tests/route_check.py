@@ -4,8 +4,14 @@ change that moves a test case off its route fails by name instead of silently dr
 A route is a key of ROUTE_KERNELS, optionally followed by ":" and comma-separated template arguments, which must match
 the kernel's trailing template arguments (bool arguments as 0 / 1): "smalln:16" is thin_smalln_kernel<*, 16>,
 "scan_fwd:128,32" is lstm_scan_fwd_kernel<128, 32>.  Each test module keeps its own RouteLog for its report."""
+import json
+import os
 import re
+import subprocess
+import sys
+import tempfile
 import time
+from collections import Counter
 
 # route name -> kernel (base name) that serves it
 ROUTE_KERNELS = {
@@ -55,6 +61,85 @@ def parse_route(route):
     return key, (tuple(int(v) for v in spec.split(",")) if spec else None)
 
 
+SENTINEL = "FillFunctor"                      # the kernel of cuda_session's fill
+PAUSES = (0.1, 0.3, 1.0, 2.0, 4.0, 8.0, 8.0)  # seconds between the sessions of observe: eight sessions in all
+
+
+def route_names(names):
+    """The names in `names` that belong to a route kernel."""
+    return [n for n in names if any(b in n for b in ROUTE_KERNELS.values())]
+
+
+def recorded_route(names):
+    return bool(route_names(names))
+
+
+def recorded_sentinel(names):
+    return any(SENTINEL in n for n in names)
+
+
+def cuda_session(fn):
+    """fn() and then a fill kernel of torch's own (the sentinel) under torch.profiler -> (fn's result, the name of every
+    CUDA kernel launch recorded)."""
+    import torch
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        out = fn()
+        torch.empty(256, device="cuda").fill_(1.0)
+        torch.cuda.synchronize()
+    return out, [e.name for e in prof.events() if e.device_type == DeviceType.CUDA]
+
+
+def observe(case, fn, complete, *, agree=False, lost=None, session=cuda_session):
+    """session(fn) until one is complete -> (fn's result, kernel names) of that session, or None when none of
+    len(PAUSES) + 1 sessions was.  Every session runs fn in full, so fn must be idempotent.
+
+    torch.profiler now and then returns a session without some or all of the kernels it ran (on an H100 with torch
+    2.11 / CUDA 12.8, about one session in a hundred, and then often the next few sessions too; in a long-lived test
+    process, after the hundreds of sessions other test files run, collection can stop altogether, which is why the route
+    suites observe in a fresh process).  complete(names) tells a usable session: recorded_route or recorded_sentinel.
+    agree: the caller asserts launch counts exactly, so a session that kept only part of the kernels must not be taken:
+    a complete session counts only when the complete session just before it recorded the same route kernel launches.
+    Each repeated session appends `case` to `lost` and is preceded by a growing pause."""
+    prev = None
+    for pause in PAUSES + (None,):
+        out, names = session(fn)
+        counts = Counter(route_names(names)) if complete(names) else None
+        if counts is not None and (not agree or counts == prev):
+            return out, names
+        prev = counts
+        if lost is not None:
+            lost.append(case)
+        if pause is not None:
+            time.sleep(pause)
+    return None
+
+
+def launch_counts(case, fn, agree=False):
+    """{profiler name of a route kernel: launches} of fn, from a session that recorded a route kernel (observe)."""
+    got = observe(case, fn, recorded_route, agree=agree)
+    assert got is not None, (f"{case}: no two profiler sessions in a row recorded the same launches" if agree else
+                             f"{case}: the profiler recorded no route kernel in {len(PAUSES) + 1} sessions")
+    return dict(Counter(route_names(got[1])))
+
+
+def observe_in_fresh_process(module, timeout):
+    """The JSON that tests/<module>.py's route_child(path) writes, run in a new Python interpreter: route kernels are
+    observed there because a long-lived test process can stop recording them (observe)."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    root = os.path.dirname(here)
+    with tempfile.TemporaryDirectory() as d:
+        out = os.path.join(d, "routes.json")
+        code = ("import sys; sys.path[:0] = %r; import %s as t; t.route_child(%r)"
+                % ([here, root, os.path.join(root, "pytorch-r2d2-dpg_b200")], module, out))
+        res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=timeout, cwd=root)
+        assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
+        with open(out) as f:
+            return json.load(f)
+
+
 class RouteLog:
     """Profiled calls of one test module: `seen` maps a case to the route kernels that ran, `lost` lists the cases whose
     profiler session had to be repeated."""
@@ -64,30 +149,13 @@ class RouteLog:
         self.lost = []
 
     def profile(self, case, fn):
-        """Run fn (idempotent) under the CUDA profiler -> (fn's result, sorted names of the route kernels that ran).
-        torch.profiler now and then returns a session without any of the kernels it ran (on an H100 with torch 2.11 /
-        CUDA 12.8, about one session in a hundred, and then often the next few sessions too): a session that recorded
-        no route kernel at all is repeated after a growing pause, five sessions in all, and then fails.  Every session
-        runs fn in full; the caller checks the values of the last one.  In a long-lived test process, after the hundreds
-        of sessions other test files run, collection can stop altogether (tests/test_gpu_value_rescaling.py): a module
-        with many cases observes them in a fresh process instead (tests/test_gpu_hidden_size.py)."""
-        import torch
-        from torch.autograd import DeviceType
-        from torch.profiler import ProfilerActivity, profile
-        for pause in (0.1, 0.3, 1.0, 3.0, None):
-            torch.cuda.synchronize()
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                out = fn()
-                torch.cuda.synchronize()
-            names = sorted({e.name for e in prof.events() if e.device_type == DeviceType.CUDA})
-            routed = [n for n in names if any(b in n for b in ROUTE_KERNELS.values())]
-            if routed or pause is None:
-                break
-            self.lost.append(case)
-            time.sleep(pause)
-        assert routed, f"{case}: the profiler recorded no route kernel in five sessions (kernels recorded: {names})"
+        """Run fn (idempotent) under the CUDA profiler (observe) -> (fn's result in the last session, sorted names of
+        the route kernels that ran)."""
+        got = observe(case, fn, recorded_route, lost=self.lost)
+        assert got is not None, f"{case}: the profiler recorded no route kernel in {len(PAUSES) + 1} sessions"
+        routed = sorted(set(route_names(got[1])))
         self.seen[case] = routed
-        return out, routed
+        return got[0], routed
 
     def run_routed(self, case, route, fn):
         """profile(), then assert that of the route kernels exactly the expected one served the call (a session that
@@ -100,7 +168,7 @@ class RouteLog:
         """Of the route kernels in `names` (profiler kernel names), exactly the one of `route` and those of the route
         keys `others` ran, and the `route` kernel with its template arguments."""
         key, args = parse_route(route)
-        self.seen.setdefault(case, [n for n in names if any(b in n for b in ROUTE_KERNELS.values())])
+        self.seen.setdefault(case, route_names(names))
         keys = sorted(k for k in ROUTE_KERNELS if any(ROUTE_KERNELS[k] in n for n in names))
         assert keys == sorted({key, *others}), f"{case}: expected route {key} ({ROUTE_KERNELS[key]}), ran: {names}"
         assert ran(names, ROUTE_KERNELS[key], args), f"{case}: expected {ROUTE_KERNELS[key]} {args}: {names}"

@@ -13,17 +13,18 @@ A relative L2 norm over a whole tensor dilutes an error confined to one action c
 with an action axis is also bounded per column (col_err).  Each kernel-level case runs under torch.profiler (run_routed)
 and asserts the kernel that served it, so a dispatch change that moves a case off its route fails by name instead of
 silently dropping the coverage.  Run with -s for the routes seen and the worst errors per group."""
-from collections import defaultdict
-
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_l2
-from learner_harness import col_err, oracle_for
+from kernel_harness import WorstLog, dev, f64, ptr, td_inputs
+from kernel_harness import nv_routes as nv  # noqa: F401
+from learner_harness import col_err, episode, oracle_for
 from oracle import actor_oracle
 from oracle import learner_oracle as lo
 from oracle import ref_port
+from oracle.actor_oracle import NETS, policy_params
 from oracle.sumtree import SumTreeOracle
 from route_check import RouteLog
 
@@ -34,7 +35,7 @@ LEARNER_TOL = 1e-3
 NT, NN, TN = 0, 1, 2
 EPI_NONE, EPI_TANH, EPI_MUL_DTANH = 0, 1, 2
 
-WORST = defaultdict(lambda: [0.0, 0.0])   # group -> [worst rel_l2, worst col_err]
+WORST = WorstLog()
 ROUTES = RouteLog()
 run_routed = ROUTES.run_routed
 
@@ -42,40 +43,8 @@ run_routed = ROUTES.run_routed
 @pytest.fixture(scope="module", autouse=True)
 def report():
     yield
-    print("\nworst errors per group (rel_l2, col_err):")
-    for g, (r, c) in sorted(WORST.items()):
-        print(f"  {g:18s} {r:.2e}  {c:.2e}")
+    WORST.report()
     ROUTES.report()
-
-
-def check(group, name, x, ref, tol, A=None):
-    """rel_l2 < tol, and col_err < tol when the output has an action axis of width A (last axis after reshape)."""
-    r = rel_l2(x, ref)
-    c = col_err(x, ref, A) if A else 0.0
-    w = WORST[group]
-    w[0], w[1] = max(w[0], r), max(w[1], c)
-    assert r < tol, f"{name}: rel_l2 {r:.3e} >= {tol:.0e}"
-    assert c < tol, f"{name}: col_err {c:.3e} >= {tol:.0e} (worst action column)"
-
-
-def dev(a):
-    return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).cuda()
-
-
-def f64(a):
-    return np.asarray(a, np.float32).astype(np.float64)
-
-
-def ptr(t, offset_floats=0):
-    return None if t is None else t.data_ptr() + 4 * offset_floats
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    native.lib()
-    assert native.lib().r2d2_get_gemm_impl() == 1, "these routes are the default implementation's"
-    return native
 
 
 @pytest.fixture(scope="module")
@@ -92,15 +61,6 @@ def gemm(nv, layout, M, N, K, A, lda, B, ldb, C, ldc, *, A2=None, lda2=0, B2=Non
 
 
 # ------------------------------------------------------------------------------------------------ 1. TD / priority
-def td_inputs(L, B, A, Bn, n, seed):
-    rng = np.random.default_rng(seed)
-    T = Bn + L + n
-    q, qn = rng.standard_normal((L, B, A)) * 2, rng.standard_normal((L, B, A)) * 5
-    rew = rng.standard_normal((T, B)) * 3
-    term = (rng.uniform(size=(T, B)) < 0.15).astype(np.float64)    # terminals anywhere, the window's middle included
-    return q, qn, rew, term
-
-
 def td_call(nv, inputs, L, B, A, Bn, n, want=("y", "dq", "td", "p", "loss"), w=None):
     """r2d2_td_priority (or _weighted when w is given) with the outputs in `want`, NULL for the others; the requested
     outputs start as NaN so that an unwritten element fails every bound."""
@@ -122,13 +82,13 @@ def td_call(nv, inputs, L, B, A, Bn, n, want=("y", "dq", "td", "p", "loss"), w=N
 def check_td(group, o, ref, A):
     y, loss, dq, td_sq, prio = ref
     if "y" in o:
-        check(group, "target", o["y"], y, 1e-6, A)
+        WORST.bound(group, "target", o["y"], y, 1e-6, cols=A)
     if "dq" in o:
-        check(group, "dq", o["dq"], dq, 1e-5, A)
+        WORST.bound(group, "dq", o["dq"], dq, 1e-5, cols=A)
     if "td" in o:
-        check(group, "td_sq", o["td"], td_sq, 1e-5)
+        WORST.bound(group, "td_sq", o["td"], td_sq, 1e-5)
     if "p" in o:
-        check(group, "priority", o["p"], prio, 1e-5)
+        WORST.bound(group, "priority", o["p"], prio, 1e-5)
     if "loss" in o:
         assert abs(o["loss"][0] - loss) < 1e-5 * abs(loss), (o["loss"][0], loss)
 
@@ -201,7 +161,7 @@ def test_critic_l1_two_segments(nv, O, A, N, route):
     run_routed(f"critic l1 O={O} A={A} N={N}", route, lambda: gemm(
         nv, NT, M, N, O, ptr(d_obs), O, ptr(d_w1), I, ptr(C), N, A2=ptr(d_act), lda2=A, B2=ptr(d_w1, O), ldb2=I, K2=A,
         bias=ptr(d_b1), epi=EPI_TANH))
-    check("critic_l1", "z1", C.cpu().numpy(), ref, GEMM_TOL)
+    WORST.bound("critic_l1", "z1", C.cpu().numpy(), ref, GEMM_TOL)
 
 
 HEAD_A = (8, 9, 16, 17, 24, 25, 32, 33, 64)
@@ -234,7 +194,7 @@ def test_head_forward(nv, A, H, epi, route):
     C = torch.full((M, A), float("nan"), device="cuda")
     run_routed(f"head A={A} H={H} epi={epi}", route, lambda: gemm(
         nv, NT, M, A, H, ptr(d_h), H, ptr(d_w3), H, ptr(C), A, bias=ptr(d_b3), epi=epi))
-    check("head", "out", C.cpu().numpy(), ref, GEMM_TOL, A)
+    WORST.bound("head", "out", C.cpu().numpy(), ref, GEMM_TOL, cols=A)
 
 
 # d_act = (d(pre-l1) W1[:, O:]) * (1 - mu^2): NN with B = W1 + O, ldb = O + A; O = 17 / 20 / 24 puts B 68 / 80 / 96 bytes
@@ -254,7 +214,7 @@ def test_d_act(nv, O, A, H, route):
     C = torch.full((M, A), float("nan"), device="cuda")
     run_routed(f"d_act O={O} A={A} H={H}", route, lambda: gemm(
         nv, NN, M, A, H, ptr(d_dp1), H, ptr(d_w1, O), I, ptr(C), A, Z=ptr(d_mu), ldz=A, epi=EPI_MUL_DTANH))
-    check("d_act", "d_act", C.cpu().numpy(), ref, GEMM_TOL, A)
+    WORST.bound("d_act", "d_act", C.cpu().numpy(), ref, GEMM_TOL, cols=A)
 
 
 def tn_route(A):
@@ -284,7 +244,7 @@ def test_weight_gradient_blocks(nv, which, A, K, route):
             gemm(nv, TN, A, H, K, ptr(a_op), A, ptr(b_op), H, ptr(C), H, split=split)
         run_routed(f"dW3 A={A} K={K}", route, run)
         got = C.cpu().numpy().astype(np.float64) - C0
-        check("dW3", "dW3", got.T, ref.T, GEMM_TOL, A)                # per action row
+        WORST.bound("dW3", "dW3", got.T, ref.T, GEMM_TOL, cols=A)          # per action row
     else:
         z1 = rng.standard_normal((K, H)).astype(np.float32)
         act = rng.uniform(-1, 1, (K, A)).astype(np.float32)
@@ -299,7 +259,7 @@ def test_weight_gradient_blocks(nv, which, A, K, route):
         run_routed(f"dW1 action block A={A} K={K}", route, run)
         out = C.cpu().numpy()
         assert np.array_equal(out[:, :O], C0[:, :O]), "the obs columns of dW1 were written"
-        check("dW1_act", "dW1[:, O:]", out[:, O:].astype(np.float64) - C0[:, O:], ref, GEMM_TOL, A)
+        WORST.bound("dW1_act", "dW1[:, O:]", out[:, O:].astype(np.float64) - C0[:, O:], ref, GEMM_TOL, cols=A)
 
 
 # ------------------------------------------------------------------------------------------------ 3. learner vs port
@@ -333,9 +293,8 @@ def check_learner(group, eng, eng_mod, ref, O, A):
             gv, wv = action_views(got, O, A), action_views(want, O, A)
             for k in wv:
                 errs[f"{net}_{ref_key}/{k} per column"] = (0.0, col_err(gv[k], wv[k], A))
-    w = WORST[group]
-    w[0] = max([w[0]] + [r for r, _ in errs.values()])
-    w[1] = max([w[1]] + [c for _, c in errs.values()])
+    WORST.note(f"{group} rel_l2", *(r for r, _ in errs.values()))
+    WORST.note(f"{group} col_err", *(c for _, c in errs.values()))
     return {k: v for k, v in errs.items() if not (v[0] < LEARNER_TOL and v[1] < LEARNER_TOL)}
 
 
@@ -398,18 +357,6 @@ def test_weighted_learner_iteration_column_kernel(eng_mod):
 
 
 # ------------------------------------------------------------------------------------------------ 4. replay / actor side
-def make_episode(rng, cfg, E):
-    n_rows = E + cfg.n_step
-    obs = rng.standard_normal((n_rows, cfg.obs)).astype(np.float32)
-    act = rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32)
-    rew = rng.standard_normal(n_rows).astype(np.float32)
-    term = np.zeros(n_rows, np.float32)
-    obs[E:], act[E:], rew[E:], term[E:] = 0, 0, 0, 1
-    states = (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32)
-    prio = rng.uniform(0.01, 1.0, E - (cfg.burn_in + cfg.learning)).astype(np.float32)
-    return obs, act, rew, term, states, prio
-
-
 @pytest.mark.parametrize("A", [25, 32, 64])
 def test_replay_gather_wide_action_rows(eng_mod, A):
     """A % 4 == 0 moves the action rows as float4, A = 25 element by element: both bit-exact."""
@@ -420,7 +367,7 @@ def test_replay_gather_wide_action_rows(eng_mod, A):
     oracle = SumTreeOracle(cap)
     eps, row = [], 0
     for E in rng.integers(20, 200, size=60):
-        ep = make_episode(rng, cfg, int(E))
+        ep = episode(rng, cfg, int(E), zero_pad=True)
         rp.add_episode(*ep)
         oracle.set_range(row, ep[5])
         oracle.set_range(row + len(ep[5]), None, ep[0].shape[0] - len(ep[5]))
@@ -447,26 +394,11 @@ def test_replay_gather_wide_action_rows(eng_mod, A):
     eng.close()
 
 
-NETS = ("actor", "target_actor", "critic", "target_critic")
-
-
-def _params(O, A, H, seed):
-    rng = np.random.default_rng(seed)
-    out = {}
-    for k, name in enumerate(NETS):
-        I = O + (A if k >= 2 else 0)
-        u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.sqrt(fan)  # noqa: E731
-        out[name] = {"l1.weight": u((H, I), I), "l1.bias": u(H, I), "l2.weight_ih": u((4 * H, H), H),
-                     "l2.weight_hh": u((4 * H, H), H), "l2.bias_ih": u(4 * H, H), "l2.bias_hh": u(4 * H, H),
-                     "l3.weight": u((A, H), H), "l3.bias": u(A, H)}
-    return out
-
-
 def test_actor_priorities_38_actions():
     """Actor-side n-step sums and initial priorities at A = 38, episodes of different lengths in one batch."""
     from r2d2_b200 import actor_priority as ap
     O, A, H, Bn, L, n, gamma = 24, 38, 64, 20, 40, 5, 0.997
-    nets = _params(O, A, H, seed=38)
+    nets = policy_params(O, A, H, seed=38)
     rng = np.random.default_rng(38)
     episodes = []
     for E in (60, 61, 77, 103, 150):
@@ -488,21 +420,6 @@ def test_actor_priorities_38_actions():
             assert rel_l2(p, want_p) < 1e-3, rel_l2(p, want_p)
 
 
-def _oracle_step(P, obs, state):
-    """Actor.run's step in float64 (P: float64 weights): state [4,2,N,H] before -> (mu, state after)."""
-    new = np.empty_like(state)
-
-    def run(k, x, critic):
-        sv = lo.net_forward(P[NETS[k]], x[None], state[k, 0], state[k, 1], critic=critic)
-        new[k, 0], new[k, 1] = sv["hs"][1], sv["cs"][1]
-        return sv["out"][0]
-    mu = run(0, obs, False)
-    mu_t = run(1, obs, False)
-    run(2, np.concatenate((obs, mu), 1), True)
-    run(3, np.concatenate((obs, mu_t), 1), True)
-    return mu, new
-
-
 # N = 17 leaves a 16-lane tile with a single lane; A = 64 is the documented maximum
 POLICY_CASES = [(A, N, H) for A in (25, 33, 64) for N in (1, 17, 256) for H in (64, 256)]
 
@@ -511,7 +428,7 @@ POLICY_CASES = [(A, N, H) for A in (25, 33, 64) for N in (1, 17, 256) for H in (
 def test_policy_step_wide(A, N, H):
     from r2d2_b200.policy_step import PolicyStepper
     O = 11
-    md = _params(O, A, H, seed=A * 100 + N + H)
+    md = policy_params(O, A, H, seed=A * 100 + N + H)
     st = PolicyStepper(O, A, H, N, device="cuda", max_episode_steps=64)
     st.load(md)
     P = {n: {k: v.astype(np.float64) for k, v in md[n].items()} for n in NETS}
@@ -525,19 +442,19 @@ def test_policy_step_wide(A, N, H):
             ref[:, :, lanes] = 0
         obs = rng.standard_normal((N, O)).astype(np.float32)
         mu = st.step(obs)
-        mu_ref, ref = _oracle_step(P, obs.astype(np.float64), ref)
+        mu_ref, ref = actor_oracle.policy_step(P, obs.astype(np.float64), ref)
         got = st.current_states().cpu().numpy()
-        check("policy", f"mu step {s}", mu, mu_ref, 2e-5, A)
+        WORST.bound("policy", f"mu step {s}", mu, mu_ref, 2e-5, cols=A)
         for k, name in enumerate(NETS):
-            check("policy", f"{name}.h step {s}", got[k, 0], ref[k, 0], 2e-5)
-            check("policy", f"{name}.c step {s}", got[k, 1], ref[k, 1], 2e-5)
+            WORST.bound("policy", f"{name}.h step {s}", got[k, 0], ref[k, 0], 2e-5)
+            WORST.bound("policy", f"{name}.c step {s}", got[k, 1], ref[k, 1], 2e-5)
 
 
 def test_policy_lanes_bitwise_independent_64_actions():
     from r2d2_b200.policy_step import PolicyStepper, policy_step
     O, A, H, N = 11, 64, 128, 33
     st = PolicyStepper(O, A, H, 1, device="cuda")
-    st.load(_params(O, A, H, seed=64))
+    st.load(policy_params(O, A, H, seed=64))
     g = torch.Generator(device="cuda").manual_seed(0)
     obs = torch.randn((N, O), device="cuda", generator=g)
     s_in = 0.5 * torch.randn((4, 2, N, H), device="cuda", generator=g)

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 import exploration_oracle as xo
-from test_gpu_policy_step import _params
+from oracle.actor_oracle import policy_params
 
 pytestmark = pytest.mark.gpu
 
@@ -20,7 +20,7 @@ O = 24
 def _stepper(A, H, N, seed, max_episode_steps=4):
     from r2d2_b200.policy_step import PolicyStepper
     st = PolicyStepper(O, A, H, N, device="cuda", max_episode_steps=max_episode_steps)
-    st.load(_params(O, A, H, seed))
+    st.load(policy_params(O, A, H, seed))
     return st
 
 
@@ -193,7 +193,7 @@ def test_policy_stepper_matches_models_stepper(mode):
     from actor_pool import ModelsStepper
     from r2d2_b200.exploration import Exploration
     A, H, N = 6, 128, 16
-    md = {k: {n: torch.from_numpy(v) for n, v in sd.items()} for k, sd in _params(O, A, H, seed=8).items()}
+    md = {k: {n: torch.from_numpy(v) for n, v in sd.items()} for k, sd in policy_params(O, A, H, seed=8).items()}
     ids = list(range(N))[::-1]
     opt = Exploration(mode, 0.3, 0.05, N, seed=1)
     gpu = _stepper(A, H, N, seed=8, max_episode_steps=64)

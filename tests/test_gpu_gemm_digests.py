@@ -16,6 +16,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from conftest import GOLDEN  # noqa: E402
+from kernel_harness import nv  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 
@@ -122,13 +123,6 @@ def digests(nv):
         z1, gin, img, _ = run_net_case(nv, name)
         out[name] = {"z1": _sha(z1), "gin": _sha(gin), "z1_image": _sha(img)}
     return out
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    native.lib()
-    return native
 
 
 @pytest.fixture(scope="module")

@@ -20,21 +20,20 @@ checked here.  Run with -s for the switch points, the (H, NB) cells and routes s
 import ctypes
 import json
 import math
-import os
-import subprocess
-import sys
-import tempfile
-from collections import defaultdict
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_l2
-from learner_harness import col_err, tile_err, unit_group_err
+from kernel_harness import WorstLog, dev, f64, make_params, scan_status, smem_optin
+from kernel_harness import nv_routes as nv  # noqa: F401
+from learner_harness import col_err
 from oracle import learner_oracle as lo
 from oracle import ref_port
-from route_check import ROUTE_KERNELS, RouteLog, ran, template_args
+from oracle import actor_oracle
+from oracle.actor_oracle import NETS, policy_params
+from route_check import ROUTE_KERNELS, RouteLog, observe_in_fresh_process, ran, template_args
 
 pytestmark = pytest.mark.gpu
 
@@ -50,57 +49,19 @@ B_MAX = 1 << 17          # bisection ceiling: far beyond any tile switch of an H
 
 ROUTES = RouteLog()      # asserted routes, reported
 PROBES = RouteLog()      # bisection probes, in the route process
-WORST = defaultdict(float)
+WORST = WorstLog()
 CELLS = {d: set() for d in DIRS}
 
 
 @pytest.fixture(scope="module", autouse=True)
 def report():
     yield
-    print("\nworst errors per group:")
-    for g, e in sorted(WORST.items()):
-        print(f"  {g:34s} {e:.2e}")
+    WORST.report()
     for d in DIRS:
         print(f"{d} (H, NB) cells run: {sorted(CELLS[d])}")
         missing = sorted(set(INSTANCES) - CELLS[d])
         print(f"{d} instantiations not run: {missing if missing else 'none'}")
     ROUTES.report()
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    lib = native.lib()
-    assert lib.r2d2_get_gemm_impl() == 1, "these routes are the default implementation's"
-    lib.r2d2_set_scan_impl(1)
-    return native
-
-
-def dev(a):
-    return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).cuda()
-
-
-def f64(a):
-    return np.asarray(a, np.float32).astype(np.float64)
-
-
-def bound(group, name, x, ref, tol, NB=None, H=None, unit_axis=-1):
-    """rel_l2 < tol; with NB also the worst batch tile (axis -2), with H also the worst 32-unit group."""
-    errs = {"rel_l2": rel_l2(x, ref)}
-    if NB:
-        errs["tile_err"] = tile_err(x, ref, NB)
-    if H:
-        errs["unit_group_err"] = unit_group_err(x, ref, H, unit_axis)
-    for k, e in errs.items():
-        WORST[f"{group} {k}"] = max(WORST[f"{group} {k}"], e)
-    bad = {k: f"{e:.3e}" for k, e in errs.items() if not e < tol}
-    assert not bad, f"{name}: {bad} (bound {tol:.0e})"
-
-
-def scan_status(nv):
-    status = ctypes.c_int(0)
-    nv.check(nv.lib().r2d2_scan_status(ctypes.byref(status), nv.current_stream()))
-    return status.value
 
 
 # ------------------------------------------------------------------------------------------------ 1. cluster scans
@@ -239,7 +200,7 @@ def run_scan_chain(nv, direction, H, B, NB, T, repeat, state, hfs):
     got = runs[0]
     for k, tol in (("hs", TOL_FWD), ("cs", TOL_FWD), ("gates", TOL_FWD), ("head_in", TOL_FWD), ("dgates", TOL_BWD),
                    ("dgin", TOL_BWD)):
-        bound(f"scan {k}", f"H={H} B={B} NB={NB} repeat={repeat} {k}", got[k], ref[k], tol, NB=NB, H=H)
+        WORST.bound(f"scan {k}", f"H={H} B={B} NB={NB} repeat={repeat} {k}", got[k], ref[k], tol, tile=NB, H=H)
 
 
 SCAN_CASES = [(d, H, NB, where) for d in DIRS for (H, NB) in INSTANCES for where in ("first", "ragged")]
@@ -282,15 +243,6 @@ def per_step_launches(nv, H, B):
     buf = ScanBuffers(T, B, H, 1, fill=0.0)
     return {f"per-step fwd H={H} B={B}": lambda: buf.forward(nv, gin, whh, None, None),
             f"per-step bwd H={H} B={B}": lambda: buf.backward(nv, whh, dh, 0)}
-
-
-def make_params(rng, O, A, H, critic):
-    I = O + (A if critic else 0)
-    u = lambda shp, b: rng.uniform(-b, b, shp)  # noqa: E731
-    return {"l1.weight": u((H, I), 1 / np.sqrt(I)), "l1.bias": u((H,), 0.2),
-            "l2.weight_ih": u((4 * H, H), 2 / np.sqrt(4 * H)), "l2.weight_hh": u((4 * H, H), 2 / np.sqrt(4 * H)),
-            "l2.bias_ih": u((4 * H,), 0.1), "l2.bias_hh": u((4 * H,), 0.1),
-            "l3.weight": u((A, H), 1 / np.sqrt(H)), "l3.bias": u((A,), 0.1)}
 
 
 UNIT_AXIS = {"l1.weight": 0, "l1.bias": 0, "l2.weight_ih": 0, "l2.weight_hh": 0, "l2.bias_ih": 0, "l2.bias_hh": 0,
@@ -338,24 +290,20 @@ def test_net_per_step_path(nv, routes, H, O, A, B, T, repeat, critic, first_row)
                                         nv.dptr(grads), nv.dptr(d_act), nv.dptr(ws), nv.current_stream()))
     torch.cuda.synchronize()
     case = f"H={H} B={B} {'critic' if critic else 'actor'}"
-    bound("per-step out", f"{case} out", out.cpu().numpy(), out_ref, TOL_FWD)
+    WORST.bound("per-step out", f"{case} out", out.cpu().numpy(), out_ref, TOL_FWD)
     if critic:
-        bound("per-step d_act", f"{case} d_act", d_act.cpu().numpy(), dx_ref[:, :, O:], TOL_BWD)
+        WORST.bound("per-step d_act", f"{case} d_act", d_act.cpu().numpy(), dx_ref[:, :, O:], TOL_BWD)
     g = grads.cpu().numpy()
     off = 0
     for k in lo.PARAM_KEYS:
         n = g_ref[k].size
         ax = UNIT_AXIS[k]
-        bound(f"per-step grad {k}", f"{case} grad {k}", g[off:off + n].reshape(g_ref[k].shape), g_ref[k], TOL_BWD,
+        WORST.bound(f"per-step grad {k}", f"{case} grad {k}", g[off:off + n].reshape(g_ref[k].shape), g_ref[k], TOL_BWD,
               H=H if ax is not None else None, unit_axis=ax if ax is not None else -1)
         off += n
 
 
 # ------------------------------------------------------------------------------------------------ 3. heads at K = H
-def smem_optin():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).shared_memory_per_block_optin
-
-
 def wide_k_route(N, K):
     """thin_smalln_kernel keeps a [NP][ceil(K / 128) 128] fp32 weight tile in shared memory; a product whose tile
     does not fit the opt-in limit goes to the single-launch mma.sync kernel (N < 32) or to wgmma (N = 32)."""
@@ -400,9 +348,9 @@ def test_head_wide_k(nv, routes, N, K, epi):
     d_h, d_w3, d_b3 = dev(h), dev(W3), dev(b3)
     head_launch(nv, N, K, epi, d_h, d_w3, d_b3, C)()
     got = C.cpu().numpy()
-    bound("head", f"head N={N} K={K}", got, ref, TOL_GEMM)
+    WORST.bound("head", f"head N={N} K={K}", got, ref, TOL_GEMM)
     c = col_err(got, ref, N)
-    WORST["head col_err"] = max(WORST["head col_err"], c)
+    WORST.note("head col_err", c)
     assert c < TOL_GEMM, f"head N={N} K={K}: col_err {c:.3e}"
 
 
@@ -422,9 +370,9 @@ def test_d_act_wide_k(nv, routes, N, K):
     d_dp1, d_w1, d_mu = dev(dp1), dev(W1), dev(mu)
     d_act_launch(nv, N, K, d_dp1, d_w1, d_mu, C)()
     got = C.cpu().numpy()
-    bound("d_act", f"d_act N={N} K={K}", got, ref, TOL_GEMM)
+    WORST.bound("d_act", f"d_act N={N} K={K}", got, ref, TOL_GEMM)
     c = col_err(got, ref, N)
-    WORST["d_act col_err"] = max(WORST["d_act col_err"], c)
+    WORST.note("d_act col_err", c)
     assert c < TOL_GEMM, f"d_act N={N} K={K}: col_err {c:.3e}"
 
 
@@ -475,43 +423,13 @@ def test_learner_against_port(obs, act, hidden, batch):
                 gv, wv = _action_views(got, obs, act), _action_views(want, obs, act)
                 for k in wv:
                     errs[f"{net}_{ref_key}/{k} per column"] = col_err(gv[k], wv[k], act)
-        WORST["learner"] = max([WORST["learner"]] + list(errs.values()))
+        WORST.note("learner", *errs.values())
         bad = {k: f"{v:.2e}" for k, v in errs.items() if not v < TOL_LEARNER}
         assert not bad, f"iteration {it}: {bad}"
     eng.close()
 
 
 # ------------------------------------------------------------------------------------------------ 4. policy step
-NETS = ("actor", "target_actor", "critic", "target_critic")
-
-
-def _policy_params(O, A, H, seed):
-    rng = np.random.default_rng(seed)
-    out = {}
-    for k, name in enumerate(NETS):
-        I = O + (A if k >= 2 else 0)
-        u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.sqrt(fan)  # noqa: E731
-        out[name] = {"l1.weight": u((H, I), I), "l1.bias": u(H, I), "l2.weight_ih": u((4 * H, H), H),
-                     "l2.weight_hh": u((4 * H, H), H), "l2.bias_ih": u(4 * H, H), "l2.bias_hh": u(4 * H, H),
-                     "l3.weight": u((A, H), H), "l3.bias": u(A, H)}
-    return out
-
-
-def _oracle_step(P, obs, state):
-    """Actor.run's step in float64 (P: float64 weights): state [4,2,N,H] before -> (mu, state after)."""
-    new = np.empty_like(state)
-
-    def run(k, x, critic):
-        sv = lo.net_forward(P[NETS[k]], x[None], state[k, 0], state[k, 1], critic=critic)
-        new[k, 0], new[k, 1] = sv["hs"][1], sv["cs"][1]
-        return sv["out"][0]
-    mu = run(0, obs, False)
-    mu_t = run(1, obs, False)
-    run(2, np.concatenate((obs, mu), 1), True)
-    run(3, np.concatenate((obs, mu_t), 1), True)
-    return mu, new
-
-
 # every H with every O; across the three O of an H, each A and each N once (O = 513 / 1100: two / three KC = 512
 # chunks of the staged l1 input)
 POLICY_H, POLICY_O, POLICY_A, POLICY_N = (96, 160, 384, 480), (11, 513, 1100), (1, 6, 17), (1, 17, 256)
@@ -522,7 +440,7 @@ POLICY_CASES = [(H, O, POLICY_A[(i + j) % 3], POLICY_N[(i + 2 * j) % 3])
 @pytest.mark.parametrize("H,O,A,N", POLICY_CASES)
 def test_policy_step_hidden(routes, H, O, A, N):
     from r2d2_b200.policy_step import PolicyStepper
-    md = _policy_params(O, A, H, seed=H * 100 + O + N)
+    md = policy_params(O, A, H, seed=H * 100 + O + N)
     st = PolicyStepper(O, A, H, N, device="cuda", max_episode_steps=64)
     st.load(md)
     P = {n: {k: v.astype(np.float64) for k, v in md[n].items()} for n in NETS}
@@ -540,19 +458,19 @@ def test_policy_step_hidden(routes, H, O, A, N):
             ref[:, :, lanes] = 0
         obs = rng.standard_normal((N, O)).astype(np.float32)
         mu = st.step(obs)
-        mu_ref, ref = _oracle_step(P, obs.astype(np.float64), ref)
+        mu_ref, ref = actor_oracle.policy_step(P, obs.astype(np.float64), ref)
         got = st.current_states().cpu().numpy()
-        bound("policy mu", f"mu step {s}", mu, mu_ref, TOL_FWD)
+        WORST.bound("policy mu", f"mu step {s}", mu, mu_ref, TOL_FWD)
         for k, name in enumerate(NETS):
-            bound("policy h", f"{name}.h step {s}", got[k, 0], ref[k, 0], TOL_FWD)
-            bound("policy c", f"{name}.c step {s}", got[k, 1], ref[k, 1], TOL_FWD)
+            WORST.bound("policy h", f"{name}.h step {s}", got[k, 0], ref[k, 0], TOL_FWD)
+            WORST.bound("policy c", f"{name}.c step {s}", got[k, 1], ref[k, 1], TOL_FWD)
 
 
 def test_policy_lanes_bitwise_independent_h160_o1100():
     from r2d2_b200.policy_step import PolicyStepper, policy_step
     O, A, H, N = 1100, 6, 160, 33
     st = PolicyStepper(O, A, H, 1, device="cuda")
-    st.load(_policy_params(O, A, H, seed=160))
+    st.load(policy_params(O, A, H, seed=160))
     g = torch.Generator(device="cuda").manual_seed(0)
     obs = torch.randn((N, O), device="cuda", generator=g)
     s_in = 0.5 * torch.randn((4, 2, N, H), device="cuda", generator=g)
@@ -629,16 +547,7 @@ def route_child(out_path):
 def routes(nv):
     """{case: route kernels that ran} and "switch": {(direction, H): {NB: first B}}, observed in a fresh Python process
     (route_child).  Prints the switch points."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "routes.json")
-        code = ("import sys; sys.path[:0] = %r; import test_gpu_hidden_size as t; t.route_child(%r)"
-                % ([here, root, os.path.join(root, "pytorch-r2d2-dpg_b200")], out))
-        res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=1200, cwd=root)
-        assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-        with open(out) as f:
-            got = json.load(f)
+    got = observe_in_fresh_process("test_gpu_hidden_size", timeout=1200)
     routes = dict(got["names"])
     routes["switch"] = {(d, H): {int(nb): b for nb, b in t.items()} for d, H, t in got["switch"]}
     print(f"\nroute process: {got['probes']} bisection probes, {got['lost']} profiler sessions repeated")

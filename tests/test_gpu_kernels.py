@@ -6,22 +6,12 @@ import pytest
 import torch
 
 from conftest import rel_l2
+from kernel_harness import dev, nv, scan_status  # noqa: F401
 from oracle import learner_oracle as lo
 
 pytestmark = pytest.mark.gpu
 
 TOL = 2e-5
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    native.lib()
-    return native
-
-
-def dev(a):
-    return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).cuda()
 
 
 # ----------------------------------------------------------------------------------------------
@@ -111,6 +101,7 @@ def test_gemm(nv, gemm_impl, layout, M, N, K, K2, bias, epi, split):
 
 
 # ----------------------------------------------------------------------------------------------
+# not kernel_harness.make_params: its bounds differ (l1 by 1 / sqrt(H), l3 by 0.1)
 def make_params(rng, O, A, H, critic):
     I = O + (A if critic else 0)
     u = lambda shp, b: rng.uniform(-b, b, shp)  # noqa: E731
@@ -155,11 +146,9 @@ def scan_impl(request, nv):
     lib = nv.lib()
     lib.r2d2_set_scan_impl(1 if request.param == "tc" else 0)
     yield request.param
-    import ctypes
-    status = ctypes.c_int(0)
-    nv.check(lib.r2d2_scan_status(ctypes.byref(status), nv.current_stream()))
+    status = scan_status(nv)
     lib.r2d2_set_scan_impl(1)
-    assert status.value == 0, f"a bounded mbarrier wait timed out inside a scan kernel (code {status.value})"
+    assert status == 0, f"a bounded mbarrier wait timed out inside a scan kernel (code {status})"
 
 
 @pytest.mark.parametrize("O,A,H,B,T,repeat,critic,first_row", NET_CASES)

@@ -18,13 +18,8 @@ and the CPU port of the reference.
 Which kernel served each kernel-level case is observed under torch.profiler in one fresh process (the `routes` fixture,
 as in tests/test_gpu_hidden_size.py); the values are checked here.  Run with -s for the routes seen and the worst errors
 per group."""
-import ctypes
 import json
 import math
-import os
-import subprocess
-import sys
-import tempfile
 from collections import Counter, defaultdict
 
 import numpy as np
@@ -32,11 +27,16 @@ import pytest
 import torch
 
 from conftest import rel_l2
-from learner_harness import col_err, tile_err
+from kernel_harness import WorstLog, dev, f64, make_params, num_sms, scan_status, smem_optin
+from kernel_harness import nv_routes as nv  # noqa: F401
+from learner_harness import col_err, episode
+from oracle import actor_oracle
 from oracle import learner_oracle as lo
 from oracle import ref_port
+from oracle.actor_oracle import NETS, policy_params
 from oracle.sumtree import SumTreeOracle
-from route_check import ROUTE_KERNELS, RouteLog, parse_route, ran, template_args
+from route_check import (ROUTE_KERNELS, RouteLog, launch_counts, observe_in_fresh_process, parse_route, ran,
+                         template_args)
 
 pytestmark = pytest.mark.gpu
 
@@ -47,61 +47,20 @@ O_BUCKETS = (1, 3, 4, 31, 32, 33, 47, 63, 64, 65, 127, 376, 1101)
 SENTINEL = 0x7FC0BEEF            # a NaN bit pattern: what the z1 image region holds before the forward
 
 ROUTES = RouteLog()
-WORST = defaultdict(float)
+WORST = WorstLog()
 SEEN = defaultdict(set)          # product -> routes asserted
 
 
 @pytest.fixture(scope="module", autouse=True)
 def report():
     yield
-    print("\nworst errors per group:")
-    for g, e in sorted(WORST.items()):
-        print(f"  {g:34s} {e:.2e}")
+    WORST.report()
     for prod, routes in sorted(SEEN.items()):
         print(f"{prod} routes asserted: {sorted(routes)}")
     ROUTES.report()
 
 
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    lib = native.lib()
-    assert lib.r2d2_get_gemm_impl() == 1, "these routes are the default implementation's"
-    lib.r2d2_set_scan_impl(1)
-    return native
-
-
-def dev(a):
-    return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).cuda()
-
-
-def f64(a):
-    return np.asarray(a, np.float32).astype(np.float64)
-
-
-def bound(group, name, x, ref, tol, cols=None, row_tile=None):
-    """rel_l2 < tol; with `cols` also the worst of `cols` columns (col_err), with `row_tile` the worst tile of that many
-    rows along axis 0."""
-    errs = {"rel_l2": rel_l2(x, ref)}
-    if cols:
-        errs["col_err"] = col_err(x, ref, cols)
-    if row_tile:
-        errs["tile_err"] = tile_err(x, ref, row_tile, axis=0)
-    for k, e in errs.items():
-        WORST[f"{group} {k}"] = max(WORST[f"{group} {k}"], e)
-    bad = {k: f"{e:.3e}" for k, e in errs.items() if not e < tol}
-    assert not bad, f"{name}: {bad} (bound {tol:.0e})"
-
-
 # ------------------------------------------------------------------------------------------------ expected routes
-def num_sms():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def smem_optin():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).shared_memory_per_block_optin
-
-
 def split_k(M, N, K):
     """gemm_suggest_split_k in the default mode (gemm.cu:280-292, gemm_tc.cu:295-305)."""
     skinny = K < 64 or N < 32 or M < 32
@@ -167,19 +126,10 @@ def test_actor_l1(nv, routes, O, M, N):
     SEEN["actor l1"].add(route)
     C = torch.full((M, N), float("nan"), device="cuda")
     l1_launch(nv, M, N, O, dev(obs), dev(W1), dev(b1), C)()
-    bound("l1", case, C.cpu().numpy(), ref, TOL_GEMM, row_tile=128)
+    WORST.bound("l1", case, C.cpu().numpy(), ref, TOL_GEMM, tile=128, tile_axis=0)
 
 
 # ------------------------------------------------------------------------------------------------ 2. chains
-def make_params(rng, O, A, H, critic):
-    I = O + (A if critic else 0)
-    u = lambda shp, b: rng.uniform(-b, b, shp)  # noqa: E731
-    return {"l1.weight": u((H, I), 1 / np.sqrt(I)), "l1.bias": u((H,), 0.2),
-            "l2.weight_ih": u((4 * H, H), 2 / np.sqrt(4 * H)), "l2.weight_hh": u((4 * H, H), 2 / np.sqrt(4 * H)),
-            "l2.bias_ih": u((4 * H,), 0.1), "l2.bias_hh": u((4 * H,), 0.1),
-            "l3.weight": u((A, H), 1 / np.sqrt(H)), "l3.bias": u((A,), 0.1)}
-
-
 class Chain:
     """Device buffers of one r2d2_lstm_net_forward / _backward call (repeat 1, head from row 0).  The z1 image region
     (the workspace's last sub-buffer, ChainWs::carve) starts as SENTINEL words, the rest of the workspace as zeros."""
@@ -316,25 +266,25 @@ def test_chain(nv, routes, O, A, H, critic, T, B):
     img = ch.img.cpu().numpy()
     ch.backward()
     torch.cuda.synchronize()
-    status = ctypes.c_int(0)
-    nv.check(nv.lib().r2d2_scan_status(ctypes.byref(status), nv.current_stream()))
-    assert status.value == 0, f"{case}: a bounded hand-off wait expired inside a scan kernel"
+    assert scan_status(nv) == 0, f"{case}: a bounded hand-off wait expired inside a scan kernel"
 
-    bound("chain z1", f"{case} z1", z1, sv["z1"].reshape(M, H), TOL_FWD)
-    bound("chain out", f"{case} out", ch.out.cpu().numpy(), sv["out"], TOL_FWD)
+    WORST.bound("chain z1", f"{case} z1", z1, sv["z1"].reshape(M, H), TOL_FWD)
+    WORST.bound("chain out", f"{case} out", ch.out.cpu().numpy(), sv["out"], TOL_FWD)
     if critic:
-        bound("chain d_act", f"{case} d_act", ch.d_act.cpu().numpy(), dx_ref[:, :, O:], TOL_BWD, cols=A)
+        WORST.bound("chain d_act", f"{case} d_act", ch.d_act.cpu().numpy(), dx_ref[:, :, O:], TOL_BWD, cols=A)
     g, off = ch.grads.cpu().numpy(), 0
     for k in lo.PARAM_KEYS:
         n = g_ref[k].size
         got, want = g[off:off + n].reshape(g_ref[k].shape), g_ref[k]
         off += n
         if k == "l1.weight":
-            bound("chain dW1 obs block", f"{case} grad l1.weight[:, :O]", got[:, :O], want[:, :O], TOL_BWD, cols=O)
+            WORST.bound("chain dW1 obs block", f"{case} grad l1.weight[:, :O]", got[:, :O], want[:, :O], TOL_BWD,
+                        cols=O)
             if critic:
-                bound("chain dW1 act block", f"{case} grad l1.weight[:, O:]", got[:, O:], want[:, O:], TOL_BWD, cols=A)
+                WORST.bound("chain dW1 act block", f"{case} grad l1.weight[:, O:]", got[:, O:], want[:, O:], TOL_BWD,
+                            cols=A)
         else:
-            bound(f"chain grad {k}", f"{case} grad {k}", got, want, TOL_BWD)
+            WORST.bound(f"chain grad {k}", f"{case} grad {k}", got, want, TOL_BWD)
 
     # 3. the z1 operand image (the critic's l1 has two K segments: its image follows the same rule at K = O + A)
     K1 = O + (A if critic else 0)
@@ -395,25 +345,13 @@ def test_learner_against_port(obs, act, hidden, batch):
                 gv, wv = _obs_views(got, obs), _obs_views(want, obs)
                 for k in wv:
                     errs[f"{net}_{ref_key}/{k} per column"] = col_err(gv[k], wv[k], obs)
-        WORST["learner"] = max([WORST["learner"]] + list(errs.values()))
+        WORST.note("learner", *errs.values())
         bad = {k: f"{v:.2e}" for k, v in errs.items() if not v < TOL_LEARNER}
         assert not bad, f"iteration {it}: {bad}"
     eng.close()
 
 
 # ------------------------------------------------------------------------------------------------ 5. replay gather
-def make_episode(rng, cfg, E):
-    n_rows = E + cfg.n_step
-    obs = rng.standard_normal((n_rows, cfg.obs)).astype(np.float32)
-    act = rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32)
-    rew = rng.standard_normal(n_rows).astype(np.float32)
-    term = np.zeros(n_rows, np.float32)
-    obs[E:], act[E:], rew[E:], term[E:] = 0, 0, 0, 1
-    states = (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32)
-    prio = rng.uniform(0.01, 1.0, E - (cfg.burn_in + cfg.learning)).astype(np.float32)
-    return obs, act, rew, term, states, prio
-
-
 def assert_window(got, ep, s, rows, what):
     """Slot column `got` (obs, act, rew, term [rows, ...] and states [4, 2, H]) against episode `ep` from row s."""
     obs, act, rew, term, states = got
@@ -435,7 +373,7 @@ def test_replay_gather_obs_rows(O):
     oracle = SumTreeOracle(cap)
     eps, row = [], 0
     for n in rng.integers(20, 200, size=50):
-        ep = make_episode(rng, cfg, int(n))
+        ep = episode(rng, cfg, int(n), zero_pad=True)
         rp.add_episode(*ep)
         oracle.set_range(row, ep[5])
         oracle.set_range(row + len(ep[5]), None, ep[0].shape[0] - len(ep[5]))
@@ -498,36 +436,6 @@ def test_global_gather_obs_rows(O):
 
 
 # ------------------------------------------------------------------------------------------------ 6. policy step
-NETS = ("actor", "target_actor", "critic", "target_critic")
-
-
-def _policy_params(O, A, H, seed):
-    rng = np.random.default_rng(seed)
-    out = {}
-    for k, name in enumerate(NETS):
-        I = O + (A if k >= 2 else 0)
-        u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.sqrt(fan)  # noqa: E731
-        out[name] = {"l1.weight": u((H, I), I), "l1.bias": u(H, I), "l2.weight_ih": u((4 * H, H), H),
-                     "l2.weight_hh": u((4 * H, H), H), "l2.bias_ih": u(4 * H, H), "l2.bias_hh": u(4 * H, H),
-                     "l3.weight": u((A, H), H), "l3.bias": u(A, H)}
-    return out
-
-
-def _oracle_step(P, obs, state):
-    """Actor.run's step in float64 (P: float64 weights): state [4,2,N,H] before -> (mu, state after)."""
-    new = np.empty_like(state)
-
-    def run(k, x, critic):
-        sv = lo.net_forward(P[NETS[k]], x[None], state[k, 0], state[k, 1], critic=critic)
-        new[k, 0], new[k, 1] = sv["hs"][1], sv["cs"][1]
-        return sv["out"][0]
-    mu = run(0, obs, False)
-    mu_t = run(1, obs, False)
-    run(2, np.concatenate((obs, mu), 1), True)
-    run(3, np.concatenate((obs, mu_t), 1), True)
-    return mu, new
-
-
 # O = 1: a one-wide staged chunk; O = 512: exactly one full 512-wide chunk of the staged l1 input (policy.cu:116-119)
 POLICY_CASES = [(O, 3, 64, 17) for O in (1, 4, 512)]
 
@@ -539,7 +447,7 @@ def test_policy_step_obs(routes, O, A, H, N):
     ROUTES.assert_route(case, "policy", routes[case])
     missing = [p for p in range(1, 6) if not ran(routes[case], ROUTE_KERNELS["policy"], (p,))]
     assert not missing, f"policy phases {missing} did not run: {routes[case]}"
-    md = _policy_params(O, A, H, seed=O * 100 + N)
+    md = policy_params(O, A, H, seed=O * 100 + N)
     st = PolicyStepper(O, A, H, N, device="cuda", max_episode_steps=64)
     st.load(md)
     P = {n: {k: v.astype(np.float64) for k, v in md[n].items()} for n in NETS}
@@ -553,40 +461,15 @@ def test_policy_step_obs(routes, O, A, H, N):
             ref[:, :, lanes] = 0
         obs = rng.standard_normal((N, O)).astype(np.float32)
         mu = st.step(obs)
-        mu_ref, ref = _oracle_step(P, obs.astype(np.float64), ref)
+        mu_ref, ref = actor_oracle.policy_step(P, obs.astype(np.float64), ref)
         got = st.current_states().cpu().numpy()
-        bound("policy mu", f"O={O} mu step {s}", mu, mu_ref, TOL_FWD, cols=A)
+        WORST.bound("policy mu", f"O={O} mu step {s}", mu, mu_ref, TOL_FWD, cols=A)
         for k, name in enumerate(NETS):
-            bound("policy h", f"O={O} {name}.h step {s}", got[k, 0], ref[k, 0], TOL_FWD)
-            bound("policy c", f"O={O} {name}.c step {s}", got[k, 1], ref[k, 1], TOL_FWD)
+            WORST.bound("policy h", f"O={O} {name}.h step {s}", got[k, 0], ref[k, 0], TOL_FWD)
+            WORST.bound("policy c", f"O={O} {name}.c step {s}", got[k, 1], ref[k, 1], TOL_FWD)
 
 
 # ------------------------------------------------------------------------------------------------ route observation
-def launch_counts(case, fn, agree=False):
-    """{profiler name of a route kernel: launches} of fn under the CUDA profiler; a session that recorded no route kernel
-    at all is repeated after a growing pause (RouteLog.profile), five sessions in all.  agree: the launch counts are
-    asserted exactly, so a session that kept only part of the kernels it ran must not be taken: sessions repeat until two
-    in a row record the same counts (at most six)."""
-    import time
-    from torch.autograd import DeviceType
-    from torch.profiler import ProfilerActivity, profile
-    prev = None
-    for pause in (0.1, 0.3, 1.0, 3.0, 3.0, None):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        c = dict(Counter(e.name for e in prof.events()
-                         if e.device_type == DeviceType.CUDA and any(b in e.name for b in ROUTE_KERNELS.values())))
-        if c and (not agree or c == prev):
-            return c
-        prev = c or None
-        if pause is not None:
-            time.sleep(pause)
-    assert c, f"{case}: the profiler recorded no route kernel in six sessions"
-    raise AssertionError(f"{case}: no two profiler sessions in a row recorded the same launches")
-
-
 def policy_launch(O, A, H, N):
     from r2d2_b200.policy_step import PolicyStepper, policy_step
     st = PolicyStepper(O, A, H, N, device="cuda", max_episode_steps=1)
@@ -617,13 +500,4 @@ def route_child(out_path):
 @pytest.fixture(scope="module")
 def routes(nv):
     """{case: {route kernel: launches}} observed in a fresh Python process (route_child)."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "routes.json")
-        code = ("import sys; sys.path[:0] = %r; import test_gpu_obs_width as t; t.route_child(%r)"
-                % ([here, root, os.path.join(root, "pytorch-r2d2-dpg_b200")], out))
-        res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=1200, cwd=root)
-        assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-        with open(out) as f:
-            return json.load(f)
+    return observe_in_fresh_process("test_gpu_obs_width", timeout=1200)

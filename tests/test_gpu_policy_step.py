@@ -1,5 +1,5 @@
-"""r2d2_policy_step and ActorPool on the GPU: the step kernels against a float64 oracle built from
-oracle/learner_oracle.net_forward the way Actor.run calls the nets, lane independence bit for bit, shape errors, and
+"""r2d2_policy_step and ActorPool on the GPU: the step kernels against the float64 policy step of
+oracle/actor_oracle, lane independence bit for bit, shape errors, and
 the pool end to end (files the drop-in nets reproduce, priorities against oracle/actor_oracle, model.pt reload, and a
 learner that ingests the files)."""
 import os
@@ -12,39 +12,9 @@ import torch
 
 from conftest import rel_l2
 from oracle import actor_oracle
-from oracle import learner_oracle as lo
+from oracle.actor_oracle import NETS, policy_params
 
 pytestmark = pytest.mark.gpu
-
-NETS = ("actor", "target_actor", "critic", "target_critic")
-
-
-def _params(O, A, H, seed):
-    rng = np.random.default_rng(seed)
-    out = {}
-    for k, name in enumerate(NETS):
-        I = O + (A if k >= 2 else 0)
-        u = lambda shape, fan: rng.uniform(-1, 1, shape).astype(np.float32) / np.sqrt(fan)  # noqa: E731
-        out[name] = {"l1.weight": u((H, I), I), "l1.bias": u(H, I), "l2.weight_ih": u((4 * H, H), H),
-                     "l2.weight_hh": u((4 * H, H), H), "l2.bias_ih": u(4 * H, H), "l2.bias_hh": u(4 * H, H),
-                     "l3.weight": u((A, H), H), "l3.bias": u(A, H)}
-    return out
-
-
-def _oracle_step(P, obs, state):
-    """Actor.run's step in float64 (P: float64 weights): state [4,2,N,H] before -> (mu, state after)."""
-    new = np.empty_like(state)
-
-    def run(k, x, critic):
-        sv = lo.net_forward(P[NETS[k]], x[None], state[k, 0], state[k, 1], critic=critic)
-        new[k, 0], new[k, 1] = sv["hs"][1], sv["cs"][1]
-        return sv["out"][0]
-    mu = run(0, obs, False)
-    mu_t = run(1, obs, False)
-    run(2, np.concatenate((obs, mu), 1), True)
-    run(3, np.concatenate((obs, mu_t), 1), True)
-    return mu, new
-
 
 CASES = [(O, A, H, N) for (O, A, H) in ((24, 6, 128), (17, 6, 256), (376, 17, 512), (5, 1, 32))
          for N in (1, 3, 64, 256) if N < 256 or H <= 256]
@@ -53,7 +23,7 @@ CASES = [(O, A, H, N) for (O, A, H) in ((24, 6, 128), (17, 6, 256), (376, 17, 51
 @pytest.mark.parametrize("O,A,H,N", CASES)
 def test_policy_step_matches_float64_oracle(O, A, H, N):
     from r2d2_b200.policy_step import PolicyStepper
-    md = _params(O, A, H, seed=O + H + N)
+    md = policy_params(O, A, H, seed=O + H + N)
     st = PolicyStepper(O, A, H, N, device="cuda", max_episode_steps=64)
     st.load(md)
     P = {n: {k: v.astype(np.float64) for k, v in md[n].items()} for n in NETS}
@@ -67,7 +37,7 @@ def test_policy_step_matches_float64_oracle(O, A, H, N):
             ref[:, :, lanes] = 0
         obs = rng.standard_normal((N, O)).astype(np.float32)
         mu = st.step(obs)
-        mu_ref, ref = _oracle_step(P, obs.astype(np.float64), ref)
+        mu_ref, ref = actor_oracle.policy_step(P, obs.astype(np.float64), ref)
         got = st.current_states().cpu().numpy()
         errs = {"mu": rel_l2(mu, mu_ref)}
         for k, name in enumerate(NETS):
@@ -91,7 +61,7 @@ def test_lanes_are_bitwise_independent():
     from r2d2_b200.policy_step import PolicyStepper
     O, H, N = 17, 256, 64
     st = PolicyStepper(O, ACT, H, 1, device="cuda")
-    st.load(_params(O, ACT, H, seed=5))
+    st.load(policy_params(O, ACT, H, seed=5))
     g = torch.Generator(device="cuda").manual_seed(0)
     obs = torch.randn((N, O), device="cuda", generator=g)
     s_in = 0.5 * torch.randn((4, 2, N, H), device="cuda", generator=g)

@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from conftest import load_golden
+from learner_harness import episode
 from oracle.sumtree import SumTreeOracle
 
 pytestmark = pytest.mark.gpu
@@ -19,25 +20,10 @@ def eng_mod():
     return engine
 
 
-def make_episode(rng, cfg, E):
-    n_rows = E + cfg.n_step
-    obs = rng.standard_normal((n_rows, cfg.obs)).astype(np.float32)
-    act = rng.uniform(-1, 1, (n_rows, cfg.act)).astype(np.float32)
-    rew = rng.standard_normal(n_rows).astype(np.float32)
-    term = np.zeros(n_rows, np.float32)
-    obs[E:] = 0
-    act[E:] = 0
-    rew[E:] = 0
-    term[E:] = 1
-    states = (0.1 * rng.standard_normal((E, 4, 2, cfg.hidden))).astype(np.float32)
-    prio = rng.uniform(0.01, 1.0, E - (cfg.burn_in + cfg.learning)).astype(np.float32)
-    return obs, act, rew, term, states, prio
-
-
 def fill(rp, oracle, rng, cfg, lens):
     eps, row = [], 0
     for E in lens:
-        ep = make_episode(rng, cfg, E)
+        ep = episode(rng, cfg, E, zero_pad=True)
         rp.add_episode(*ep)
         n_rows = ep[0].shape[0]
         oracle.set_range(row, ep[5])
@@ -132,7 +118,7 @@ def test_fifo_eviction(eng_mod):
     live, head = [], 0
     for i in range(30):
         E = int(rng.integers(30, 120))
-        ep = make_episode(rng, cfg, E)
+        ep = episode(rng, cfg, E, zero_pad=True)
         n_rows = E + cfg.n_step
         if head + n_rows > 1000:
             head = 0

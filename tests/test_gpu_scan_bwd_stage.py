@@ -7,7 +7,6 @@ order, so the bits must not change.
 
   python tests/test_gpu_scan_bwd_stage.py --write-digests PATH   # digests of the library R2D2_B200_LIB points at
 """
-import ctypes
 import hashlib
 import json
 import os
@@ -18,6 +17,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from conftest import GOLDEN, rel_l2  # noqa: E402
+from kernel_harness import nv, scan_status  # noqa: E402,F401
 from oracle import learner_oracle as lo  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -73,19 +73,6 @@ def run_chain(nv, H, B, T, repeat, head_first_step):
 def digests(dgates, dgin):
     return {"dgates": hashlib.sha256(np.ascontiguousarray(dgates).tobytes()).hexdigest(),
             "dgin": hashlib.sha256(np.ascontiguousarray(dgin).tobytes()).hexdigest()}
-
-
-def scan_status(nv):
-    status = ctypes.c_int(0)
-    nv.check(nv.lib().r2d2_scan_status(ctypes.byref(status), nv.current_stream()))
-    return status.value
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    native.lib()
-    return native
 
 
 @pytest.fixture(scope="module")

@@ -2,13 +2,13 @@
 recurrence.  The kernels hand h_t (forward) and the dh partials (BPTT) from CTA to CTA through per-source mbarriers
 that are reused every second step, so chains of 125+ steps wrap every barrier phase many times; the batch sizes need
 several waves of clusters and leave a ragged last tile.  The same chain run twice must give the same bits."""
-import ctypes
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_l2
+from kernel_harness import nv, scan_status  # noqa: F401
 from oracle import learner_oracle as lo
 
 pytestmark = pytest.mark.gpu
@@ -22,13 +22,6 @@ CASES = [
     (512, 456, 125, 1),
     (512, 300, 64, 2),
 ]
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    native.lib()
-    return native
 
 
 @pytest.mark.parametrize("H,B,T,repeat", CASES)
@@ -60,9 +53,8 @@ def test_long_chain_matches_oracle_and_repeats_bitwise(nv, H, B, T, repeat):
                                              nv.dptr(dgates), nv.dptr(dgin), T, B, H, repeat, nv.dptr(scratch), st))
         torch.cuda.synchronize()
         runs.append((hs.cpu().numpy(), dgin.cpu().numpy()))
-    status = ctypes.c_int(0)
-    nv.check(lib.r2d2_scan_status(ctypes.byref(status), st))
-    assert status.value == 0, f"a bounded hand-off wait expired inside a scan kernel (code {status.value})"
+    status = scan_status(nv, st)
+    assert status == 0, f"a bounded hand-off wait expired inside a scan kernel (code {status})"
 
     (hs_a, dgin_a), (hs_b, dgin_b) = runs
     assert np.array_equal(hs_a, hs_b) and np.array_equal(dgin_a, dgin_b), "two runs of the same chain differ"

@@ -20,26 +20,21 @@ Every time-major output is bounded per time row (step_err) as well as over the w
 hundreds of rows dilutes an error confined to one step.  Which kernel served each case is observed under torch.profiler
 in one fresh process (the `routes` fixture); the values are checked here.  Run with -s for the switch points, the routes
 seen and the worst errors per group."""
-import ctypes
 import json
-import os
-import subprocess
-import sys
-import tempfile
-import time
-from collections import Counter, defaultdict
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_l2
+from kernel_harness import WorstLog, dev, f64, make_params, ptr, scan_status, td_inputs
+from kernel_harness import nv_routes as nv  # noqa: F401
 from learner_harness import TOL, check_against_oracle, episode, oracle_for, port_case, step_err
 from oracle import actor_oracle
 from oracle import learner_oracle as lo
 from oracle import ref_port
 from oracle.sumtree import SumTreeOracle
-from route_check import ROUTE_KERNELS, RouteLog, ran, template_args
+from route_check import ROUTE_KERNELS, RouteLog, launch_counts, observe_in_fresh_process, ran, template_args
 
 pytestmark = pytest.mark.gpu
 
@@ -49,79 +44,20 @@ NATIVE = {"reference": 0, "invertible": 1, "squared": 0, "abs": 1}
 B_MAX = 1 << 14          # bisection ceiling in rows: far beyond the split-K switch of any product here
 
 ROUTES = RouteLog()
-WORST = defaultdict(float)
+WORST = WorstLog()
 
 
 @pytest.fixture(scope="module", autouse=True)
 def report():
     yield
-    print("\nworst errors per group:")
-    for g, e in sorted(WORST.items()):
-        print(f"  {g:34s} {e:.2e}")
+    WORST.report()
     ROUTES.report()
-
-
-@pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    lib = native.lib()
-    assert lib.r2d2_get_gemm_impl() == 1, "these routes are the default implementation's"
-    lib.r2d2_set_scan_impl(1)
-    return native
 
 
 @pytest.fixture(scope="module")
 def eng_mod():
     from r2d2_b200 import engine
     return engine
-
-
-def dev(a):
-    return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).cuda()
-
-
-def f64(a):
-    return np.asarray(a, np.float32).astype(np.float64)
-
-
-def ptr(t):
-    return None if t is None else t.data_ptr()
-
-
-def bound(group, name, x, ref, tol, time_axis=None, step_tol=None):
-    """rel_l2 < tol; with time_axis also the worst single time row: step_err < step_tol (default tol)."""
-    errs = {"rel_l2": (rel_l2(x, ref), tol)}
-    if time_axis is not None:
-        errs["step_err"] = (step_err(x, ref, time_axis), step_tol or tol)
-    for k, (e, _) in errs.items():
-        WORST[f"{group} {k}"] = max(WORST[f"{group} {k}"], e)
-    bad = {k: f"{e:.3e} (bound {t:.0e})" for k, (e, t) in errs.items() if not e < t}
-    assert not bad, f"{name}: {bad}"
-
-
-def scan_status(nv):
-    status = ctypes.c_int(0)
-    nv.check(nv.lib().r2d2_scan_status(ctypes.byref(status), nv.current_stream()))
-    return status.value
-
-
-def launch_counts(case, fn):
-    """{profiler name of a route kernel: launches} of fn under the CUDA profiler.  A session that recorded no route
-    kernel at all is repeated after a growing pause (RouteLog.profile), five sessions in all."""
-    from torch.autograd import DeviceType
-    from torch.profiler import ProfilerActivity, profile
-    for pause in (0.1, 0.3, 1.0, 3.0, None):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-        c = Counter(e.name for e in prof.events()
-                    if e.device_type == DeviceType.CUDA and any(b in e.name for b in ROUTE_KERNELS.values()))
-        if c or pause is None:
-            break
-        time.sleep(pause)
-    assert c, f"{case}: the profiler recorded no route kernel in five sessions"
-    return dict(c)
 
 
 def count(counts, key, args=None):
@@ -132,15 +68,6 @@ def count(counts, key, args=None):
 
 
 # ------------------------------------------------------------------------------------------------ 1. TD / priority
-def td_inputs(L, B, A, Bn, n, seed):
-    rng = np.random.default_rng(seed)
-    T = Bn + L + n
-    q, qn = rng.standard_normal((L, B, A)) * 2, rng.standard_normal((L, B, A)) * 5
-    rew = rng.standard_normal((T, B)) * 3
-    term = (rng.uniform(size=(T, B)) < 0.15).astype(np.float64)
-    return q, qn, rew, term
-
-
 def td_call(nv, inputs, L, B, A, Bn, n, want=("y", "dq", "td", "p", "loss"), w=None, opts=None, check=True):
     """r2d2_td_priority (w and opts None), _weighted (w given) or _ex (opts = (rescaling, eps, metric)) with the
     outputs in `want`, NULL for the others; requested outputs start as NaN.  Returns ({output: host array}, rc)."""
@@ -178,10 +105,10 @@ def check_td(group, case, o, ref, opts=None):
     for k, got, want, tol, ax in (("y", o.get("y"), y, tol_y, 0), ("dq", o.get("dq"), dq, 1e-5, 0),
                                   ("td", o.get("td"), td_sq, 1e-5, 0), ("p", o.get("p"), prio, 1e-5, None)):
         if got is not None:
-            bound(f"td {group} {k}", f"{case} {k}", got, want, tol, time_axis=ax, step_tol=1e-5)
+            WORST.bound(f"td {group} {k}", f"{case} {k}", got, want, tol, time_axis=ax, step_tol=1e-5)
     if "loss" in o:
         e = abs(o["loss"][0] / loss - 1.0)
-        WORST[f"td {group} loss"] = max(WORST[f"td {group} loss"], e)
+        WORST.note(f"td {group} loss", e)
         assert e < 1e-5, (case, o["loss"][0], loss)
 
 
@@ -251,15 +178,6 @@ def test_td_quirk_drops_the_last_element(nv, L, B, A):
 
 
 # ------------------------------------------------------------------------------------------------ nets
-def make_params(rng, O, A, H, critic):
-    I = O + (A if critic else 0)
-    u = lambda shp, b: rng.uniform(-b, b, shp).astype(np.float32)  # noqa: E731
-    return {"l1.weight": u((H, I), 1 / np.sqrt(I)), "l1.bias": u((H,), 0.2),
-            "l2.weight_ih": u((4 * H, H), 2 / np.sqrt(4 * H)), "l2.weight_hh": u((4 * H, H), 2 / np.sqrt(4 * H)),
-            "l2.bias_ih": u((4 * H,), 0.1), "l2.bias_hh": u((4 * H,), 0.1),
-            "l3.weight": u((A, H), 1 / np.sqrt(H)), "l3.bias": u((A,), 0.1)}
-
-
 class NetRun:
     """Device buffers of one r2d2_lstm_net_forward / _backward case (zero inputs without a seed); out and d_act start
     as NaN so that an unwritten element fails every bound."""
@@ -320,15 +238,15 @@ class NetRun:
         d_full = np.zeros_like(sv["out"])
         d_full[repeat - 1::repeat][fr:] = f64(self.d_out)
         g_ref, dx_ref, _ = lo.net_backward(p, sv, d_full, critic=critic, want_wgrad=True, want_dx=critic)
-        bound(f"{group} out", f"{case} out", self.out.cpu().numpy(), sv["out"][repeat - 1::repeat][fr:], tol_fwd,
+        WORST.bound(f"{group} out", f"{case} out", self.out.cpu().numpy(), sv["out"][repeat - 1::repeat][fr:], tol_fwd,
               time_axis=0)
         if critic:
-            bound(f"{group} d_act", f"{case} d_act", self.d_act.cpu().numpy(), dx_ref[:, :, self.O:], tol_bwd,
+            WORST.bound(f"{group} d_act", f"{case} d_act", self.d_act.cpu().numpy(), dx_ref[:, :, self.O:], tol_bwd,
                   time_axis=0)
         g, off = self.grads.cpu().numpy(), 0
         for k in lo.PARAM_KEYS:
             n = g_ref[k].size
-            bound(f"{group} grad", f"{case} grad {k}", g[off:off + n].reshape(g_ref[k].shape), g_ref[k], tol_bwd)
+            WORST.bound(f"{group} grad", f"{case} grad {k}", g[off:off + n].reshape(g_ref[k].shape), g_ref[k], tol_bwd)
             off += n
 
 
@@ -521,7 +439,7 @@ def test_learner_window(eng_mod, Bn, L, n, B):
             errs[f"oracle/{net}/{k}"] = rel_l2(mine[k], getattr(ol, net)[k])
             errs[f"port/{net}/{k}"] = rel_l2(mine[k], port_after[k])
     eng.close()
-    WORST["learner"] = max([WORST["learner"]] + list(errs.values()))
+    WORST.note("learner", *errs.values())
     bad = {k: f"{v:.2e}" for k, v in errs.items() if not v < TOL}
     assert not bad, bad
 
@@ -549,7 +467,7 @@ def test_replay_fed_learner_at_burn_in_zero(eng_mod):
         ref = ol.iteration(batch)
         torch.cuda.synchronize()
         errs = {k: rel_l2(getattr(eng, k).cpu().numpy(), ref[k]) for k in ("q_value", "target_q_value", "priority")}
-        WORST["learner replay-fed"] = max([WORST["learner replay-fed"]] + list(errs.values()))
+        WORST.note("learner replay-fed", *errs.values())
         assert all(v < TOL for v in errs.values()), (it, errs)
         rp.update_priorities(eng.leaf_idx, eng.priority)
     rp.close()
@@ -562,7 +480,7 @@ def test_twin_critic_at_burn_in_zero(eng_mod, L, n, B):
     kw = dict(obs=5, act=2, hidden=32, batch=B, burn_in=0, learning=L, n_step=n)
     actor, critic, batches = port_case(kw, seed=3, n_batches=2, batch_seed=40)
     worst = check_against_oracle(eng_mod, dict(kw, twin_critic=True), actor, critic, batches, 2)
-    WORST["learner twin"] = max(WORST["learner twin"], worst)
+    WORST.note("learner twin", worst)
 
 
 # ------------------------------------------------------------------------------------------------ 5. replay, actor side
@@ -661,14 +579,14 @@ def test_actor_side_windows(nv, Bn, L, n, rescaling, metric):
     rew_h, prio_h = rew.cpu().numpy(), prio.cpu().numpy()
     for b, N in enumerate(lens):
         want_r = actor_oracle.nstep_rewards(raw[:N, b], n, gamma)
-        bound("actor nstep", f"b={b} rewards", rew_h[:N, b], want_r, 1e-6, time_axis=0)
+        WORST.bound("actor nstep", f"b={b} rewards", rew_h[:N, b], want_r, 1e-6, time_axis=0)
         assert (rew_h[N:, b] == 0).all()
         want = actor_oracle.window_priorities(f64(q[:N - n, b]), f64(qt[:N, b]), f64(rew_h[:N, b]), f64(term[:N, b]),
                                               burn_in=Bn, learning=L, n_step=n, gamma=gamma, rescaling=rescaling,
                                               eps=float(np.float32(1e-2)), metric=metric)
         assert want.size == N - n - (Bn + L)
         if want.size:
-            bound("actor priority", f"b={b} priorities", prio_h[b, :want.size], want, 1e-5)
+            WORST.bound("actor priority", f"b={b} priorities", prio_h[b, :want.size], want, 1e-5)
         assert (prio_h[b, want.size:] == 0).all(), f"b={b}: padding past {want.size} starts is not 0"
 
 
@@ -698,10 +616,10 @@ def test_td_one_step_window_without_priority(nv, A, want):
     y = lo.n_step_target(rew[Bn:Bn + L, :, None], 0.997 ** n * (1.0 - term[Bn + n - 1:Bn + n - 1 + L, :, None]), qn)
     diff = q - y
     assert all(np.isfinite(v).all() for v in o.values())
-    bound("td L=1 y", "y", o["y"], y, 1e-6)
-    bound("td L=1 dq", "dq", o["dq"], 2.0 * diff / diff.size, 1e-5)
+    WORST.bound("td L=1 y", "y", o["y"], y, 1e-6)
+    WORST.bound("td L=1 dq", "dq", o["dq"], 2.0 * diff / diff.size, 1e-5)
     if "td" in o:
-        bound("td L=1 td_sq", "td_sq", o["td"], np.mean(diff * diff, axis=2), 1e-5)
+        WORST.bound("td L=1 td_sq", "td_sq", o["td"], np.mean(diff * diff, axis=2), 1e-5)
     assert abs(o["loss"][0] / np.mean(diff * diff) - 1.0) < 1e-5
 
 
@@ -755,16 +673,7 @@ def route_child(out_path):
 def routes(nv):
     """{case: {route kernel: launches}} and "wgrad_switch": {product: first T·B on thin_tn}, observed in a fresh Python
     process (route_child).  Prints the switch points."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "routes.json")
-        code = ("import sys; sys.path[:0] = %r; import test_gpu_sequence_geometry as t; t.route_child(%r)"
-                % ([here, root, os.path.join(root, "pytorch-r2d2-dpg_b200")], out))
-        res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=1200, cwd=root)
-        assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-        with open(out) as f:
-            got = json.load(f)
+    got = observe_in_fresh_process("test_gpu_sequence_geometry", timeout=1200)
     routes = dict(got["seen"])
     routes["wgrad_switch"] = got["switch"]
     print(f"\nroute process: {got['probes']} bisection probes")

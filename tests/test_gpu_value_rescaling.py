@@ -12,20 +12,20 @@ absolute-TD-error priorities, through the C ABI, the learner engine, the actor s
 import json
 import os
 import re
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import rel_l2
+from kernel_harness import dev, f64, nv, ptr  # noqa: F401
 from learner_harness import (SMALL, assert_pipelined_matches_sequential, assert_resumed_run_is_bit_identical,
                              assert_same_bits, check_against_oracle, col_err, golden_case, port_case, replay_fed_run,
                              snapshot, trained_dropin_learner)
 from oracle import actor_oracle
 from oracle import learner_oracle as lo
 from oracle import ref_port
+from route_check import observe, observe_in_fresh_process, recorded_sentinel
 
 pytestmark = pytest.mark.gpu
 
@@ -35,33 +35,15 @@ NEW = dict(value_rescaling="invertible", rescaling_eps=1e-3, priority_metric="ab
 
 
 @pytest.fixture(scope="module")
-def nv():
-    from r2d2_b200 import native
-    native.lib()
-    return native
-
-
-@pytest.fixture(scope="module")
 def eng_mod():
     from r2d2_b200 import engine
     return engine
 
 
-def dev(a):
-    return torch.as_tensor(np.ascontiguousarray(a, dtype=np.float32)).cuda()
-
-
-def f64(a):
-    return np.asarray(a, np.float32).astype(np.float64)
-
-
-def ptr(t):
-    return None if t is None else t.data_ptr()
-
-
 # ------------------------------------------------------------------------------------------------ helpers
 def td_inputs(L, B, A, Bn, n, seed):
-    """q' log-uniform in magnitude 1e-6 .. 1e4 with both signs and exact zeros; terminals anywhere."""
+    """q' log-uniform in magnitude 1e-6 .. 1e4 with both signs and exact zeros; terminals anywhere.  Not
+    kernel_harness.td_inputs: h_eps and its inverse are exercised over many decades of |q'|, not around 1."""
     rng = np.random.default_rng(seed)
     T = Bn + L + n
     qn = 10.0 ** rng.uniform(-6, 4, (L, B, A)) * rng.choice([-1.0, 1.0], (L, B, A))
@@ -122,43 +104,6 @@ def _flags(name, base):
     return tuple(int(x) for x in re.findall(r"Lb([01])E", m.group(1))) if m else None
 
 
-def _profiled_session(fn):
-    """fn() under torch.profiler, then a sentinel kernel of torch's own (a fill): (CUDA kernel names, whether the
-    sentinel was recorded)."""
-    from torch.autograd import DeviceType
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.empty(256, device="cuda").fill_(1.0)
-        torch.cuda.synchronize()
-    names = {e.name for e in prof.events() if e.device_type == DeviceType.CUDA}
-    return names, any("FillFunctor" in n for n in names)
-
-
-def observe_instantiations(fn, lost):
-    """The TD / actor-priority kernel instantiations fn launches, {base name: sorted [template flags]}, from one complete
-    torch.profiler session.  A session is complete when it recorded the sentinel; one without any kernel (torch.profiler
-    returns those now and then, sometimes several in a row) is repeated after a pause, eight sessions in all."""
-    import time
-    bases = ("td_elem_kernel", "td_reduce_kernel", "td_priority_column_kernel", "actor_priority_kernel")
-    for pause in (0.1, 0.3, 1.0, 2.0, 4.0, 8.0, 8.0, None):
-        names, complete = _profiled_session(fn)
-        if complete:
-            break
-        lost.append(1)
-        if pause is None:
-            return None
-        time.sleep(pause)
-    seen = {}
-    for n in names:
-        for b in bases:
-            f = _flags(n, b)
-            if f is not None:
-                seen.setdefault(b, set()).add(f)
-    return {k: sorted(list(f) for f in v) for k, v in seen.items()}
-
-
 def td_route_key(A, td_sq, weighted, rescaling, metric):
     return f"td/A={A}/td_sq={int(td_sq)}/w={int(weighted)}/{rescaling}/{metric}"
 
@@ -186,12 +131,21 @@ def _route_cases(nv):
 
 
 def route_child(out_path):
-    """Entry point of the fresh process behind the `routes` fixture: every case once under the profiler."""
+    """Entry point of the fresh process behind the `routes` fixture: every case once under the profiler, from a session
+    that recorded the sentinel -> {base name: sorted [template flags]} of the TD / actor-priority kernels, or None."""
     from r2d2_b200 import native
     native.lib()
+    bases = ("td_elem_kernel", "td_reduce_kernel", "td_priority_column_kernel", "actor_priority_kernel")
     lost, out = [], {}
     for key, fn in _route_cases(native).items():
-        out[key] = observe_instantiations(fn, lost)
+        got = observe(key, fn, recorded_sentinel, lost=lost)
+        seen = {}
+        for n in (got[1] if got else ()):
+            for b in bases:
+                f = _flags(n, b)
+                if f is not None:
+                    seen.setdefault(b, set()).add(f)
+        out[key] = None if got is None else {k: sorted(list(f) for f in v) for k, v in seen.items()}
     out["lost_sessions"] = len(lost)
     with open(out_path, "w") as f:
         json.dump(out, f)
@@ -203,17 +157,7 @@ def routes():
     collection in a long-lived test process can stop for several sessions in a row after the hundreds of sessions other
     test files run (seen on an H100 with torch 2.11 / CUDA 12.8, never in a fresh process), which says nothing about this
     library; a fresh process gives every case a complete session.  The values are checked in this process."""
-    import subprocess
-    here = os.path.dirname(os.path.abspath(__file__))
-    root = os.path.dirname(here)
-    with tempfile.TemporaryDirectory() as d:
-        out = os.path.join(d, "routes.json")
-        code = ("import sys; sys.path[:0] = %r; import test_gpu_value_rescaling as t; t.route_child(%r)"
-                % ([here, root, os.path.join(root, "pytorch-r2d2-dpg_b200")], out))
-        res = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, cwd=root)
-        assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
-        with open(out) as f:
-            got = json.load(f)
+    got = observe_in_fresh_process("test_gpu_value_rescaling", timeout=900)
     print(f"\nprofiler sessions repeated in the route process: {got.pop('lost_sessions')}")
     return got
 
